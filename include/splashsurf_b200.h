@@ -254,6 +254,28 @@ int ss_context_set_compute_sph_normals(ss_context *ctx, int on);
 int ss_surface_copy_normals(const ss_surface *s, float *dst_xyz);
 const float *ss_surface_device_normals(const ss_surface *s);
 
+/* ---- Anisotropic kernels (J. Yu and G. Turk, "Reconstructing Surfaces of Particle-Based Fluids Using Anisotropic Kernels", ACM TOG
+ * 32(1), 2013; specification in DESIGN.md section 11).  Every particle's kernel is centred at a smoothed position x_bar and
+ * stretched along the principal axes of its density neighbourhood (weighted PCA), so that flat fluid surfaces come out flat:
+ *     phi(x) = sum_j V_j det(G_j) W(|G_j (x - x_bar_j)|),   G_j = R diag(1 / s_k) R^T,  s_k = max(sigma_k, sigma_1 / max_stretch) / sigma_1
+ * `smoothing` (lambda, in [0, 1]) blends the particle position with the weighted mean of its neighbourhood; particles with fewer
+ * than `min_neighbors` neighbours keep the isotropic kernel.  The support never exceeds the isotropic ball of radius h.
+ * Opt-in per context (NULL = off, the default).  Densities, grid, marching cubes and stitching are unchanged (densities bit for bit).
+ * Subdomain path only: with spatial_decomposition = 0 the reconstruction returns SS_ERR_UNSUPPORTED, and the decomposition is always
+ * used (the auto-disable rule does not apply); ss_reconstruct_partition_f32 / _cb_f32 return SS_ERR_UNSUPPORTED.  SPH normals and the
+ * [bins] post-processing entries below keep the isotropic kernel at the particle positions. */
+typedef struct ss_anisotropy_f32 {
+    float smoothing;                     /* lambda, default 0.9 */
+    float max_stretch;                   /* k_r >= 1, default 4 */
+    uint32_t min_neighbors;              /* default 10 (neighbours without the particle itself) */
+} ss_anisotropy_f32;
+int ss_context_set_anisotropy_f32(ss_context *ctx, const ss_anisotropy_f32 *aniso /* NULL = off */);
+/* Parity tap: smoothed kernel centres x_bar (num_particles x 3) and G (num_particles x 6: g00 g01 g02 g11 g12 g22) of the filtered
+ * particles; either pointer may be NULL.  SS_ERR_INVALID_PARAMETER when the surface was not reconstructed in this mode. */
+int ss_surface_copy_anisotropy(const ss_surface *s, float *xbar, float *g);
+/* Device time of the anisotropy stage (weighted PCA per particle), ms; 0 without anisotropic kernels.  ss_timings.density excludes it. */
+float ss_surface_anisotropy_ms(const ss_surface *s);
+
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.
  * The entries marked [bins] query the particles through the splat bins of the reconstruction that produced the surface and

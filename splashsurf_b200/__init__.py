@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -71,6 +71,11 @@ class _Timings(C.Structure):
                 ("levelset_fixup_points", C.c_uint64), ("levelset_pairs", C.c_double),
                 ("bricks_total", C.c_uint64), ("bricks_levelset", C.c_uint64), ("bricks_mc", C.c_uint64), ("bricks_fixscan", C.c_uint64),
                 ("levelset_cert_evals", C.c_double), ("tile_setup", C.c_double)]
+
+
+class _Anisotropy(C.Structure):
+    """ss_anisotropy_f32 (include/splashsurf_b200.h)."""
+    _fields_ = [("smoothing", C.c_float), ("max_stretch", C.c_float), ("min_neighbors", C.c_uint32)]
 
 
 _LIB = None
@@ -177,6 +182,10 @@ def _bind(L):
                                     C.POINTER(_MeshAttribute), C.c_uint32, C.c_uint32]
     L.ss_format_f32.argtypes = [C.c_float, C.c_char_p, u64]
     L.ss_meshio_set_chunk_items.argtypes = [u64]
+    L.ss_context_set_anisotropy_f32.argtypes = [vp, C.POINTER(_Anisotropy)]
+    L.ss_surface_copy_anisotropy.argtypes = [vp, vp, vp]
+    L.ss_surface_anisotropy_ms.argtypes = [vp]
+    L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
         raise ImportError("libsplashsurf_b200.so ABI version mismatch")
     return L
@@ -575,6 +584,51 @@ class SurfaceReconstruction:
     subdomains: Optional[dict] = None
     levelset_tile: Optional[np.ndarray] = None
     normals: Optional[np.ndarray] = None       # (V, 3) unit SPH normals when requested
+    # with anisotropic kernels (``anisotropy=Anisotropy()``): kernel centres x_bar (N, 3) and matrices G (N, 3, 3) of the particles
+    smoothed_particles: Optional[np.ndarray] = None
+    anisotropy_matrices: Optional[np.ndarray] = None
+
+
+@dataclass(frozen=True)
+class Anisotropy:
+    """Anisotropic kernels after Yu & Turk (ACM TOG 32(1), 2013) for the level set; DESIGN.md section 11.
+
+    Every particle's kernel is centred at ``x_bar = x + smoothing * (weighted mean of its neighbourhood - x)`` and stretched along the
+    principal axes of the neighbourhood's weighted covariance: flat along a free surface, round inside the fluid.  ``max_stretch``
+    bounds the ratio of the longest to the shortest axis; particles with fewer than ``min_neighbors`` neighbours keep the isotropic
+    kernel.  The support never exceeds the isotropic one (radius h).  Densities, grid and marching cubes are unchanged; SPH normals
+    and attribute interpolation keep the isotropic kernel.  Requires ``subdomain_grid=True`` (always decomposed)."""
+    smoothing: float = 0.9
+    max_stretch: float = 4.0
+    min_neighbors: int = 10
+
+    def _abi(self) -> _Anisotropy:
+        if int(self.min_neighbors) < 0 or int(self.min_neighbors) > 0xffffffff:
+            raise ValueError("min_neighbors must be a non-negative 32-bit integer")
+        return _Anisotropy(float(np.float32(self.smoothing)), float(np.float32(self.max_stretch)), int(self.min_neighbors))
+
+
+def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Optional[Anisotropy]):
+    """ctx.reconstruct_raw with the context's anisotropy set for this one call (and reset whatever happens)."""
+    L = ctx._L
+    _check(L, L.ss_context_set_anisotropy_f32(ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
+    try:
+        return ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
+    finally:
+        if anisotropy is not None:
+            L.ss_context_set_anisotropy_f32(ctx._h, None)
+
+
+def _collect_anisotropy(ctx: "Context", s, res: "SurfaceReconstruction"):
+    L = ctx._L
+    n = len(res.particle_densities)
+    xbar, g = np.empty((n, 3), np.float32), np.empty((n, 6), np.float32)
+    if n:
+        _check(L, L.ss_surface_copy_anisotropy(s, xbar.ctypes.data, g.ctypes.data))
+    res.smoothed_particles = xbar
+    res.anisotropy_matrices = np.ascontiguousarray(g[:, [0, 1, 2, 1, 3, 4, 2, 4, 5]].reshape(n, 3, 3))
+    if res.timings is not None:
+        res.timings["anisotropy"] = float(L.ss_surface_anisotropy_ms(s))
 
 
 # ---------------------------------------------------------------------------- context ----
@@ -944,12 +998,14 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                         multi_threading: bool = True, simd: bool = True, global_neighborhood_list: bool = False,
                         subdomain_grid: bool = True, subdomain_grid_auto_disable: bool = True,
                         subdomain_num_cubes_per_dim: int = 64, context: Optional[Context] = None,
-                        keep_levelset_tile_of: Optional[int] = None, with_debug: bool = False, sph_normals: bool = False) -> SurfaceReconstruction:
+                        keep_levelset_tile_of: Optional[int] = None, with_debug: bool = False, sph_normals: bool = False,
+                        anisotropy: Optional[Anisotropy] = None) -> SurfaceReconstruction:
     """Performs a surface reconstruction from the given particles (no post-processing) on the GPU.
 
     Same signature and semantics as ``pysplashsurf.reconstruct_surface``; ``particles`` is an (N, 3) float32
     array (float64 input is not provided by the device path and raises, like an unsupported dtype does in the
-    reference, pysplashsurf/src/reconstruction.rs:204-206).
+    reference, pysplashsurf/src/reconstruction.rs:204-206).  ``anisotropy=Anisotropy(...)`` switches the level set to anisotropic
+    kernels (not part of the reference; see ``Anisotropy``).
     """
     arr = np.asarray(particles)
     if arr.dtype != np.float32:
@@ -966,9 +1022,11 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1 if keep_levelset_tile_of is None else int(keep_levelset_tile_of)))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, int(bool(sph_normals))))
-    s = ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy)
     try:
         res = _collect(ctx, s, len(arr), p, with_debug or keep_levelset_tile_of is not None, keep_levelset_tile_of is not None)
+        if anisotropy is not None:
+            _collect_anisotropy(ctx, s, res)
         if sph_normals:
             nrm = np.empty((res.mesh.nvertices, 3), dtype=np.float32)
             if len(nrm):
@@ -1181,7 +1239,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                             mesh_smoothing_iters: Optional[int] = None, mesh_smoothing_weights: bool = True,
                             mesh_smoothing_weights_normalization: float = 13.0, output_mesh_smoothing_weights: bool = False,
                             output_raw_normals: bool = False, output_raw_mesh: bool = False, context: Optional[Context] = None,
-                            with_debug: bool = False, **post):
+                            with_debug: bool = False, anisotropy: Optional[Anisotropy] = None, **post):
     """``pysplashsurf.reconstruction_pipeline`` (pysplashsurf/src/pipeline.rs:109-200) on the GPU: surface reconstruction plus
     the post-processing steps of splashsurf/src/reconstruct.rs:1094-1391 that run on the device -- smoothing weights, weighted
     Laplacian smoothing, SPH or area-weighted normals (at the smoothed vertices), normal smoothing and SPH interpolation of
@@ -1193,7 +1251,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     ``quad_max_edge_diag_ratio`` / ``quad_max_normal_angle`` / ``quad_max_interior_angle``) runs last (reconstruct.rs:1410-1441, host):
     the returned mesh is then a MixedTriQuadMesh3d.  ``mesh_aabb_min`` / ``mesh_aabb_max`` (+ ``mesh_aabb_clamp_vertices``) clamp the
     finished mesh (reconstruct.rs:1394-1408) and ``check_mesh_closed`` / ``check_mesh_manifold`` raise SplashsurfError with the
-    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541)."""
+    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy`` as in
+    ``reconstruct_surface``."""
     passive = ("mesh_cleanup", "decimate_barnacles", "mesh_cleanup_snap_dist", "keep_vertices", "generate_quads", "quad_max_edge_diag_ratio",
                "quad_max_normal_angle", "quad_max_interior_angle", "mesh_aabb_min", "mesh_aabb_max", "mesh_aabb_clamp_vertices",
                "check_mesh_closed", "check_mesh_manifold", "check_mesh_orientation", "check_mesh_debug")
@@ -1222,9 +1281,11 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, 0))
-    s = ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy)
     try:
         rec = _collect(ctx, s, len(arr), p, with_debug, False)                  # raw mesh, densities, grids
+        if anisotropy is not None:
+            _collect_anisotropy(ctx, s, rec)
         out_mesh = rec.mesh
         if mesh_cleanup or decimate_barnacles:                                  # reconstruct.rs:1058-1092
             out_mesh = rec.mesh.copy()

@@ -111,6 +111,11 @@ def main(argv=None):
     r.add_argument("--device", type=int, default=None)                               # CUDA device of this process (default: LOCAL_RANK or 0)
     r.add_argument("--partition", choices=["on", "off"], default="off")              # under a multi-process launcher: ONE frame over all GPUs (slab partition)
     r.add_argument("--shard", default=None, metavar="I/N")                           # this process takes frames I, I + N, ... (default: RANK / WORLD_SIZE)
+    # anisotropic kernels (Yu & Turk 2013; splashsurf_b200.Anisotropy, DESIGN.md section 11) -- not part of the reference CLI
+    r.add_argument("--anisotropic", choices=["on", "off"], default="off")
+    r.add_argument("--aniso-smoothing", type=float, default=0.9)                      # kernel-centre smoothing lambda in [0, 1]
+    r.add_argument("--aniso-max-stretch", type=float, default=4.0)                    # longest / shortest kernel axis, >= 1
+    r.add_argument("--aniso-min-neighbors", type=int, default=10)                     # fewer neighbours: isotropic kernel
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -247,6 +252,10 @@ def reconstruct(a) -> int:
     on = lambda v: str(v).lower() == "on"         # noqa: E731
     if on(a.double_precision):
         raise ValueError("--double-precision=on: the device path reconstructs float32 particles only (SURVEY.md 8b)")
+    if on(a.partition) and on(a.anisotropic):
+        raise ValueError("--anisotropic=on is not available with --partition=on: anisotropic kernels run on one GPU per frame")
+    from . import Anisotropy
+    aniso = Anisotropy(a.aniso_smoothing, a.aniso_max_stretch, a.aniso_min_neighbors) if on(a.anisotropic) else None
     paths = collect_paths(a)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)
@@ -292,10 +301,10 @@ def reconstruct(a) -> int:
                     keep_vertices=on(a.keep_verts), generate_quads=on(a.generate_quads), quad_max_edge_diag_ratio=a.quad_max_edge_diag_ratio,
                     quad_max_normal_angle=a.quad_max_normal_angle, quad_max_interior_angle=a.quad_max_interior_angle, mesh_aabb_min=mmin,
                     mesh_aabb_max=mmax, mesh_aabb_clamp_vertices=on(a.mesh_aabb_clamp_verts), check_mesh_closed=closed, check_mesh_manifold=manifold,
-                    check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, **base)
+                    check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso, **base)
                 raw = rec.mesh
             else:
-                raw = reconstruct_surface(p, context=ctx, **base).mesh
+                raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, **base).mesh
                 out = MeshWithData(raw, {}, {})
             dt = time.perf_counter() - t
             quads = out.mesh.get_quads() if on(a.generate_quads) else None

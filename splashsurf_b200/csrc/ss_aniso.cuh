@@ -1,0 +1,364 @@
+// ss_aniso.cuh -- anisotropic-kernel level set (J. Yu and G. Turk, "Reconstructing Surfaces of Particle-Based Fluids Using
+// Anisotropic Kernels", ACM TOG 32(1), 2013), the opt-in mode of ss_context_set_anisotropy_f32.  DESIGN.md §11 is the
+// specification; tests/anisotropic_oracle.c restates it in plain C in the same operation order, so results are bit-exact.
+//
+//   k_aniso_init        x_bar = x, G = I, det G = 1 for every particle (particles without an owning subdomain keep these)
+//   k_aniso             per particle in its owning subdomain: weighted mean and covariance of its density neighbourhood (the
+//                       density stage's walk, ss_nbr_walk), cyclic Jacobi, clamped stretch -> x_bar, G (6 entries), det G
+//   k_records_aniso     splat records (x_bar, V det G) + the G entries of every binned membership
+//   k_aniso_levelset    warp per 8^3-point brick over the non-empty-brick work list: candidates of the brick's bins sorted by
+//                       particle index, per 4x4x4 sub-box the candidates within h of the sub-box, two grid points per lane;
+//                       bricks with more candidates than the slice go to a 4096-slot instantiation, beyond that to
+//                       k_aniso_select (O(C^2) selection in index order)
+// Every value the level set writes is exact; there is no certification in this mode.
+#pragma once
+
+#define SS_AN_SWEEPS 8                  // cyclic Jacobi sweeps (pivots (0,1), (0,2), (1,2))
+#define SS_AN_WARPS 4                   // bricks per CTA of the default slice
+#define SS_AN_CAP 512                   // candidates staged per brick (default slice)
+#define SS_AN_BIG_CAP 4096              // one warp per CTA: 40 KB of static shared memory
+
+// ------------------------------------------------------------------ per-particle anisotropy ----
+__global__ void k_aniso_init(const float *__restrict__ xyz, uint32_t n, float *__restrict__ xbar, float *__restrict__ gmat, float *__restrict__ gdet) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    for (int d = 0; d < 3; ++d) xbar[3 * (uint64_t)p + d] = xyz[3 * (uint64_t)p + d];
+    const float id[6] = { 1.0f, 0.0f, 0.0f, 1.0f, 0.0f, 1.0f };
+    for (int q = 0; q < 6; ++q) gmat[6 * (uint64_t)p + q] = id[q];
+    gdet[p] = 1.0f;
+}
+
+// One Jacobi rotation of the symmetric 3x3 matrix a (and the accumulated eigenvectors v, columns) that zeroes a[p][q];
+// skipped when a[p][q] is exactly 0.  Classic formulas: theta = (a_qq - a_pp) / (2 a_pq), t = sgn(theta) / (|theta| +
+// sqrt(theta^2 + 1)), c = 1 / sqrt(t^2 + 1), s = t c.
+template <int p, int q>
+__device__ __forceinline__ void ss_jacobi_rot(float (&a)[3][3], float (&v)[3][3]) {
+    constexpr int r = 3 - p - q;
+    const float apq = a[p][q];
+    if (apq == 0.0f) return;
+    const float theta = __fdiv_rn(__fsub_rn(a[q][q], a[p][p]), __fmul_rn(2.0f, apq));
+    float t = __fdiv_rn(1.0f, __fadd_rn(fabsf(theta), __fsqrt_rn(__fadd_rn(__fmul_rn(theta, theta), 1.0f))));
+    if (theta < 0.0f) t = -t;
+    const float c = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(__fmul_rn(t, t), 1.0f)));
+    const float s = __fmul_rn(t, c);
+    const float app = __fsub_rn(a[p][p], __fmul_rn(t, apq)), aqq = __fadd_rn(a[q][q], __fmul_rn(t, apq));
+    const float arp = __fsub_rn(__fmul_rn(c, a[r][p]), __fmul_rn(s, a[r][q]));
+    const float arq = __fadd_rn(__fmul_rn(s, a[r][p]), __fmul_rn(c, a[r][q]));
+    a[p][p] = app; a[q][q] = aqq; a[p][q] = 0.0f; a[q][p] = 0.0f;
+    a[r][p] = arp; a[p][r] = arp; a[r][q] = arq; a[q][r] = arq;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float vkp = v[k][p], vkq = v[k][q];
+        v[k][p] = __fsub_rn(__fmul_rn(c, vkp), __fmul_rn(s, vkq));
+        v[k][q] = __fadd_rn(__fmul_rn(s, vkp), __fmul_rn(c, vkq));
+    }
+}
+
+// G (g00, g01, g02, g11, g12, g22) and det G of a covariance matrix (DESIGN.md §11).
+__device__ __forceinline__ void ss_aniso_matrix(const SsDev &P, float (&a)[3][3], uint32_t nn, float g[6], float &det) {
+    float v[3][3] = { { 1.0f, 0.0f, 0.0f }, { 0.0f, 1.0f, 0.0f }, { 0.0f, 0.0f, 1.0f } };
+#pragma unroll
+    for (int sweep = 0; sweep < SS_AN_SWEEPS; ++sweep) {
+        ss_jacobi_rot<0, 1>(a, v);
+        ss_jacobi_rot<0, 2>(a, v);
+        ss_jacobi_rot<1, 2>(a, v);
+    }
+    float e[3] = { a[0][0], a[1][1], a[2][2] };
+    int ord[3] = { 0, 1, 2 };
+    // descending, stable: compare-exchange (0,1), (1,2), (0,1)
+#define SS_AN_CX(i, j) if (e[i] < e[j]) { const float te = e[i]; e[i] = e[j]; e[j] = te; const int to = ord[i]; ord[i] = ord[j]; ord[j] = to; }
+    SS_AN_CX(0, 1) SS_AN_CX(1, 2) SS_AN_CX(0, 1)
+#undef SS_AN_CX
+#pragma unroll
+    for (int k = 0; k < 3; ++k) e[k] = e[k] < 0.0f ? 0.0f : e[k];
+    if (nn < P.an_min_nb || e[0] == 0.0f) {
+        g[0] = 1.0f; g[1] = 0.0f; g[2] = 0.0f; g[3] = 1.0f; g[4] = 0.0f; g[5] = 1.0f; det = 1.0f;
+        return;
+    }
+    const float floor_s = __fdiv_rn(e[0], P.an_kr);
+    float inv[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) inv[k] = __fdiv_rn(1.0f, __fdiv_rn(fmaxf(e[k], floor_s), e[0]));
+    det = __fmul_rn(__fmul_rn(inv[0], inv[1]), inv[2]);
+    float R[3][3];                                  // R[row][k] = component `row` of the k-th eigenvector (descending)
+#pragma unroll
+    for (int row = 0; row < 3; ++row) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) R[row][k] = ord[k] == 0 ? v[row][0] : (ord[k] == 1 ? v[row][1] : v[row][2]);
+    }
+    const int ia[6] = { 0, 0, 0, 1, 1, 2 }, ib[6] = { 0, 1, 2, 1, 2, 2 };
+#pragma unroll
+    for (int q = 0; q < 6; ++q) {
+        float acc = __fmul_rn(__fmul_rn(R[ia[q]][0], inv[0]), R[ib[q]][0]);
+        acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(R[ia[q]][1], inv[1]), R[ib[q]][1]));
+        acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(R[ia[q]][2], inv[2]), R[ib[q]][2]));
+        g[q] = acc;
+    }
+}
+
+// One thread per particle inside its subdomain (the density stage's compacted list).
+__global__ void __launch_bounds__(128)
+k_aniso(SsDev P, uint32_t m, const uint32_t *__restrict__ list, const uint32_t *__restrict__ list_off, const uint32_t *__restrict__ list_flag,
+        const uint32_t *__restrict__ key, const float4 *__restrict__ spos, const uint32_t *__restrict__ sub_flat,
+        const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend, float *__restrict__ xbar, float *__restrict__ gmat,
+        float *__restrict__ gdet) {
+    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= list_off[m - 1] + list_flag[m - 1]) return;
+    const uint32_t e = list[tid];
+    const float4 pi = spos[e];
+    const uint32_t p = __float_as_uint(pi.w);
+    // weighted mean of the offsets x_j - x_i (self: w = 1, offset 0)
+    float sw = 1.0f, mx = 0.0f, my = 0.0f, mz = 0.0f;
+    uint32_t nn = 0;
+    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &, float dx, float dy, float dz, float d2) {
+        const float q = __fdiv_rn(__fsqrt_rn(d2), P.h);
+        const float w = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(q, q), q));
+        sw = __fadd_rn(sw, w);
+        mx = __fadd_rn(mx, __fmul_rn(w, dx)); my = __fadd_rn(my, __fmul_rn(w, dy)); mz = __fadd_rn(mz, __fmul_rn(w, dz));
+        ++nn;
+    });
+    const float ux = __fdiv_rn(mx, sw), uy = __fdiv_rn(my, sw), uz = __fdiv_rn(mz, sw);
+    // weighted covariance about the mean, self term first
+    float c00, c01, c02, c11, c12, c22;
+    {
+        const float ex = __fsub_rn(0.0f, ux), ey = __fsub_rn(0.0f, uy), ez = __fsub_rn(0.0f, uz);
+        c00 = __fmul_rn(ex, ex); c01 = __fmul_rn(ex, ey); c02 = __fmul_rn(ex, ez);
+        c11 = __fmul_rn(ey, ey); c12 = __fmul_rn(ey, ez); c22 = __fmul_rn(ez, ez);
+    }
+    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &, float dx, float dy, float dz, float d2) {
+        const float q = __fdiv_rn(__fsqrt_rn(d2), P.h);
+        const float w = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(q, q), q));
+        const float ex = __fsub_rn(dx, ux), ey = __fsub_rn(dy, uy), ez = __fsub_rn(dz, uz);
+        const float wx = __fmul_rn(w, ex), wy = __fmul_rn(w, ey), wz = __fmul_rn(w, ez);
+        c00 = __fadd_rn(c00, __fmul_rn(wx, ex)); c01 = __fadd_rn(c01, __fmul_rn(wx, ey)); c02 = __fadd_rn(c02, __fmul_rn(wx, ez));
+        c11 = __fadd_rn(c11, __fmul_rn(wy, ey)); c12 = __fadd_rn(c12, __fmul_rn(wy, ez)); c22 = __fadd_rn(c22, __fmul_rn(wz, ez));
+    });
+    c00 = __fdiv_rn(c00, sw); c01 = __fdiv_rn(c01, sw); c02 = __fdiv_rn(c02, sw);
+    c11 = __fdiv_rn(c11, sw); c12 = __fdiv_rn(c12, sw); c22 = __fdiv_rn(c22, sw);
+    float a[3][3] = { { c00, c01, c02 }, { c01, c11, c12 }, { c02, c12, c22 } };
+    float g[6], det;
+    ss_aniso_matrix(P, a, nn, g, det);
+    xbar[3 * (uint64_t)p] = __fadd_rn(pi.x, __fmul_rn(P.an_lambda, ux));
+    xbar[3 * (uint64_t)p + 1] = __fadd_rn(pi.y, __fmul_rn(P.an_lambda, uy));
+    xbar[3 * (uint64_t)p + 2] = __fadd_rn(pi.z, __fmul_rn(P.an_lambda, uz));
+#pragma unroll
+    for (int q = 0; q < 6; ++q) gmat[6 * (uint64_t)p + q] = g[q];
+    gdet[p] = det;
+}
+
+// After k_records ran on the smoothed centres: rec.w = V det G, grec = (g00, g01, g02, g11), (g12, g22, 0, 0) per membership.
+__global__ void k_records_aniso(uint32_t m, const uint32_t *__restrict__ key, const uint32_t *__restrict__ pidx, const float *__restrict__ gmat,
+                                const float *__restrict__ gdet, float4 *__restrict__ rec, float4 *__restrict__ grec) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m || key[e] == 0xffffffffu) return;
+    const uint32_t p = pidx[e];
+    const float *g = gmat + 6 * (uint64_t)p;
+    rec[e].w = __fmul_rn(rec[e].w, gdet[p]);
+    grec[2 * (uint64_t)e] = make_float4(g[0], g[1], g[2], g[3]);
+    grec[2 * (uint64_t)e + 1] = make_float4(g[4], g[5], 0.0f, 0.0f);
+}
+
+// ------------------------------------------------------------------ level set ----
+struct SsAnArgs {
+    const uint32_t *bin_start, *bin_end;
+    const float4 *rec;                 // (x_bar, V det G), bin-sorted
+    const float4 *grec;                // two per record: (g00, g01, g02, g11), (g12, g22, -, -)
+    const uint32_t *pidx;              // bin-sorted particle indices
+    const SsTile *tile_tab;
+    const int2 *brick_rng;
+    const uint32_t *bricks;            // listed bricks (linear index)
+    uint32_t n_bricks;
+    float *tiles;
+    uint8_t *bstate;                   // set to 2 (exact values) by the first launch over the work list; NULL in fallback launches
+    uint32_t *fallback;                // bricks left to the next stage: [0] = count, [1..] = linear brick indices
+};
+
+// One term of phi(x) = sum_j V_j det G_j W(|G_j (x - x_bar_j)|), counted when |G_j (x - x_bar_j)|^2 < h^2.
+__device__ __forceinline__ float ss_aniso_term(const SsDev &P, const float4 r, const float4 g0, const float4 g1, float gx, float gy, float gz, float phi) {
+    const float dx = __fsub_rn(r.x, gx), dy = __fsub_rn(r.y, gy), dz = __fsub_rn(r.z, gz);
+    const float u0 = __fadd_rn(__fadd_rn(__fmul_rn(g0.x, dx), __fmul_rn(g0.y, dy)), __fmul_rn(g0.z, dz));
+    const float u1 = __fadd_rn(__fadd_rn(__fmul_rn(g0.y, dx), __fmul_rn(g0.w, dy)), __fmul_rn(g1.x, dz));
+    const float u2 = __fadd_rn(__fadd_rn(__fmul_rn(g0.z, dx), __fmul_rn(g1.x, dy)), __fmul_rn(g1.y, dz));
+    const float uu = __fadd_rn(__fadd_rn(__fmul_rn(u0, u0), __fmul_rn(u1, u1)), __fmul_rn(u2, u2));
+    return uu < P.h2 ? __fadd_rn(phi, __fmul_rn(r.w, ss_kernel_scalar(P, __fsqrt_rn(uu)))) : phi;
+}
+
+struct SsAnBrick { int bx, by, bz, tile; int2 rx, ry, rz; int nyr, nruns; SsTile T; };
+__device__ __forceinline__ SsAnBrick ss_an_brick(const SsDev &P, const SsAnArgs &A, uint32_t brick_lin) {
+    SsAnBrick B;
+    uint32_t q = brick_lin;
+    const uint32_t nb = (uint32_t)P.nb;
+    B.bz = (int)(q % nb); q /= nb;
+    B.by = (int)(q % nb); q /= nb;
+    B.bx = (int)(q % nb); B.tile = (int)(q / nb);
+    B.T = A.tile_tab[B.tile];
+    B.rx = A.brick_rng[B.bx]; B.ry = A.brick_rng[B.by]; B.rz = A.brick_rng[B.bz];
+    B.nyr = B.ry.y - B.ry.x + 1;
+    B.nruns = (B.rx.y - B.rx.x + 1) * B.nyr;
+    return B;
+}
+// candidate run r of the brick: bins (X, Y, rz.x .. rz.y), contiguous in key order
+__device__ __forceinline__ uint32_t ss_an_run(const SsDev &P, const SsAnArgs &A, const SsAnBrick &B, int r, uint32_t &start) {
+    start = 0;
+    if (r >= B.nruns) return 0;
+    const int X = B.rx.x + r / B.nyr, Y = B.ry.x + r % B.nyr;
+    uint32_t a = 0xffffffffu, b = 0;
+    const uint32_t base = B.T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
+    for (int Z = B.rz.x; Z <= B.rz.y; ++Z) {
+        const uint32_t st = A.bin_start[base + Z];
+        if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
+    }
+    if (a == 0xffffffffu) return 0;
+    start = a;
+    return b - a;
+}
+
+// lane -> its two grid points (k, k + 1) of a 4x4x4 sub-box
+#define SS_AN_LANE_IJK(lane, li, lj, lk) const int li = (lane) >> 3, lj = ((lane) >> 1) & 3, lk = ((lane) & 1) * 2
+
+template <int CAP>
+__device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A, unsigned long long *s_key, uint16_t *s_list, uint32_t work, int lane) {
+    const uint32_t brick_lin = A.bricks[work];
+    const SsAnBrick B = ss_an_brick(P, A, brick_lin);
+    if (A.bstate && lane == 0) A.bstate[brick_lin] = 2;
+    uint32_t C = 0;
+    for (int r0 = 0; r0 < B.nruns; r0 += 32) {
+        uint32_t a;
+        uint32_t len = ss_an_run(P, A, B, r0 + lane, a);
+        for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
+        C += len;
+    }
+    if (C == 0) return;                                      // pre-zeroed tile: phi = 0 exactly
+    if (C > (uint32_t)CAP) {
+        if (lane == 0) A.fallback[1 + atomicAdd(&A.fallback[0], 1u)] = brick_lin;
+        return;
+    }
+    // ---- stage the sort keys (particle index << 32 | record index), run by run
+    uint32_t dst0 = 0;
+    for (int r0 = 0; r0 < B.nruns; r0 += 32) {
+        uint32_t a;
+        const uint32_t len = ss_an_run(P, A, B, r0 + lane, a);
+        uint32_t incl = len;
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        const uint32_t dst = dst0 + incl - len;
+        const int nr = min(32, B.nruns - r0);
+        for (int rr = 0; rr < nr; ++rr) {
+            const uint32_t ra = __shfl_sync(0xffffffffu, a, rr), rl = __shfl_sync(0xffffffffu, len, rr), rd = __shfl_sync(0xffffffffu, dst, rr);
+            for (uint32_t t = lane; t < rl; t += 32) s_key[rd + t] = ((unsigned long long)A.pidx[ra + t] << 32) | (unsigned long long)(ra + t);
+        }
+        dst0 += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    int npow = 32;
+    while (npow < (int)C) npow <<= 1;
+    for (int t = (int)C + lane; t < npow; t += 32) s_key[t] = ~0ull;
+    __syncwarp();
+    ss_warp_bitonic(s_key, npow, lane);
+    __syncwarp();
+
+    const int pmax = P.np - 1;
+    float *const tile = A.tiles + (size_t)B.tile * P.np * P.np * P.np;
+    SS_AN_LANE_IJK(lane, li, lj, lk);
+    const float cull2 = P.h2 * 1.0001f;
+    for (int b = 0; b < 8; ++b) {
+        const int i0 = B.bx * 8 + 4 * ((b >> 2) & 1), j0 = B.by * 8 + 4 * ((b >> 1) & 1), k0 = B.bz * 8 + 4 * (b & 1);
+        if (i0 > pmax || j0 > pmax || k0 > pmax) continue;
+        const int i = i0 + li, j = j0 + lj, k = k0 + lk;
+        const int gi = B.T.gbase[0] + i, gj = B.T.gbase[1] + j, gk = B.T.gbase[2] + k;
+        // grid point coordinates: point_coordinates (uniform_grid.rs:418-425), min + index * cell
+        const float gx = __fadd_rn(P.gmin[0], __fmul_rn((float)gi, P.c)), gy = __fadd_rn(P.gmin[1], __fmul_rn((float)gj, P.c));
+        const float gzA = __fadd_rn(P.gmin[2], __fmul_rn((float)gk, P.c)), gzB = __fadd_rn(P.gmin[2], __fmul_rn((float)(gk + 1), P.c));
+        // sub-box in world coordinates (culling only: |G d| >= |d| because every eigenvalue of G is >= 1)
+        const int i1 = min(i0 + 3, pmax), j1 = min(j0 + 3, pmax), k1 = min(k0 + 3, pmax);
+        const float bxl = fmaf((float)(B.T.gbase[0] + i0), P.c, P.gmin[0]), bxh = fmaf((float)(B.T.gbase[0] + i1), P.c, P.gmin[0]);
+        const float byl = fmaf((float)(B.T.gbase[1] + j0), P.c, P.gmin[1]), byh = fmaf((float)(B.T.gbase[1] + j1), P.c, P.gmin[1]);
+        const float bzl = fmaf((float)(B.T.gbase[2] + k0), P.c, P.gmin[2]), bzh = fmaf((float)(B.T.gbase[2] + k1), P.c, P.gmin[2]);
+        int nlist = 0;
+        for (int w = 0; w < (int)((C + 31) >> 5); ++w) {
+            const int rnk = w * 32 + lane;
+            bool keep = false;
+            if (rnk < (int)C) {
+                const float4 r = A.rec[(uint32_t)s_key[rnk]];
+                keep = ss_axis_d2(r.x, bxl, bxh) + ss_axis_d2(r.y, byl, byh) + ss_axis_d2(r.z, bzl, bzh) < cull2;
+            }
+            const uint32_t mword = __ballot_sync(0xffffffffu, keep);
+            if (keep) s_list[nlist + __popc(mword & ((1u << lane) - 1u))] = (uint16_t)rnk;
+            nlist += __popc(mword);
+        }
+        __syncwarp();
+        float phiA = 0.0f, phiB = 0.0f;
+        for (int n = 0; n < nlist; ++n) {
+            const uint32_t src = (uint32_t)s_key[s_list[n]];
+            const float4 r = A.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
+            phiA = ss_aniso_term(P, r, g0, g1, gx, gy, gzA, phiA);
+            phiB = ss_aniso_term(P, r, g0, g1, gx, gy, gzB, phiB);
+        }
+        if (i <= pmax && j <= pmax) {
+            if (k <= pmax) tile[((size_t)i * P.np + j) * P.np + k] = phiA;
+            if (k + 1 <= pmax) tile[((size_t)i * P.np + j) * P.np + k + 1] = phiB;
+        }
+        __syncwarp();                                        // the list is rebuilt for the next sub-box
+    }
+}
+
+template <int CAP, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
+k_aniso_levelset(SsDev P, SsAnArgs A) {
+    __shared__ unsigned long long s_key[WARPS][CAP];
+    __shared__ uint16_t s_list[WARPS][CAP];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t work = blockIdx.x * WARPS + wib;
+    if (work >= A.n_bricks) return;
+    ss_aniso_brick<CAP>(P, A, s_key[wib], s_list[wib], work, lane);
+}
+
+// Bricks with more candidates than the largest slice (extreme clustering): one warp per brick walks the candidates in
+// ascending particle index by repeated selection of the next key, O(C^2 / 32), and folds each into its 16 grid points.
+__global__ void __launch_bounds__(32)
+k_aniso_select(SsDev P, SsAnArgs A) {
+    if (blockIdx.x >= A.n_bricks) return;
+    const int lane = threadIdx.x & 31;
+    const SsAnBrick B = ss_an_brick(P, A, A.bricks[blockIdx.x]);
+    const int pmax = P.np - 1;
+    SS_AN_LANE_IJK(lane, li, lj, lk);
+    float phi[16];
+#pragma unroll
+    for (int q = 0; q < 16; ++q) phi[q] = 0.0f;
+    unsigned long long last = 0;
+    bool first = true;
+    for (;;) {
+        unsigned long long best = ~0ull;
+        for (int X = B.rx.x; X <= B.rx.y; ++X) for (int Y = B.ry.x; Y <= B.ry.y; ++Y) {
+            const uint32_t base = B.T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
+            for (int Z = B.rz.x; Z <= B.rz.y; ++Z) {
+                const uint32_t st = A.bin_start[base + Z];
+                if (st == 0xffffffffu) continue;
+                const uint32_t en = A.bin_end[base + Z];
+                for (uint32_t t = st + lane; t < en; t += 32) {
+                    const unsigned long long kk = ((unsigned long long)A.pidx[t] << 32) | (unsigned long long)t;
+                    if ((first || kk > last) && kk < best) best = kk;
+                }
+            }
+        }
+        for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
+        if (best == ~0ull) break;
+        last = best; first = false;
+        const uint32_t src = (uint32_t)best;
+        const float4 r = A.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+            const int gi = B.T.gbase[0] + B.bx * 8 + 4 * ((b >> 2) & 1) + li, gj = B.T.gbase[1] + B.by * 8 + 4 * ((b >> 1) & 1) + lj;
+            const int gk = B.T.gbase[2] + B.bz * 8 + 4 * (b & 1) + lk;
+            const float gx = __fadd_rn(P.gmin[0], __fmul_rn((float)gi, P.c)), gy = __fadd_rn(P.gmin[1], __fmul_rn((float)gj, P.c));
+            phi[2 * b] = ss_aniso_term(P, r, g0, g1, gx, gy, __fadd_rn(P.gmin[2], __fmul_rn((float)gk, P.c)), phi[2 * b]);
+            phi[2 * b + 1] = ss_aniso_term(P, r, g0, g1, gx, gy, __fadd_rn(P.gmin[2], __fmul_rn((float)(gk + 1), P.c)), phi[2 * b + 1]);
+        }
+    }
+    float *const tile = A.tiles + (size_t)B.tile * P.np * P.np * P.np;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) {
+        const int i = B.bx * 8 + 4 * ((b >> 2) & 1) + li, j = B.by * 8 + 4 * ((b >> 1) & 1) + lj, k = B.bz * 8 + 4 * (b & 1) + lk;
+        if (i > pmax || j > pmax) continue;
+        if (k <= pmax) tile[((size_t)i * P.np + j) * P.np + k] = phi[2 * b];
+        if (k + 1 <= pmax) tile[((size_t)i * P.np + j) * P.np + k + 1] = phi[2 * b + 1];
+    }
+}

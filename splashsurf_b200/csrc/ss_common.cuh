@@ -50,6 +50,10 @@ struct SsDev {
     int sup;                                   // supported points per axis = 2R + 2
     // multi-GPU partition: memberships are kept only for subdomains with keep_lo <= ijk[part_axis] < keep_hi
     int part_axis, keep_lo, keep_hi;
+    // anisotropic kernels (ss_aniso.cuh): margin is the wider membership margin, grow / nsD stay on the standard one
+    int aniso;                                 // 1: memberships outside the neighbourhood-search grid are dropped, not an error
+    float an_lambda, an_kr;                    // smoothing of the kernel centres, maximum stretch k_r
+    uint32_t an_min_nb;                        // fewer neighbours than this: isotropic kernel
 };
 
 // ------------------------------------------------------------------ exact helpers ----

@@ -183,6 +183,7 @@ __global__ void k_ns_keys(SsDev P, const float *__restrict__ xyz, uint32_t m, co
         c[d] = ss_cell_of(xyz[3 * (uint64_t)p + d], ns.amin[d], P.h);
         if (c[d] < 0 || c[d] >= ns.nc[d] || ns.nc[d] > P.nsD) { bad = true; c[d] = 0; }
     }
+    if (bad && P.aniso) { key[e] = 0xffffffffu; return; }   // wide anisotropic margin: no density neighbour of an owned particle
     if (bad) atomicExch(err, 1);   // reference: unwrap() panic "particle outside NS grid"
     key[e] = s * (uint32_t)P.ns_stride + (uint32_t)((c[0] * P.nsD + c[1]) * P.nsD + c[2]);
 }
@@ -226,6 +227,7 @@ __global__ void k_density_flags(SsDev P, uint32_t m, const uint32_t *__restrict_
                                 const uint32_t *__restrict__ sub_flat, uint32_t *__restrict__ flag) {
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= m) return;
+    if (key[e] == 0xffffffffu) { flag[e] = 0u; return; }       // dropped member (anisotropic margin, k_ns_keys)
     const uint32_t s = key[e] / (uint32_t)P.ns_stride;
     const float4 pi = spos[e];
     const SsSubGeom g = ss_sub_geom(P, sub_flat[s]);
@@ -234,27 +236,19 @@ __global__ void k_density_flags(SsDev P, uint32_t m, const uint32_t *__restrict_
     flag[e] = inside ? 1u : 0u;
 }
 
-// The ordered neighbour sum of ONE membership entry `e` (thread-serial): the per-particle routine of k_density and the
-// fallback of the cell-cooperative kernel (ss_density.cuh) for oversized cells.
-template <bool FILL>
-__device__ __forceinline__ void ss_density_entry(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-                                                 const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
-                                                 float *__restrict__ rho, unsigned long long *__restrict__ nbr_count,
-                                                 const unsigned long long *__restrict__ nbr_off, uint32_t *__restrict__ nbr_idx) {
+// Neighbour walk of ONE membership entry `e` (thread-serial): visit(pj, dx, dy, dz, d2) for every other particle with
+// d^2 < h^2, in the reference's order (26 adjacent cells x-major, then the own cell; ascending index inside a cell), with
+// dx = xj - xi.  Shared by the densities, the neighbour lists and the anisotropy of a particle (ss_aniso.cuh).
+template <typename F>
+__device__ __forceinline__ void ss_nbr_walk(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
+                                            const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
+                                            F &&visit) {
     uint32_t k = key[e];
     uint32_t s = k / (uint32_t)P.ns_stride, cell = k - s * (uint32_t)P.ns_stride;
     float4 pi = spos[e];
     SsSubGeom g = ss_sub_geom(P, sub_flat[s]);
     SsNsGrid ns = ss_ns_grid(P, g);
     int c0 = (int)cell / (P.nsD * P.nsD), c1 = ((int)cell / P.nsD) % P.nsD, c2 = (int)cell % P.nsD;
-    // Phase 1 collects the squared distances of the neighbours (d^2 < h^2) in visiting order, phase 2 evaluates the kernel
-    // over that list: the expensive evaluation is then not executed for every candidate of the warp (only ~15 % of the
-    // candidates of the 27 cells are neighbours), and the summation order is unchanged.
-    float d2list[FILL ? 1 : SS_NS_LIST];
-    int nl = 0;
-    unsigned long long ncount = 0;
-    const unsigned long long fill_base = FILL ? nbr_off[__float_as_uint(pi.w)] : 0ull;
-    float acc = ss_kernel_scalar(P, 0.0f);
     const uint32_t base = s * (uint32_t)P.ns_stride;
     for (int pass = 0; pass < 2; ++pass) {
         for (int sx = -1; sx <= 1; ++sx) for (int sy = -1; sy <= 1; ++sy) for (int sz = -1; sz <= 1; ++sz) {
@@ -271,18 +265,39 @@ __device__ __forceinline__ void ss_density_entry(const SsDev &P, const uint32_t 
                 float4 pj = spos[t];
                 float dx = __fsub_rn(pj.x, pi.x), dy = __fsub_rn(pj.y, pi.y), dz = __fsub_rn(pj.z, pi.z);
                 float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-                if (d2 < P.h2) {
-                    if (FILL) { nbr_idx[fill_base + ncount] = __float_as_uint(pj.w); ++ncount; continue; }
-                    ++ncount;
-                    if (nl == SS_NS_LIST) {          // list full (very dense cluster): drain it, order is preserved
-                        for (int n = 0; n < SS_NS_LIST; ++n) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2list[n])));
-                        nl = 0;
-                    }
-                    d2list[nl++] = d2;
-                }
+                if (d2 < P.h2) visit(pj, dx, dy, dz, d2);
             }
         }
     }
+}
+
+// The ordered neighbour sum of ONE membership entry `e` (thread-serial): the per-particle routine of k_density and the
+// fallback of the cell-cooperative kernel (ss_density.cuh) for oversized cells.
+template <bool FILL>
+__device__ __forceinline__ void ss_density_entry(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
+                                                 const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
+                                                 float *__restrict__ rho, unsigned long long *__restrict__ nbr_count,
+                                                 const unsigned long long *__restrict__ nbr_off, uint32_t *__restrict__ nbr_idx) {
+    const float4 pi = spos[e];
+    // Phase 1 collects the squared distances of the neighbours (d^2 < h^2) in visiting order, phase 2 evaluates the kernel
+    // over that list: the expensive evaluation is then not executed for every candidate of the warp (only ~15 % of the
+    // candidates of the 27 cells are neighbours), and the summation order is unchanged.
+    float d2list[FILL ? 1 : SS_NS_LIST];
+    int nl = 0;
+    unsigned long long ncount = 0;
+    const unsigned long long fill_base = FILL ? nbr_off[__float_as_uint(pi.w)] : 0ull;
+    float acc = ss_kernel_scalar(P, 0.0f);
+    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &pj, float, float, float, float d2) {
+        if constexpr (FILL) { nbr_idx[fill_base + ncount] = __float_as_uint(pj.w); ++ncount; }
+        else {
+            ++ncount;
+            if (nl == SS_NS_LIST) {      // list full (very dense cluster): drain it, order is preserved
+                for (int n = 0; n < SS_NS_LIST; ++n) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2list[n])));
+                nl = 0;
+            }
+            d2list[nl++] = d2;
+        }
+    });
     if (FILL) return;
     for (int n = 0; n < nl; ++n) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2list[n])));
     if (nbr_count) nbr_count[__float_as_uint(pi.w)] = ncount;

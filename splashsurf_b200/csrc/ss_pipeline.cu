@@ -8,6 +8,7 @@
 #include "ss_kernels.cuh"
 #include "ss_certify.cuh"
 #include "ss_exact.cuh"
+#include "ss_aniso.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
 
@@ -101,10 +102,13 @@ struct ss_context {
     cudaEvent_t ev_stage[2] = { nullptr, nullptr };
     int sm_count = 132;              // streaming multiprocessors of the device (persistent-kernel grid sizing)
     int sph_normals = 0;             // 1: SPH normals at the mesh vertices (sph_interpolation.rs:82-133)
+    int an_on = 0;                   // 1: anisotropic kernels (ss_aniso.cuh) with the parameters `an`
+    ss_anisotropy_f32 an{};
+    cudaEvent_t ev_an[2] = { nullptr, nullptr };
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
         sub_flat, sub_off, sub_sparse, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, batch_subs, tiles, vcnt,
-        tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs;
+        tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
     uint64_t launches = 0;
     int big_attr_set = 0;            // dynamic shared memory opt-in of k_exact_warp_big done
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
@@ -130,6 +134,9 @@ struct ss_surface {
     int S = 0;
     DevBuf verts, tris, vkeys, rho, normals, nbr_off, nbr_idx;
     DevBuf weights, adj_row, adj_idx, inc_row, inc_idx;      // post-processing: smoothing weights, vertex->vertex / vertex->triangle CSR
+    DevBuf an_xbar, an_g;                                    // anisotropic mode: smoothed centres (n x 3), G entries (n x 6)
+    int has_aniso = 0;
+    float an_ms = 0.f;                                       // anisotropy stage (k_aniso), ms
     int has_normals = 0, has_neighbors = 0, has_weights = 0, has_adj = 0, has_inc = 0;
     uint64_t frame = 0;              // ss_context::frame of the reconstruction that produced this surface
     uint64_t n_neighbors = 0;
@@ -245,6 +252,7 @@ extern "C" int ss_context_create(int device, ss_context **out) {
 #endif
         for (auto &ev : c->ev) CK(cudaEventCreate(&ev));
         for (auto &ev : c->ev_stage) CK(cudaEventCreate(&ev));
+        for (auto &ev : c->ev_an) CK(cudaEventCreate(&ev));
         {
             signed char table[256][16];
             ss_mc_unpack(table);
@@ -268,11 +276,12 @@ extern "C" void ss_context_destroy(ss_context *c) {
                        &c->val_a, &c->val_b, &c->cid, &c->cub_tmp, &c->sub_flat, &c->sub_off, &c->sub_sparse, &c->sub_owned, &c->gkey_a, &c->gkey_b, &c->gval_a, &c->gval_b, &c->flags, &c->scan,
                        &c->spos, &c->rho, &c->tab_a, &c->tab_b, &c->rec, &c->ksplit, &c->batch_subs, &c->tiles, &c->vcnt, &c->tcnt,
                        &c->vmask, &c->voff, &c->vblk_off, &c->tblk_off, &c->tile_tab, &c->brick_rng, &c->bstate, &c->flag_ls, &c->off_ls, &c->list_ls, &c->flag_mc, &c->flag_fix, &c->off_mc, &c->off_fix, &c->list_mc, &c->list_fix, &c->wflag, &c->wstate, &c->desc_ls, &c->dflag, &c->doff, &c->dlist, &c->fallback, &c->fallback2, &c->fallback3, &c->pack_cnt, &c->pack_off, &c->brick_seen, &c->fix_list, &c->nflag, &c->bkeys_a, &c->bkeys_b, &c->bids_a, &c->bids_b, &c->bcount, &c->remap, &c->keep, &c->newid,
-                       &c->err, &c->pairs, &c->o_verts, &c->o_tris, &c->o_vkeys, &c->o_rho, &c->o_verts2, &c->o_vkeys2, &c->o_normals };
+                       &c->err, &c->pairs, &c->an_det, &c->an_grec, &c->o_verts, &c->o_tris, &c->o_vkeys, &c->o_rho, &c->o_verts2, &c->o_vkeys2, &c->o_normals };
     for (DevBuf *b : bufs) b->release();
     c->post.release_all();
     for (auto &ev : c->ev) cudaEventDestroy(ev);
     for (auto &ev : c->ev_stage) if (ev) cudaEventDestroy(ev);
+    for (auto &ev : c->ev_an) if (ev) cudaEventDestroy(ev);
     for (auto &h : c->h_stage) if (h) cudaFreeHost(h);
     cudaStreamDestroy(c->stream);
     delete c;
@@ -307,6 +316,14 @@ extern "C" int ss_surface_copy_normals(const ss_surface *s, float *dst) {
 }
 extern "C" const float *ss_surface_device_normals(const ss_surface *s) { return (s && s->has_normals) ? s->normals.as<float>() : nullptr; }
 extern "C" int ss_context_set_count_pairs(ss_context *c, int on) { if (!c) return SS_ERR_INVALID_PARAMETER; c->count_pairs = on ? 1 : 0; return SS_OK; }
+extern "C" int ss_context_set_anisotropy_f32(ss_context *c, const ss_anisotropy_f32 *a) {
+    if (!c) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL context");
+    if (!a) { c->an_on = 0; return SS_OK; }
+    if (!(a->smoothing >= 0.0f && a->smoothing <= 1.0f)) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropy smoothing must lie in [0, 1]");
+    if (!(a->max_stretch >= 1.0f) || !std::isfinite(a->max_stretch)) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropy max_stretch must be finite and >= 1");
+    c->an = *a; c->an_on = 1;
+    return SS_OK;
+}
 
 // ------------------------------------------------------------------ stage: input, filter, AABB, grid ----
 struct Prepared {
@@ -543,7 +560,8 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
     LAUNCH(c, k_ns_keys, nblk(M, 256), 256, D, d_xyz, M, c->cid.as<uint32_t>(), c->sub_flat.as<uint32_t>(), c->val_b.as<uint32_t>(),
            c->key_a.as<uint32_t>(), c->err.as<int>());
     const uint64_t ns_keys = (uint64_t)nsub * D.ns_stride;
-    cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>(), M, bits_for(ns_keys));
+    // anisotropic mode: members outside the neighbourhood-search grid carry key 0xffffffff and sort behind every cell
+    cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>(), M, D.aniso ? 32 : bits_for(ns_keys));
     c->tab_a.ensure(ns_keys * 4); c->tab_b.ensure(ns_keys * 4);
     CK(cudaMemsetAsync(c->tab_a.p, 0xff, ns_keys * 4, st));
     LAUNCH(c, k_mark_starts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_a.as<uint32_t>(), (uint32_t)ns_keys);
@@ -554,7 +572,7 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
     if (want_nbrs) { out->nbr_off.ensure((n + 1) * 8); d_ncnt = out->nbr_off.as<unsigned long long>(); CK(cudaMemsetAsync(d_ncnt, 0, (n + 1) * 8, st)); }
     // entries with the particle inside the subdomain (every particle is inside at most one: <= n of them), compacted
     c->dflag.ensure((size_t)M * 4); c->doff.ensure((size_t)M * 4 + 4); c->dlist.ensure(std::max<uint64_t>(n, 1) * 4);
-    if (c->density_variant >= 1 && !want_nbrs) {
+    if (c->density_variant >= 1 && !want_nbrs && !D.aniso) {
         // cell-cooperative kernel (ss_density.cuh): one warp per h-cell that holds a particle inside its subdomain (<= n cells), persistent grid
         LAUNCH(c, k_density_cell_flags, nblk(M, 256), 256, D, M, c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
                c->tab_b.as<uint32_t>(), c->dflag.as<uint32_t>());
@@ -612,7 +630,10 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
 
 // Splat bins: memberships sorted by (subdomain, 8^3-point brick bin) + the particle records (x, y, z, V) the level set gathers.
 // val_b still holds the membership particle indices in subdomain order (stable input for the bin sort).
-static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, const float *d_rho, uint32_t M, uint32_t nsub, bool partitioned) {
+// Anisotropic mode: d_xyz are the smoothed centres and `an_g` / `an_det` the per-particle G entries and determinants; the records
+// then carry V det G and the G entries go to c->an_grec.  `record_event` = false: a re-binning that is not part of the stage time.
+static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, const float *d_rho, uint32_t M, uint32_t nsub, bool partitioned,
+                         const float *an_g = nullptr, const float *an_det = nullptr, bool record_event = true) {
     cudaStream_t st = c->stream;
     LAUNCH(c, k_bin_keys, nblk(M, 256), 256, D, d_xyz, M, c->cid.as<uint32_t>(), c->sub_flat.as<uint32_t>(), c->val_b.as<uint32_t>(),
            partitioned ? c->sub_owned.as<uint8_t>() : nullptr, c->key_a.as<uint32_t>());
@@ -625,9 +646,14 @@ static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, cons
     c->rec.ensure((size_t)M * 16); c->ksplit.ensure((size_t)M * 4);
     LAUNCH(c, k_records, nblk(M, 256), 256, D, d_xyz, d_rho, M, c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(),
            c->sub_flat.as<uint32_t>(), c->rec.as<float4>(), c->ksplit.as<int>());
+    if (an_g) {
+        c->an_grec.ensure((size_t)M * 32);
+        LAUNCH(c, k_records_aniso, nblk(M, 256), 256, M, c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(), an_g, an_det, c->rec.as<float4>(),
+               c->an_grec.as<float4>());
+    }
     int h_err = 0;
     CK(cudaMemcpyAsync(&h_err, c->err.p, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(c->ev[5], st));
+    if (record_event) CK(cudaEventRecord(c->ev[5], st));
     CK(cudaStreamSynchronize(st));
     if (h_err) return ss_fail(SS_ERR_INVALID_PARAMETER, "particle outside of its subdomain's neighbourhood-search grid (reference: panic)");
     return SS_OK;
@@ -692,6 +718,45 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
     }
 }
 
+// Anisotropic level set of one batch (ss_aniso.cuh): work list of non-empty bricks without extension tasks (the single-point
+// planes of the last brick are bricks of their own), warp-per-brick kernel, then the 4096-slot slice, then selection.  Every
+// listed brick gets state 2 (exact values).  Returns the length of the work list.
+static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, uint64_t &ls_launches) {
+    SsDev Dw = D;
+    Dw.ext_bricks = 0;
+    const uint32_t n_work = build_worklist(c, Dw, nbatch);
+    if (!n_work) return 0;
+    cudaStream_t st = c->stream;
+    SsAnArgs A{};
+    A.bin_start = c->tab_a.as<uint32_t>(); A.bin_end = c->tab_b.as<uint32_t>(); A.rec = c->rec.as<float4>(); A.grec = c->an_grec.as<float4>();
+    A.pidx = c->val_a.as<uint32_t>(); A.tile_tab = c->tile_tab.as<SsTile>(); A.brick_rng = c->brick_rng.as<int2>();
+    A.bricks = c->list_ls.as<uint32_t>(); A.n_bricks = n_work; A.tiles = c->tiles.as<float>(); A.bstate = c->bstate.as<uint8_t>();
+    c->fallback.ensure(((size_t)n_work + 1) * 4);
+    CK(cudaMemsetAsync(c->fallback.p, 0, 4, st));
+    A.fallback = c->fallback.as<uint32_t>();
+    LAUNCH(c, (k_aniso_levelset<SS_AN_CAP, SS_AN_WARPS>), (n_work + SS_AN_WARPS - 1) / SS_AN_WARPS, SS_AN_WARPS * 32, Dw, A);
+    ++ls_launches;
+    uint32_t n_fb = 0;
+    CK(cudaMemcpyAsync(&n_fb, c->fallback.p, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (n_fb) {
+        c->fallback2.ensure(((size_t)n_fb + 1) * 4);
+        CK(cudaMemsetAsync(c->fallback2.p, 0, 4, st));
+        SsAnArgs B = A;
+        B.bricks = c->fallback.as<uint32_t>() + 1; B.n_bricks = n_fb; B.bstate = nullptr; B.fallback = c->fallback2.as<uint32_t>();
+        LAUNCH(c, (k_aniso_levelset<SS_AN_BIG_CAP, 1>), n_fb, 32, Dw, B);
+        ++ls_launches;
+        CK(cudaMemcpyAsync(&n_fb, c->fallback2.p, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (n_fb) {
+            B.bricks = c->fallback2.as<uint32_t>() + 1; B.n_bricks = n_fb; B.fallback = nullptr;
+            LAUNCH(c, k_aniso_select, n_fb, 32, Dw, B);
+            ++ls_launches;
+        }
+    }
+    return n_work;
+}
+
 // Level set of one batch of tiles: work list, certification + exact values (fused kernel, or variant 1: certification kernel +
 // exact pass), brick classification, fix-up sweep.  Leaves the tiles, the per-brick states and the marching-cubes brick list
 // (c->list_mc, *n_mc_out entries) in the context scratch.
@@ -705,10 +770,10 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     A.pairs = c->count_pairs ? c->pairs.as<unsigned long long>() : nullptr;
     A.mode = exact_all ? SS_LS_EXACT_ALL : SS_LS_CERTIFY;
     A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = c->bstate.as<uint8_t>();
-    const uint32_t n_work = build_worklist(c, D, nbatch);
+    const uint32_t n_work = D.aniso ? launch_aniso_levelset(c, D, nbatch, ls_launches) : build_worklist(c, D, nbatch);
     A.work_list = c->list_ls.as<uint32_t>();
-    const bool split_certify = c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
-    if (n_work && !split_certify) { launch_levelset(c, dim3(n_work), D, A, c->count_pairs != 0, global_mode); ++ls_launches; }
+    const bool split_certify = !D.aniso && c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
+    if (n_work && !split_certify && !D.aniso) { launch_levelset(c, dim3(n_work), D, A, c->count_pairs != 0, global_mode); ++ls_launches; }
     if (n_work && split_certify) {
         // variant 1 (ss_certify.cuh): certification kernel, then the exact pass over the boxes it could not certify
         const uint32_t nbr_c = nbatch * nbricks;
@@ -910,8 +975,12 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     const float h = p->compact_support_radius, cs = p->cube_size;
     const float r2 = faddr(p->particle_radius, p->particle_radius);
     const float rest_mass = fmulr(fmulr(fmulr(r2, r2), r2), p->rest_density);
-    const float margin = global_mode ? fmulr(cs, ceilf(fdivr(h, cs)) + 2.0f)      // stencil reach (R + 1 cells) + slack
-                                     : fmulr(fmulr(ceilf(fdivr(h, cs)), cs), 1.01f);
+    const float ns_margin = global_mode ? fmulr(cs, ceilf(fdivr(h, cs)) + 2.0f)      // stencil reach (R + 1 cells) + slack
+                                        : fmulr(fmulr(ceilf(fdivr(h, cs)), cs), 1.01f);
+    // anisotropic kernels (ss_aniso.cuh): a kernel centre moves up to smoothing * h < h from its particle, so memberships need a
+    // margin of 2h; the neighbourhood-search grids and cell lists stay on the standard margin (bit-identical densities)
+    const bool aniso = c->an_on && !global_mode && !part.enabled && !part.given_rho;
+    const float margin = aniso ? fmulr(fmulr(ceilf(fdivr(fmulr(2.0f, h), cs)), cs), 1.01f) : ns_margin;
     int64_t nsd[3], ncg[3];
     for (int d = 0; d < 3; ++d) { nsd[d] = (PP.grid.nc[d] + S - 1) / S; ncg[d] = nsd[d] * S; }
     HostGrid gg, sg;
@@ -931,17 +1000,19 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     SsDev D{};
     for (int d = 0; d < 3; ++d) { D.gmin[d] = gg.mn[d]; D.nsd[d] = (int)nsd[d]; }
     D.c = cs; D.h = h; D.h2 = fmulr(h, h); D.h2m = fmulr(D.h2, 1.01f); D.thr = p->iso_surface_threshold;
-    D.rest_mass = rest_mass; D.sub_size = sub_size; D.margin = margin; D.grow = fmulr(margin, 1.5f);
+    D.rest_mass = rest_mass; D.sub_size = sub_size; D.margin = margin; D.grow = fmulr(ns_margin, 1.5f);
     D.S = (int)S; D.np = (int)S + 1; D.np_magic = (uint32_t)(4294967296ull / (uint64_t)D.np) + 1u;
     D.R = (int)ceilf(fdivr(h, cs));
     D.srad = (int)ceilf(fdivr(margin, sub_size));
     if (D.srad > 8) return ss_fail(SS_ERR_INVALID_PARAMETER, "ghost margin spans more than 8 subdomains; increase subdomain_num_cubes_per_dim");
     fill_kernel_consts(D, h);
-    D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)margin) / (double)h) + 3;
+    D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)ns_margin) / (double)h) + 3;
     D.ns_stride = D.nsD * D.nsD * D.nsD;
     fill_bins(D, cs);
     D.simd = p->enable_simd ? 1 : 0;
     D.gmode = global_mode ? 1 : 0;
+    D.aniso = aniso ? 1 : 0;
+    D.an_lambda = c->an.smoothing; D.an_kr = c->an.max_stretch; D.an_min_nb = c->an.min_neighbors;
     uint64_t g_ns_cells = 0;
     if (global_mode) {
         HostGrid ns;
@@ -979,6 +1050,11 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     out->rho.ensure(std::max<uint64_t>(n, 1) * 4);
     float *d_rho = out->rho.as<float>();
     CK(cudaMemsetAsync(d_rho, 0, std::max<uint64_t>(n, 1) * 4, st));
+    if (aniso) {
+        out->an_xbar.ensure(std::max<uint64_t>(n, 1) * 12); out->an_g.ensure(std::max<uint64_t>(n, 1) * 24); c->an_det.ensure(std::max<uint64_t>(n, 1) * 4);
+        if (n) LAUNCH(c, k_aniso_init, nblk(n, 256), 256, d_xyz, (uint32_t)n, out->an_xbar.as<float>(), out->an_g.as<float>(), c->an_det.as<float>());
+        out->has_aniso = 1;
+    }
     // NOTE (multi-GPU): the max-reduce callback is a collective -- every rank must call it exactly once per
     // reconstruction, also ranks that received no particles or own no subdomain.
     if (n == 0) {
@@ -1070,8 +1146,17 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     // ---- densities, then the splat bins
     rc = stage_densities(c, D, d_xyz, n, M, nsub, g_ns_cells, global_mode, want_nbrs, out, d_rho);
     if (rc) return rc;
+    if (aniso) {
+        // x_bar, G, det G of every particle in its owning subdomain, over the density stage's list and cell tables
+        CK(cudaEventRecord(c->ev_an[0], st));
+        LAUNCH(c, k_aniso, nblk(n, 128), 128, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
+               c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(), c->tab_a.as<uint32_t>(), c->tab_b.as<uint32_t>(),
+               out->an_xbar.as<float>(), out->an_g.as<float>(), c->an_det.as<float>());
+        CK(cudaEventRecord(c->ev_an[1], st));
+    }
     CK(cudaEventRecord(c->ev[4], st));
-    rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, part.enabled != 0);
+    if (aniso) rc = stage_binning(c, D, out->an_xbar.as<float>(), d_rho, M, nsub, false, out->an_g.as<float>(), c->an_det.as<float>());
+    else rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, part.enabled != 0);
     if (rc) return rc;
 
     // ---- level set + marching cubes over batches of subdomain tiles
@@ -1124,7 +1209,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     float ls_ms = 0.f, mc_ms = 0.f, setup_ms = 0.f;
     uint64_t ls_launches = 0, fix_points = 0;
     out->tile.clear();
-    const bool exact_all = c->ls_exact_all || c->keep_tile_flat >= 0;
+    const bool exact_all = c->ls_exact_all || c->keep_tile_flat >= 0 || aniso;
     for (uint32_t s0 = 0; s0 < nown; s0 += (uint32_t)max_tiles) {
         const uint32_t nbatch = std::min<uint32_t>((uint32_t)max_tiles, nown - s0);
         for (uint32_t q = 0; q < nbatch; ++q) {
@@ -1182,6 +1267,11 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     if (rc) return rc;
     out->nv = nv_final; out->nt = ttotal;
     c->hint_nv = vtotal; c->hint_nt = ttotal; c->hint_bc = bc;
+    if (aniso) {
+        // SPH normals and the [bins] post-processing entries use the isotropic kernel at the particle positions: bin them again
+        rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, false, nullptr, nullptr, /*record_event=*/false);
+        if (rc) return rc;
+    }
     {
         // the splat bins stay in the scratch until the next call on this context: ss_post.cuh queries them
         const float r3p = fmulr(fmulr(p->particle_radius, p->particle_radius), p->particle_radius);
@@ -1214,7 +1304,8 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     ss_timings &T = out->tm;
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, c->ev[2], c->ev[3])); T.decomposition = ms;
-    CK(cudaEventElapsedTime(&ms, c->ev[3], c->ev[4])); T.density = ms;
+    CK(cudaEventElapsedTime(&ms, c->ev[3], aniso ? c->ev_an[0] : c->ev[4])); T.density = ms;
+    if (aniso) { CK(cudaEventElapsedTime(&ms, c->ev_an[0], c->ev_an[1])); out->an_ms = ms; }
     CK(cudaEventElapsedTime(&ms, c->ev[4], c->ev[5])); T.binning = ms;
     T.levelset = ls_ms; T.marching_cubes = mc_ms; T.tile_setup = setup_ms;
     CK(cudaEventElapsedTime(&ms, c->ev[7], c->ev[8])); T.stitching = ms;
@@ -1513,6 +1604,7 @@ static int reconstruct_partition_impl(ss_context *c, const float *xyz, uint64_t 
     int rc = validate_params(p);
     if (rc) return rc;
     if (p->has_particle_aabb) return ss_fail(SS_ERR_UNSUPPORTED, "filter particles before partitioning (particle_aabb is applied by the caller)");
+    if (c->an_on) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels are not available on partitioned (multi-GPU) reconstructions");
     if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "partitioned reconstruction requires the subdomain grid");
     if (axis < 0 || axis > 2 || own_lo < 0 || own_hi < own_lo || halo < 0) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad partition");
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
@@ -1627,7 +1719,11 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
         s->n = P.n; s->grid = P.grid;
         // decomposition decision, lib.rs:421-464
         int use_dec = 0;
-        if (p->spatial_decomposition == 1) {
+        if (c->an_on) {
+            // anisotropic kernels: subdomain path only, always decomposed (no auto-disable)
+            if (p->spatial_decomposition != 1) { ss_surface_free(s); return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels require the subdomain grid (spatial_decomposition = UniformGrid)"); }
+            use_dec = 1;
+        } else if (p->spatial_decomposition == 1) {
             if (p->auto_disable) {
                 int64_t mc = std::max(P.grid.nc[0], std::max(P.grid.nc[1], P.grid.nc[2]));
                 uint32_t with_margin = (uint32_t)(1.2 * (double)p->subdomain_num_cubes_per_dim);
@@ -1675,6 +1771,7 @@ extern "C" void ss_surface_free(ss_surface *s) {
     }
     s->verts.release(); s->tris.release(); s->vkeys.release(); s->rho.release(); s->normals.release(); s->nbr_off.release(); s->nbr_idx.release();
     s->weights.release(); s->adj_row.release(); s->adj_idx.release(); s->inc_row.release(); s->inc_idx.release();
+    s->an_xbar.release(); s->an_g.release();
     delete s;
 }
 
@@ -1808,6 +1905,14 @@ extern "C" int ss_surface_copy_neighbor_lists(const ss_surface *s, uint64_t *off
     return rc;
 }
 extern "C" int ss_surface_timings(const ss_surface *s, ss_timings *o) { if (!s || !o) return SS_ERR_INVALID_PARAMETER; *o = s->tm; return SS_OK; }
+extern "C" float ss_surface_anisotropy_ms(const ss_surface *s) { return (s && s->has_aniso) ? s->an_ms : 0.0f; }
+extern "C" int ss_surface_copy_anisotropy(const ss_surface *s, float *xbar, float *g) {
+    if (!s) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL surface");
+    if (!s->has_aniso) return ss_fail(SS_ERR_INVALID_PARAMETER, "the surface was not reconstructed with anisotropic kernels");
+    int rc = xbar ? copy_out(s, xbar, s->an_xbar.p, s->n * 12) : SS_OK;
+    if (rc == SS_OK && g) rc = copy_out(s, g, s->an_g.p, s->n * 24);
+    return rc;
+}
 
 #include "ss_post.cuh"
 #include "ss_meshproc.inc"

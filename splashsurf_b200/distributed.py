@@ -216,8 +216,12 @@ def _pinned(t: torch.Tensor, device) -> torch.Tensor:
 class Runner:
     """Drives one reconstruct step on this rank's GPU (world == 1: plain C-ABI call)."""
 
-    def __init__(self, ctx, params, world: int, rank: int, local_rank: int, group=None, device=None, protocol: str = "stats"):
+    def __init__(self, ctx, params, world: int, rank: int, local_rank: int, group=None, device=None, protocol: str = "stats", anisotropy=None):
         self.ctx, self.params, self.world, self.rank, self.local_rank, self.group = ctx, params, world, rank, local_rank, group
+        # anisotropic kernels (splashsurf_b200.Anisotropy): single GPU only -- the slab partition does not provide them
+        if anisotropy is not None and world > 1:
+            raise ValueError("anisotropic kernels are not available on multi-GPU (partitioned) reconstructions; run them on one GPU")
+        self.anisotropy = anisotropy
         # how the global maximum subdomain population (sparse rule) reaches the library: "stats" (default) = the plan statistics
         # count the members of every subdomain with the exact classifier (ss_partition_members_f32), their all-reduced maximum
         # is passed to ONE library call; "two_call" = decomposition pre-pass, all-reduce, full call (one more library call per step);
@@ -274,10 +278,20 @@ class Runner:
     # -- single GPU
     def _step_single(self, xyz_ptr: int, n: int, copy_out: bool, params=None, force_copy: bool = False) -> dict:
         L = self.ctx._L
-        s = self.ctx.reconstruct_raw(xyz_ptr, n, self.params if params is None else params)
+        if self.anisotropy is not None:
+            from . import _check
+            _check(L, L.ss_context_set_anisotropy_f32(self.ctx._h, C.byref(self.anisotropy._abi())))
+        try:
+            s = self.ctx.reconstruct_raw(xyz_ptr, n, self.params if params is None else params)
+        finally:
+            if self.anisotropy is not None:
+                L.ss_context_set_anisotropy_f32(self.ctx._h, None)
         keep = self.keep_surface and self.world == 1
         try:
-            return self._collect(s, copy_out, n_local=n, force_copy=force_copy)
+            out = self._collect(s, copy_out, n_local=n, force_copy=force_copy)
+            if self.anisotropy is not None:
+                out["timings"]["anisotropy"] = float(L.ss_surface_anisotropy_ms(s))
+            return out
         finally:
             if keep:
                 self.release_kept()
@@ -735,7 +749,8 @@ class DistributedReconstructor:
     reference (lib.rs:476-516) and filters every rank's particles before the exchange; the mesh post-processing of
     `reconstruction_pipeline` is a single-GPU step."""
 
-    def __init__(self, *, sph_normals: bool = False, group=None, device=None, protocol: str = "stats", local_rank: Optional[int] = None, **params):
+    def __init__(self, *, sph_normals: bool = False, group=None, device=None, protocol: str = "stats", local_rank: Optional[int] = None,
+                 anisotropy=None, **params):
         import os
         import splashsurf_b200 as ss
         if not dist.is_initialized():
@@ -745,6 +760,9 @@ class DistributedReconstructor:
         if params.get("aabb_min") is not None and params.get("aabb_max") is not None:
             self._aabb = (np.asarray(params["aabb_min"], np.float64).astype(np.float32), np.asarray(params["aabb_max"], np.float64).astype(np.float32))
         self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
+        if anisotropy is not None and self.world > 1:
+            raise ValueError("anisotropic kernels are not available on multi-GPU (partitioned) reconstructions; run them on one GPU")
+        self.anisotropy = anisotropy
         lr = int(os.environ.get("LOCAL_RANK", "0")) if local_rank is None else int(local_rank)
         self.ctx = ss.Context(lr if device is None else 0)
         self.sph_normals = bool(sph_normals)
@@ -760,7 +778,7 @@ class DistributedReconstructor:
         ss = self._ss
         p = np.ascontiguousarray(particles_local, dtype=np.float32).reshape(-1, 3)
         if self.world == 1:
-            r = ss.reconstruct_surface(p, context=self.ctx, sph_normals=self.sph_normals, **self._kw)
+            r = ss.reconstruct_surface(p, context=self.ctx, sph_normals=self.sph_normals, anisotropy=self.anisotropy, **self._kw)
             return ss.MeshWithData(r.mesh, {"normals": r.normals} if self.sph_normals and r.normals is not None else {}, {})
         if self._aabb is not None:                    # lib.rs:369-406: particles outside the half-open box take no part
             p = np.ascontiguousarray(p[np.all(p >= self._aabb[0], axis=1) & np.all(p < self._aabb[1], axis=1)])
