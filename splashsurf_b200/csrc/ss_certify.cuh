@@ -182,6 +182,7 @@ __global__ void k_wstate_reduce(const uint8_t *__restrict__ wstate, uint32_t nbr
 //      (0.55 h .. 0.76 h, where g vanishes) follows only for the few boxes that are still short;
 //   5. certified sub-boxes store SS_MARKER, the others raise their per-box flag for the exact pass (k_levelset, SS_LS_FIX).
 // The +1 planes of tiles with 8 k + 1 points per axis (extension tasks) reuse the scalar one-point-per-lane sweep.
+// Warps are persistent and claim bricks in work-list order; step 1 of the next brick runs while step 2's copies are in flight.
 // Soundness is that of variant 0/1: every term of the reference's sum is >= 0 and g <= W / sigma, so a certified point is
 // inside for the reference too; failing to certify only costs time.  Results are therefore identical by construction.
 #include "ss_sm90.cuh"
@@ -204,6 +205,7 @@ struct SsCwArgs {
     float *tiles;
     uint8_t *wstate;                   // [batch][nb^3][16]
     unsigned long long *evals;         // optional work counter: candidate evaluations of the certification (lane-level)
+    uint32_t *taken;                   // work-list entries handed out beyond the first wave (zero at launch)
     float g1, g2, g3;                  // cubic bound in d^2: g = G0 + g1 d2 + g2 d2^2 + g3 d2^3 (G_k / h^(2k), host-computed)
     float r0sq, r1sq;                  // ring radii squared: (0.55 h)^2, (0.76 h)^2
 };
@@ -279,23 +281,26 @@ __device__ __forceinline__ void ss_cw_fold_pairs(const SsCwPoint &Q, float ngzA,
     }
 }
 
-template <bool GLOBAL, bool COUNT, int CAP, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, 20 / WARPS)
-k_certify_warp(SsDev P, SsCwArgs A) {
-    __shared__ SsCwSlice<CAP> s_slice[WARPS];
-    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    SsCwSlice<CAP> &S = s_slice[wib];
-    const uint32_t work = blockIdx.x * WARPS + wib;
-    if (work >= A.n_work) return;
-    if (lane == 0) { ss_mbar_init(&S.mbar, 1); ss_mbar_fence_init(); }
+// A listed brick's candidate runs, one per lane (ss_cw_lookup), ready to be copied into the warp's slice (ss_cw_issue).
+struct SsCwRuns {
+    uint4 desc;                        // work descriptor
+    uint32_t run_a, run_len, run_dst;  // this lane's run: source record, length, destination slot
+    int C;                             // candidates to certify; 0: the brick needs no sweep
+};
+
+// Looks up the candidate runs of the brick `desc` (global loads and shuffles only, the slice is not touched).  C = 0 when the
+// brick needs no sweep: no candidate (its boxes stay in state 0, exact zeros) or more than CAP (every box goes to the exact pass,
+// recorded here).
+template <int CAP>
+__device__ __forceinline__ SsCwRuns ss_cw_lookup(const SsDev &P, const SsCwArgs &A, const uint4 desc, int lane) {
+    SsCwRuns R;
+    R.desc = desc; R.run_a = 0; R.run_len = 0; R.run_dst = 0; R.C = 0;
     const int nb = P.nb;
-    const uint4 desc = A.work_desc[work];
     const int tile_idx = (int)desc.y;
     const int bx = (int)(desc.z & 1023u), by = (int)((desc.z >> 10) & 1023u), bz = (int)(desc.z >> 20);
     const bool ext = P.ext_bricks != 0;
     const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
-    const SsTile T = A.tile_tab[tile_idx];
-    const bool sparse = GLOBAL || T.sparse != 0;
+    const uint32_t tile_s = A.tile_tab[tile_idx].s;
     uint8_t *const wst = A.wstate + (size_t)desc.x * SS_LS_WARPS;
 
     // ---- candidate runs: one per lane, exclusive prefix by shuffles
@@ -309,7 +314,7 @@ k_certify_warp(SsDev P, SsCwArgs A) {
     if (lane < nruns) {
         const int X = rx.x + lane / nyr, Y = ry.x + lane % nyr;
         uint32_t a = 0xffffffffu, b = 0;
-        const uint32_t base = T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
+        const uint32_t base = tile_s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
         for (int Z = rz.x; Z <= rz.y; ++Z) {
             const uint32_t st = A.bin_start[base + Z];
             if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
@@ -320,7 +325,7 @@ k_certify_warp(SsDev P, SsCwArgs A) {
     for (int o = 1; o < 32; o <<= 1) { const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
     const uint32_t run_dst = incl - run_len;
     const int C = (int)__shfl_sync(0xffffffffu, incl, 31);
-    if (C == 0) return;                                         // tile is pre-zeroed: phi = 0 exactly (wstate stays 0)
+    if (C == 0) return R;                                       // phi = 0 exactly (wstate stays 0)
 
     if (C > CAP) {
         // oversized brick: everything goes to the exact pass (k_levelset's oversized path honours the per-box flags)
@@ -335,16 +340,36 @@ k_certify_warp(SsDev P, SsCwArgs A) {
                 if (lane == 0 && We.i0 < P.np && We.j0 < P.np && We.k0 < P.np) ss_mark_boxes(P, A.wstate, tile_idx, vbx, vby, vbz, We, 2);
             }
         }
-        return;
+        return R;
     }
+    R.run_a = run_a; R.run_len = run_len; R.run_dst = run_dst; R.C = C;
+    return R;
+}
 
-    // ---- stage the runs: bulk asynchronous copies (TMA engine) completing on the warp's mbarrier
-    __syncwarp();                                               // barrier initialised before anyone arrives / copies
-    if (lane == 0) ss_mbar_arrive_expect_tx(&S.mbar, (uint32_t)C * 16u);
+// Starts the bulk asynchronous copies (TMA engine) of the runs R into the warp's slice; they complete on its mbarrier.
+// The slice was last read (and, on the global path, written) by this warp's ordinary accesses: order those before the async
+// proxy's writes.
+template <int CAP>
+__device__ __forceinline__ void ss_cw_issue(SsCwSlice<CAP> &S, const SsCwArgs &A, const SsCwRuns &R, int lane) {
     __syncwarp();
-    if (run_len) ss_bulk_g2s(&S.rec[run_dst], A.rec + run_a, run_len * 16u, &S.mbar);
+    ss_fence_proxy_async();
+    if (lane == 0) ss_mbar_arrive_expect_tx(&S.mbar, (uint32_t)R.C * 16u);
     __syncwarp();
-    ss_mbar_wait(&S.mbar, 0);
+    if (R.run_len) ss_bulk_g2s(&S.rec[R.run_dst], A.rec + R.run_a, R.run_len * 16u, &S.mbar);
+    __syncwarp();
+}
+
+// Certifies one brick whose C candidate records are in place in the slice; returns the lane-level bound evaluations (COUNT).
+template <bool GLOBAL, bool COUNT, int CAP>
+__device__ __forceinline__ unsigned long long ss_cw_brick(const SsDev &P, const SsCwArgs &A, SsCwSlice<CAP> &S, const uint4 desc, int C, int lane) {
+    const int nb = P.nb;
+    const int tile_idx = (int)desc.y;
+    const int bx = (int)(desc.z & 1023u), by = (int)((desc.z >> 10) & 1023u), bz = (int)(desc.z >> 20);
+    const bool ext = P.ext_bricks != 0;
+    const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
+    const SsTile T = A.tile_tab[tile_idx];
+    const bool sparse = GLOBAL || T.sparse != 0;
+    uint8_t *const wst = A.wstate + (size_t)desc.x * SS_LS_WARPS;
 
     // ---- level 1: per candidate, ring-0 membership for the eight sub-boxes (bit b = a * 4 + bb * 2 + cc: upper half in x, y, z)
     const int nwords = (C + 31) >> 5;
@@ -506,6 +531,45 @@ k_certify_warp(SsDev P, SsCwArgs A) {
             if (st == 3 && L.valid) A.tiles[L.out_idx] = 0.0f;        // exact zero, stored (no zero-fill of the tiles beforehand)
             if (lane == 0) ss_mark_boxes(P, A.wstate, tile_idx, vbx, vby, vbz, We, st);
         }
+    }
+    __syncwarp();                                                  // the slice is refilled for the next brick
+    return n_eval;
+}
+
+// Persistent warps: warp g of G starts with listed brick g and then takes the next unclaimed entry of the work list (a counter), so
+// the bricks in flight stay a window of neighbouring bricks, whose candidates share the L2; each brick's result depends on that
+// brick only, whichever warp takes it.  The run lookup of the next brick -- a chain of dependent global loads: work descriptor, tile table, brick
+// ranges, bin table -- is done while the current brick's bulk copies are in flight, so the two latencies overlap instead of adding
+// up.  One slice per warp, so the occupancy stays that of one brick per warp (20 warps per SM).
+template <bool GLOBAL, bool COUNT, int CAP, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, 20 / WARPS)
+k_certify_warp(SsDev P, SsCwArgs A) {
+    __shared__ SsCwSlice<CAP> s_slice[WARPS];
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    SsCwSlice<CAP> &S = s_slice[wib];
+    const uint32_t stride = gridDim.x * WARPS;
+    uint32_t work = blockIdx.x * WARPS + wib;
+    if (work >= A.n_work) return;
+    if (lane == 0) { ss_mbar_init(&S.mbar, 1); ss_mbar_fence_init(); }
+    __syncwarp();                                                  // barrier initialised before anyone arrives / copies
+    SsCwRuns R = ss_cw_lookup<CAP>(P, A, A.work_desc[work], lane);
+    uint32_t phase = 0;
+    unsigned long long n_eval = 0;
+    while (work < A.n_work) {
+        if (R.C) ss_cw_issue(S, A, R, lane);
+        uint32_t next = 0;
+        if (lane == 0) next = stride + atomicAdd(A.taken, 1u);
+        next = __shfl_sync(0xffffffffu, next, 0);
+        SsCwRuns Rn = R;
+        Rn.C = 0;
+        if (next < A.n_work) Rn = ss_cw_lookup<CAP>(P, A, A.work_desc[next], lane);
+        if (R.C) {
+            ss_mbar_wait(&S.mbar, phase);
+            phase ^= 1u;
+            n_eval += ss_cw_brick<GLOBAL, COUNT, CAP>(P, A, S, R.desc, R.C, lane);
+        }
+        R = Rn;
+        work = next;
     }
     if (COUNT && A.evals) {
         for (int o = 16; o > 0; o >>= 1) n_eval += __shfl_xor_sync(0xffffffffu, n_eval, o);

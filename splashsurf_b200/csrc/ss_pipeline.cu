@@ -790,12 +790,18 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
             W.bin_start = A.bin_start; W.bin_end = A.bin_end; W.rec = A.rec; W.tile_tab = A.tile_tab; W.brick_rng = A.brick_rng;
             W.work_desc = c->desc_ls.as<uint4>(); W.n_work = n_work; W.tiles = A.tiles; W.wstate = c->wstate.as<uint8_t>();
             W.evals = c->count_pairs ? c->pairs.as<unsigned long long>() + 1 : nullptr;
+            c->nflag.ensure(8);                                  // work-list counter of the persistent warps (the fix-up sweep re-zeroes it)
+            CK(cudaMemsetAsync(c->nflag.p, 0, 4, st));
+            W.taken = c->nflag.as<uint32_t>();
             const double ih2 = 1.0 / ((double)D.h * (double)D.h);
             W.g1 = (float)((double)SS_G1 * ih2); W.g2 = (float)((double)SS_G2 * ih2 * ih2); W.g3 = (float)((double)SS_G3 * ih2 * ih2 * ih2);
             W.r0sq = 0.3025f * D.h2; W.r1sq = 0.58f * D.h2;
             const bool cw_small = certify_runs <= 16;            // at most 4 candidate bins per axis (3 + the extension plane)
-#define SS_CW_GO(G_, C_) do { if (cw_small) LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_S, SS_CW_WARPS_S>), (n_work + SS_CW_WARPS_S - 1) / SS_CW_WARPS_S, SS_CW_WARPS_S * 32, D, W); \
-                                 else LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_L, SS_CW_WARPS_L>), (n_work + SS_CW_WARPS_L - 1) / SS_CW_WARPS_L, SS_CW_WARPS_L * 32, D, W); } while (0)
+            // persistent warps: one wave of CTAs (20 warps per SM), fewer when the work list is short
+            const unsigned grid_s = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * (20 / SS_CW_WARPS_S), (n_work + SS_CW_WARPS_S - 1) / SS_CW_WARPS_S);
+            const unsigned grid_l = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * (20 / SS_CW_WARPS_L), (n_work + SS_CW_WARPS_L - 1) / SS_CW_WARPS_L);
+#define SS_CW_GO(G_, C_) do { if (cw_small) LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_S, SS_CW_WARPS_S>), grid_s, SS_CW_WARPS_S * 32, D, W); \
+                                 else LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_L, SS_CW_WARPS_L>), grid_l, SS_CW_WARPS_L * 32, D, W); } while (0)
             if (global_mode) { if (c->count_pairs) SS_CW_GO(true, true); else SS_CW_GO(true, false); }
             else { if (c->count_pairs) SS_CW_GO(false, true); else SS_CW_GO(false, false); }
 #undef SS_CW_GO
