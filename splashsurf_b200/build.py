@@ -40,7 +40,7 @@ def source_hash(only=None) -> str:
 
 # the files that define the level-set kernels (certification, exact pass, shared device helpers): a DRAM-traffic capture of the
 # level-set stage stays valid while these are unchanged
-LEVELSET_SOURCES = ("ss_certify.cuh", "ss_exact.cuh", "ss_kernels.cuh", "ss_sm90.cuh", "ss_common.cuh")
+LEVELSET_SOURCES = ("ss_brick.cuh", "ss_certify.cuh", "ss_exact.cuh", "ss_kernels.cuh", "ss_sm90.cuh", "ss_common.cuh")
 
 
 def levelset_source_hash() -> str:

@@ -160,12 +160,8 @@ __global__ void k_records_aniso(uint32_t m, const uint32_t *__restrict__ key, co
 
 // ------------------------------------------------------------------ level set ----
 struct SsAnArgs {
-    const uint32_t *bin_start, *bin_end;
-    const float4 *rec;                 // (x_bar, V det G), bin-sorted
+    SsBins bins;                       // records: (x_bar, V det G), bin-sorted
     const float4 *grec;                // two per record: (g00, g01, g02, g11), (g12, g22, -, -)
-    const uint32_t *pidx;              // bin-sorted particle indices
-    const SsTile *tile_tab;
-    const int2 *brick_rng;
     const uint32_t *bricks;            // listed bricks (linear index)
     uint32_t n_bricks;
     float *tiles;
@@ -183,48 +179,25 @@ __device__ __forceinline__ float ss_aniso_term(const SsDev &P, const float4 r, c
     return uu < P.h2 ? __fadd_rn(phi, __fmul_rn(r.w, ss_kernel_scalar(P, __fsqrt_rn(uu)))) : phi;
 }
 
-struct SsAnBrick { int bx, by, bz, tile; int2 rx, ry, rz; int nyr, nruns; SsTile T; };
+// a listed brick, its tile and its candidate bins (no extension planes: the single-point planes are bricks of their own)
+struct SsAnBrick { SsBrick B; SsTile T; SsBrickBins K; };
 __device__ __forceinline__ SsAnBrick ss_an_brick(const SsDev &P, const SsAnArgs &A, uint32_t brick_lin) {
-    SsAnBrick B;
-    uint32_t q = brick_lin;
-    const uint32_t nb = (uint32_t)P.nb;
-    B.bz = (int)(q % nb); q /= nb;
-    B.by = (int)(q % nb); q /= nb;
-    B.bx = (int)(q % nb); B.tile = (int)(q / nb);
-    B.T = A.tile_tab[B.tile];
-    B.rx = A.brick_rng[B.bx]; B.ry = A.brick_rng[B.by]; B.rz = A.brick_rng[B.bz];
-    B.nyr = B.ry.y - B.ry.x + 1;
-    B.nruns = (B.rx.y - B.rx.x + 1) * B.nyr;
-    return B;
+    SsAnBrick N;
+    N.B = ss_brick_from_lin(P, brick_lin);
+    N.T = A.bins.tile_tab[N.B.tile];
+    N.K = ss_brick_bins(P, A.bins.brick_rng, N.B.bx, N.B.by, N.B.bz, false);
+    return N;
 }
-// candidate run r of the brick: bins (X, Y, rz.x .. rz.y), contiguous in key order
-__device__ __forceinline__ uint32_t ss_an_run(const SsDev &P, const SsAnArgs &A, const SsAnBrick &B, int r, uint32_t &start) {
-    start = 0;
-    if (r >= B.nruns) return 0;
-    const int X = B.rx.x + r / B.nyr, Y = B.ry.x + r % B.nyr;
-    uint32_t a = 0xffffffffu, b = 0;
-    const uint32_t base = B.T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-    for (int Z = B.rz.x; Z <= B.rz.y; ++Z) {
-        const uint32_t st = A.bin_start[base + Z];
-        if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
-    }
-    if (a == 0xffffffffu) return 0;
-    start = a;
-    return b - a;
-}
-
-// lane -> its two grid points (k, k + 1) of a 4x4x4 sub-box
-#define SS_AN_LANE_IJK(lane, li, lj, lk) const int li = (lane) >> 3, lj = ((lane) >> 1) & 3, lk = ((lane) & 1) * 2
 
 template <int CAP>
 __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A, unsigned long long *s_key, uint16_t *s_list, uint32_t work, int lane) {
     const uint32_t brick_lin = A.bricks[work];
-    const SsAnBrick B = ss_an_brick(P, A, brick_lin);
+    const SsAnBrick N = ss_an_brick(P, A, brick_lin);
     if (A.bstate && lane == 0) A.bstate[brick_lin] = 2;
     uint32_t C = 0;
-    for (int r0 = 0; r0 < B.nruns; r0 += 32) {
+    for (int r0 = 0; r0 < N.K.nruns; r0 += 32) {
         uint32_t a;
-        uint32_t len = ss_an_run(P, A, B, r0 + lane, a);
+        uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r0 + lane, a);
         for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
         C += len;
     }
@@ -235,50 +208,34 @@ __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A
     }
     // ---- stage the sort keys (particle index << 32 | record index), run by run
     uint32_t dst0 = 0;
-    for (int r0 = 0; r0 < B.nruns; r0 += 32) {
-        uint32_t a;
-        const uint32_t len = ss_an_run(P, A, B, r0 + lane, a);
-        uint32_t incl = len;
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-        const uint32_t dst = dst0 + incl - len;
-        const int nr = min(32, B.nruns - r0);
+    for (int r0 = 0; r0 < N.K.nruns; r0 += 32) {
+        uint32_t a, tot;
+        const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r0 + lane, a);
+        const uint32_t dst = dst0 + ss_warp_excl_scan(len, lane, tot);
+        const int nr = min(32, N.K.nruns - r0);
         for (int rr = 0; rr < nr; ++rr) {
             const uint32_t ra = __shfl_sync(0xffffffffu, a, rr), rl = __shfl_sync(0xffffffffu, len, rr), rd = __shfl_sync(0xffffffffu, dst, rr);
-            for (uint32_t t = lane; t < rl; t += 32) s_key[rd + t] = ((unsigned long long)A.pidx[ra + t] << 32) | (unsigned long long)(ra + t);
+            for (uint32_t t = lane; t < rl; t += 32) s_key[rd + t] = ((unsigned long long)A.bins.pidx[ra + t] << 32) | (unsigned long long)(ra + t);
         }
-        dst0 += __shfl_sync(0xffffffffu, incl, 31);
+        dst0 += tot;
     }
-    int npow = 32;
-    while (npow < (int)C) npow <<= 1;
-    for (int t = (int)C + lane; t < npow; t += 32) s_key[t] = ~0ull;
-    __syncwarp();
-    ss_warp_bitonic(s_key, npow, lane);
-    __syncwarp();
+    ss_sort_keys<true>(s_key, (int)C);
 
-    const int pmax = P.np - 1;
-    float *const tile = A.tiles + (size_t)B.tile * P.np * P.np * P.np;
-    SS_AN_LANE_IJK(lane, li, lj, lk);
+    float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
+    const SsSubLane L = ss_sub_lane(P, lane);
     const float cull2 = P.h2 * 1.0001f;
     for (int b = 0; b < 8; ++b) {
-        const int i0 = B.bx * 8 + 4 * ((b >> 2) & 1), j0 = B.by * 8 + 4 * ((b >> 1) & 1), k0 = B.bz * 8 + 4 * (b & 1);
-        if (i0 > pmax || j0 > pmax || k0 > pmax) continue;
-        const int i = i0 + li, j = j0 + lj, k = k0 + lk;
-        const int gi = B.T.gbase[0] + i, gj = B.T.gbase[1] + j, gk = B.T.gbase[2] + k;
-        // grid point coordinates: point_coordinates (uniform_grid.rs:418-425), min + index * cell
-        const float gx = __fadd_rn(P.gmin[0], __fmul_rn((float)gi, P.c)), gy = __fadd_rn(P.gmin[1], __fmul_rn((float)gj, P.c));
-        const float gzA = __fadd_rn(P.gmin[2], __fmul_rn((float)gk, P.c)), gzB = __fadd_rn(P.gmin[2], __fmul_rn((float)(gk + 1), P.c));
-        // sub-box in world coordinates (culling only: |G d| >= |d| because every eigenvalue of G is >= 1)
-        const int i1 = min(i0 + 3, pmax), j1 = min(j0 + 3, pmax), k1 = min(k0 + 3, pmax);
-        const float bxl = fmaf((float)(B.T.gbase[0] + i0), P.c, P.gmin[0]), bxh = fmaf((float)(B.T.gbase[0] + i1), P.c, P.gmin[0]);
-        const float byl = fmaf((float)(B.T.gbase[1] + j0), P.c, P.gmin[1]), byh = fmaf((float)(B.T.gbase[1] + j1), P.c, P.gmin[1]);
-        const float bzl = fmaf((float)(B.T.gbase[2] + k0), P.c, P.gmin[2]), bzh = fmaf((float)(B.T.gbase[2] + k1), P.c, P.gmin[2]);
+        // grid point coordinates: point_coordinates (uniform_grid.rs:418-425), min + index * cell; culling box: |G d| >= |d|
+        // because every eigenvalue of G is >= 1
+        const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
+        if (!X.inside) continue;
         int nlist = 0;
         for (int w = 0; w < (int)((C + 31) >> 5); ++w) {
             const int rnk = w * 32 + lane;
             bool keep = false;
             if (rnk < (int)C) {
-                const float4 r = A.rec[(uint32_t)s_key[rnk]];
-                keep = ss_axis_d2(r.x, bxl, bxh) + ss_axis_d2(r.y, byl, byh) + ss_axis_d2(r.z, bzl, bzh) < cull2;
+                const float4 r = A.bins.rec[(uint32_t)s_key[rnk]];
+                keep = ss_axis_d2(r.x, X.bxl, X.bxh) + ss_axis_d2(r.y, X.byl, X.byh) + ss_axis_d2(r.z, X.bzl, X.bzh) < cull2;
             }
             const uint32_t mword = __ballot_sync(0xffffffffu, keep);
             if (keep) s_list[nlist + __popc(mword & ((1u << lane) - 1u))] = (uint16_t)rnk;
@@ -288,14 +245,12 @@ __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A
         float phiA = 0.0f, phiB = 0.0f;
         for (int n = 0; n < nlist; ++n) {
             const uint32_t src = (uint32_t)s_key[s_list[n]];
-            const float4 r = A.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
-            phiA = ss_aniso_term(P, r, g0, g1, gx, gy, gzA, phiA);
-            phiB = ss_aniso_term(P, r, g0, g1, gx, gy, gzB, phiB);
+            const float4 r = A.bins.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
+            phiA = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzA, phiA);
+            phiB = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzB, phiB);
         }
-        if (i <= pmax && j <= pmax) {
-            if (k <= pmax) tile[((size_t)i * P.np + j) * P.np + k] = phiA;
-            if (k + 1 <= pmax) tile[((size_t)i * P.np + j) * P.np + k + 1] = phiB;
-        }
+        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = phiA;
+        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = phiB;
         __syncwarp();                                        // the list is rebuilt for the next sub-box
     }
 }
@@ -317,9 +272,8 @@ __global__ void __launch_bounds__(32)
 k_aniso_select(SsDev P, SsAnArgs A) {
     if (blockIdx.x >= A.n_bricks) return;
     const int lane = threadIdx.x & 31;
-    const SsAnBrick B = ss_an_brick(P, A, A.bricks[blockIdx.x]);
-    const int pmax = P.np - 1;
-    SS_AN_LANE_IJK(lane, li, lj, lk);
+    const SsAnBrick N = ss_an_brick(P, A, A.bricks[blockIdx.x]);
+    const SsSubLane L = ss_sub_lane(P, lane);
     float phi[16];
 #pragma unroll
     for (int q = 0; q < 16; ++q) phi[q] = 0.0f;
@@ -327,38 +281,31 @@ k_aniso_select(SsDev P, SsAnArgs A) {
     bool first = true;
     for (;;) {
         unsigned long long best = ~0ull;
-        for (int X = B.rx.x; X <= B.rx.y; ++X) for (int Y = B.ry.x; Y <= B.ry.y; ++Y) {
-            const uint32_t base = B.T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-            for (int Z = B.rz.x; Z <= B.rz.y; ++Z) {
-                const uint32_t st = A.bin_start[base + Z];
-                if (st == 0xffffffffu) continue;
-                const uint32_t en = A.bin_end[base + Z];
-                for (uint32_t t = st + lane; t < en; t += 32) {
-                    const unsigned long long kk = ((unsigned long long)A.pidx[t] << 32) | (unsigned long long)t;
-                    if ((first || kk > last) && kk < best) best = kk;
-                }
+        for (int r = 0; r < N.K.nruns; ++r) {
+            uint32_t a;
+            const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r, a);
+            for (uint32_t t = a + lane; t < a + len; t += 32) {
+                const unsigned long long kk = ((unsigned long long)A.bins.pidx[t] << 32) | (unsigned long long)t;
+                if ((first || kk > last) && kk < best) best = kk;
             }
         }
         for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
         if (best == ~0ull) break;
         last = best; first = false;
         const uint32_t src = (uint32_t)best;
-        const float4 r = A.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
+        const float4 r = A.bins.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
 #pragma unroll
         for (int b = 0; b < 8; ++b) {
-            const int gi = B.T.gbase[0] + B.bx * 8 + 4 * ((b >> 2) & 1) + li, gj = B.T.gbase[1] + B.by * 8 + 4 * ((b >> 1) & 1) + lj;
-            const int gk = B.T.gbase[2] + B.bz * 8 + 4 * (b & 1) + lk;
-            const float gx = __fadd_rn(P.gmin[0], __fmul_rn((float)gi, P.c)), gy = __fadd_rn(P.gmin[1], __fmul_rn((float)gj, P.c));
-            phi[2 * b] = ss_aniso_term(P, r, g0, g1, gx, gy, __fadd_rn(P.gmin[2], __fmul_rn((float)gk, P.c)), phi[2 * b]);
-            phi[2 * b + 1] = ss_aniso_term(P, r, g0, g1, gx, gy, __fadd_rn(P.gmin[2], __fmul_rn((float)(gk + 1), P.c)), phi[2 * b + 1]);
+            const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
+            phi[2 * b] = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzA, phi[2 * b]);
+            phi[2 * b + 1] = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzB, phi[2 * b + 1]);
         }
     }
-    float *const tile = A.tiles + (size_t)B.tile * P.np * P.np * P.np;
+    float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
 #pragma unroll
     for (int b = 0; b < 8; ++b) {
-        const int i = B.bx * 8 + 4 * ((b >> 2) & 1) + li, j = B.by * 8 + 4 * ((b >> 1) & 1) + lj, k = B.bz * 8 + 4 * (b & 1) + lk;
-        if (i > pmax || j > pmax) continue;
-        if (k <= pmax) tile[((size_t)i * P.np + j) * P.np + k] = phi[2 * b];
-        if (k + 1 <= pmax) tile[((size_t)i * P.np + j) * P.np + k + 1] = phi[2 * b + 1];
+        const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
+        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = phi[2 * b];
+        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = phi[2 * b + 1];
     }
 }

@@ -16,10 +16,7 @@
 #pragma once
 
 struct SsCertArgs {
-    const uint32_t *bin_start, *bin_end;
-    const float4 *rec;
-    const SsTile *tile_tab;
-    const int2 *brick_rng;
+    SsBins bins;
     const uint4 *work_desc;      // per listed brick: (linear brick index, tile, bx | by << 10 | bz << 20, 0)
     float *tiles;
     uint8_t *wstate;             // [batch][nb^3][16]
@@ -29,12 +26,8 @@ struct SsCertArgs {
 __global__ void k_compact_desc(SsDev P, const uint32_t *__restrict__ flag, const uint32_t *__restrict__ off, uint32_t n, uint4 *__restrict__ desc) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= n || !flag[b]) return;
-    const uint32_t nb = (uint32_t)P.nb;
-    uint32_t q = b;
-    const uint32_t bz = q % nb; q /= nb;
-    const uint32_t by = q % nb; q /= nb;
-    const uint32_t bx = q % nb; const uint32_t tile = q / nb;
-    desc[off[b]] = make_uint4(b, tile, bx | (by << 10) | (bz << 20), 0u);
+    const SsBrick B = ss_brick_from_lin(P, b);
+    desc[off[b]] = make_uint4(b, (uint32_t)B.tile, (uint32_t)B.bx | ((uint32_t)B.by << 10) | ((uint32_t)B.bz << 20), 0u);
 }
 
 // marks the standard 2x4x4 boxes of brick (vbx, vby, vbz) that the point box W overlaps
@@ -61,37 +54,20 @@ template <bool GLOBAL>
 __global__ void __launch_bounds__(SS_LS_THREADS, 3)
 k_certify(SsDev P, SsCertArgs A) {
     __shared__ float4 s_rec[SS_LS_CAP];
-    const int nb = P.nb;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint4 desc = A.work_desc[blockIdx.x];
     const int tile_idx = (int)desc.y;
     const int bx = (int)(desc.z & 1023u), by = (int)((desc.z >> 10) & 1023u), bz = (int)(desc.z >> 20);
-    const bool ext = P.ext_bricks != 0;
-    const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
-    const SsTile T = A.tile_tab[tile_idx];
+    const SsTile T = A.bins.tile_tab[tile_idx];
 
     // ---- candidate runs (one per lane, host guarantees <= 32 for this variant) and their exclusive prefix, per warp
-    int2 rx = A.brick_rng[bx], ry = A.brick_rng[by], rz = A.brick_rng[bz];
-    if (ex) rx.y = A.brick_rng[bx + 1].y;
-    if (ey) ry.y = A.brick_rng[by + 1].y;
-    if (ez) rz.y = A.brick_rng[bz + 1].y;
-    const int nyr = ry.y - ry.x + 1;
-    const int nruns = (rx.y - rx.x + 1) * nyr;
-    uint32_t run_a = 0, run_len = 0;
-    if (lane < nruns) {
-        const int X = rx.x + lane / nyr, Y = ry.x + lane % nyr;
-        uint32_t a = 0xffffffffu, b = 0;
-        const uint32_t base = T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        for (int Z = rz.x; Z <= rz.y; ++Z) {
-            const uint32_t st = A.bin_start[base + Z];
-            if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
-        }
-        if (a != 0xffffffffu) { run_a = a; run_len = b - a; }
-    }
-    uint32_t incl = run_len;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
-    const uint32_t run_dst = incl - run_len;
-    const int C = (int)__shfl_sync(0xffffffffu, incl, 31);
+    const SsBrickBins K = ss_brick_bins(P, A.bins.brick_rng, bx, by, bz, P.ext_bricks != 0);
+    const bool ex = K.ex, ey = K.ey, ez = K.ez;
+    const int nyr = K.nyr, nruns = K.nruns;
+    uint32_t run_a, total;
+    const uint32_t run_len = ss_brick_run(P, A.bins, T.s, K, lane, run_a);
+    const uint32_t run_dst = ss_warp_excl_scan(run_len, lane, total);
+    const int C = (int)total;
     if (C == 0) return;                                         // tile is pre-zeroed: phi = 0 exactly (wstate stays 0)
 
     const SsWarpBox Wm = { bx * 8 + (warp >> 2) * 2, by * 8 + ((warp >> 1) & 1) * 4, bz * 8 + (warp & 1) * 4, 2, 4, 4 };
@@ -112,7 +88,7 @@ k_certify(SsDev P, SsCertArgs A) {
     for (int r = warp; r < nruns; r += SS_LS_WARPS) {
         const uint32_t a = __shfl_sync(0xffffffffu, run_a, r), len = __shfl_sync(0xffffffffu, run_len, r), dst = __shfl_sync(0xffffffffu, run_dst, r);
         for (uint32_t t = lane; t < len; t += 32) {
-            float4 rc = A.rec[a + t];
+            float4 rc = A.bins.rec[a + t];
             if (GLOBAL) { int im[3]; float d0[3]; if (!ss_global_candidate(P, rc, im, d0)) rc.w = 0.0f; }   // skipped particle: no volume
             s_rec[dst + t] = rc;
         }
@@ -120,7 +96,7 @@ k_certify(SsDev P, SsCertArgs A) {
     // the candidate sweep starts at the run that holds the brick's own bin
     int w0;
     {
-        const int ox = min(max(ss_floor_div(8 * bx, P.be) + P.nlo - rx.x, 0), rx.y - rx.x), oy = min(max(ss_floor_div(8 * by, P.be) + P.nlo - ry.x, 0), nyr - 1);
+        const int ox = min(max(ss_floor_div(8 * bx, P.be) + P.nlo - K.rx.x, 0), K.rx.y - K.rx.x), oy = min(max(ss_floor_div(8 * by, P.be) + P.nlo - K.ry.x, 0), nyr - 1);
         w0 = (int)(__shfl_sync(0xffffffffu, run_dst, ox * nyr + oy) >> 5);
         if (w0 >= ((C + 31) >> 5)) w0 = 0;
     }
@@ -196,10 +172,7 @@ __global__ void k_wstate_reduce(const uint8_t *__restrict__ wstate, uint32_t nbr
 #define SS_CW_MAXRUNS 32               // candidate runs per brick: one per lane
 
 struct SsCwArgs {
-    const uint32_t *bin_start, *bin_end;
-    const float4 *rec;
-    const SsTile *tile_tab;
-    const int2 *brick_rng;
+    SsBins bins;
     const uint4 *work_desc;            // per listed brick: (linear brick index, tile, bx | by << 10 | bz << 20, 0)
     uint32_t n_work;
     float *tiles;
@@ -295,36 +268,18 @@ template <int CAP>
 __device__ __forceinline__ SsCwRuns ss_cw_lookup(const SsDev &P, const SsCwArgs &A, const uint4 desc, int lane) {
     SsCwRuns R;
     R.desc = desc; R.run_a = 0; R.run_len = 0; R.run_dst = 0; R.C = 0;
-    const int nb = P.nb;
     const int tile_idx = (int)desc.y;
     const int bx = (int)(desc.z & 1023u), by = (int)((desc.z >> 10) & 1023u), bz = (int)(desc.z >> 20);
-    const bool ext = P.ext_bricks != 0;
-    const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
-    const uint32_t tile_s = A.tile_tab[tile_idx].s;
+    const uint32_t tile_s = A.bins.tile_tab[tile_idx].s;
     uint8_t *const wst = A.wstate + (size_t)desc.x * SS_LS_WARPS;
 
-    // ---- candidate runs: one per lane, exclusive prefix by shuffles
-    int2 rx = A.brick_rng[bx], ry = A.brick_rng[by], rz = A.brick_rng[bz];
-    if (ex) rx.y = A.brick_rng[bx + 1].y;
-    if (ey) ry.y = A.brick_rng[by + 1].y;
-    if (ez) rz.y = A.brick_rng[bz + 1].y;
-    const int nyr = ry.y - ry.x + 1;
-    const int nruns = (rx.y - rx.x + 1) * nyr;                  // host guarantees <= SS_CW_MAXRUNS for this variant
-    uint32_t run_a = 0, run_len = 0;
-    if (lane < nruns) {
-        const int X = rx.x + lane / nyr, Y = ry.x + lane % nyr;
-        uint32_t a = 0xffffffffu, b = 0;
-        const uint32_t base = tile_s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        for (int Z = rz.x; Z <= rz.y; ++Z) {
-            const uint32_t st = A.bin_start[base + Z];
-            if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
-        }
-        if (a != 0xffffffffu) { run_a = a; run_len = b - a; }
-    }
-    uint32_t incl = run_len;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
-    const uint32_t run_dst = incl - run_len;
-    const int C = (int)__shfl_sync(0xffffffffu, incl, 31);
+    // ---- candidate runs: one per lane (host guarantees <= SS_CW_MAXRUNS for this variant), exclusive prefix by shuffles
+    const SsBrickBins K = ss_brick_bins(P, A.bins.brick_rng, bx, by, bz, P.ext_bricks != 0);
+    const bool ex = K.ex, ey = K.ey, ez = K.ez;
+    uint32_t run_a, total;
+    const uint32_t run_len = ss_brick_run(P, A.bins, tile_s, K, lane, run_a);
+    const uint32_t run_dst = ss_warp_excl_scan(run_len, lane, total);
+    const int C = (int)total;
     if (C == 0) return R;                                       // phi = 0 exactly (wstate stays 0)
 
     if (C > CAP) {
@@ -355,7 +310,7 @@ __device__ __forceinline__ void ss_cw_issue(SsCwSlice<CAP> &S, const SsCwArgs &A
     ss_fence_proxy_async();
     if (lane == 0) ss_mbar_arrive_expect_tx(&S.mbar, (uint32_t)R.C * 16u);
     __syncwarp();
-    if (R.run_len) ss_bulk_g2s(&S.rec[R.run_dst], A.rec + R.run_a, R.run_len * 16u, &S.mbar);
+    if (R.run_len) ss_bulk_g2s(&S.rec[R.run_dst], A.bins.rec + R.run_a, R.run_len * 16u, &S.mbar);
     __syncwarp();
 }
 
@@ -367,7 +322,7 @@ __device__ __forceinline__ unsigned long long ss_cw_brick(const SsDev &P, const 
     const int bx = (int)(desc.z & 1023u), by = (int)((desc.z >> 10) & 1023u), bz = (int)(desc.z >> 20);
     const bool ext = P.ext_bricks != 0;
     const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
-    const SsTile T = A.tile_tab[tile_idx];
+    const SsTile T = A.bins.tile_tab[tile_idx];
     const bool sparse = GLOBAL || T.sparse != 0;
     uint8_t *const wst = A.wstate + (size_t)desc.x * SS_LS_WARPS;
 
@@ -589,11 +544,9 @@ k_zero_untouched(SsDev P, const uint8_t *__restrict__ bstate, const uint32_t *__
     const int lane = threadIdx.x & 31;
     if (b >= nbricks_total || bstate[b] != 0) return;
     const int nb = P.nb;
-    uint32_t q = b;
-    const int bz = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-    const int by = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-    const int bx = (int)(q % (uint32_t)nb);
-    const uint32_t tile = q / (uint32_t)nb;
+    const SsBrick B = ss_brick_from_lin(P, b);
+    const int bx = B.bx, by = B.by, bz = B.bz;
+    const uint32_t tile = (uint32_t)B.tile;
     bool listed = false;
     if (lane < 27) {
         const int x = bx + lane / 9 - 1, y = by + (lane / 3) % 3 - 1, z = bz + lane % 3 - 1;

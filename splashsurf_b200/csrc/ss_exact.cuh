@@ -22,12 +22,7 @@
 #define SS_XW_LIST 224                 // candidates within the support of one 4x4x4 sub-box
 
 struct SsXwArgs {
-    const uint32_t *bin_start, *bin_end;
-    const float4 *rec;
-    const int *ksplit;
-    const uint32_t *pidx;
-    const SsTile *tile_tab;
-    const int2 *brick_rng;
+    SsBins bins;
     const uint32_t *bricks;            // flagged bricks (linear index)
     uint32_t n_bricks;
     const uint8_t *wflag;              // [batch][nb^3][16] boxes that need exact values
@@ -61,22 +56,6 @@ static thread_local __align__(16) unsigned char ss_dyn_smem[sizeof(SsXwSliceBig)
 extern __shared__ __align__(16) unsigned char ss_dyn_smem[];
 #endif
 
-// warp-synchronous bitonic sort of n (power of two) keys in shared memory
-__device__ __forceinline__ void ss_warp_bitonic(unsigned long long *keys, int n, int lane) {
-    for (int k = 2; k <= n; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = lane; t < (n >> 1); t += 32) {
-                const int lo = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-                const int hi = lo | j;
-                const unsigned long long a = keys[lo], b = keys[hi];
-                const bool up = ((lo & k) == 0);
-                if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-            }
-            __syncwarp();
-        }
-    }
-}
-
 // AVX-path kernel (kernel.rs:343-378) of two radii as a pair; every element rounds like ss_kernel_avx
 __device__ __forceinline__ ss_f2 ss_kernel_avx2(const SsDev &P, float ra, float rb) {
     const ss_f2 q = ss_mul2(ss_pack(ra, rb), ss_pack(P.a_hinv, P.a_hinv));
@@ -101,15 +80,9 @@ __device__ __forceinline__ ss_f2 ss_kernel_avx2(const SsDev &P, float ra, float 
 template <bool GLOBAL, bool COUNT, int CAP, int LIST, typename SLICE>
 __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A, SLICE &S, const uint32_t work, const int lane) {
     if (lane == 0) { ss_mbar_init(&S.mbar, 1); ss_mbar_fence_init(); }
-    const int nb = P.nb;
     const uint32_t brick_lin = A.bricks[work];
-    int bx, by, bz, tile_idx;
-    {
-        uint32_t q = brick_lin;
-        bz = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-        by = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-        bx = (int)(q % (uint32_t)nb); tile_idx = (int)(q / (uint32_t)nb);
-    }
+    const SsBrick B = ss_brick_from_lin(P, brick_lin);
+    const int bx = B.bx, by = B.by, bz = B.bz, tile_idx = B.tile;
     // per-box flags of the brick: 16 bytes; sub-box (a, b, c) needs values when either of its two 2x4x4 boxes is flagged
     uint32_t need8 = 0;
     {
@@ -121,38 +94,26 @@ __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A
         }
     }
     if (!need8) return;
-    const SsTile T = A.tile_tab[tile_idx];
+    const SsTile T = A.bins.tile_tab[tile_idx];
     const bool sparse = GLOBAL || T.sparse != 0;
 
-    // ---- candidate runs (FIX mode: no extension planes), one per lane
-    const int2 rx = A.brick_rng[bx], ry = A.brick_rng[by], rz = A.brick_rng[bz];
-    const int nyr = ry.y - ry.x + 1;
-    const int nruns = (rx.y - rx.x + 1) * nyr;                  // host guarantees <= 32 for this variant
-    uint32_t run_a = 0, run_len = 0;
-    if (lane < nruns) {
-        const int X = rx.x + lane / nyr, Y = ry.x + lane % nyr;
-        uint32_t a = 0xffffffffu, b = 0;
-        const uint32_t base = T.s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        for (int Z = rz.x; Z <= rz.y; ++Z) {
-            const uint32_t st = A.bin_start[base + Z];
-            if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
-        }
-        if (a != 0xffffffffu) { run_a = a; run_len = b - a; }
-    }
-    uint32_t incl = run_len;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
-    const uint32_t run_dst = incl - run_len;
-    const int C = (int)__shfl_sync(0xffffffffu, incl, 31);
-    const int pmax = P.np - 1;
+    // ---- candidate runs (FIX mode: no extension planes), one per lane (host guarantees <= 32 for this variant)
+    const SsBrickBins K = ss_brick_bins(P, A.bins.brick_rng, bx, by, bz, false);
+    const int nruns = K.nruns;
+    uint32_t run_a, total;
+    const uint32_t run_len = ss_brick_run(P, A.bins, T.s, K, lane, run_a);
+    const uint32_t run_dst = ss_warp_excl_scan(run_len, lane, total);
+    const int C = (int)total;
     float *const tile = A.tiles + (size_t)tile_idx * P.np * P.np * P.np;
-    const int li = lane >> 3, lj = (lane >> 1) & 3, lk = (lane & 1) * 2;
+    const SsSubLane L = ss_sub_lane(P, lane);
 
     if (C == 0) {
         // nothing in reach: the exact value is 0 (the tile may hold markers from an earlier pass only if C > 0, so this is
         // defensive): store zeros for the requested sub-boxes
         for (int b = 0; b < 8; ++b) {
             if (!(need8 & (1u << b))) continue;
-            const int i = bx * 8 + 4 * ((b >> 2) & 1) + li, j = by * 8 + 4 * ((b >> 1) & 1) + lj, k = bz * 8 + 4 * (b & 1) + lk;
+            const int pmax = P.np - 1;
+            const int i = bx * 8 + 4 * ((b >> 2) & 1) + L.li, j = by * 8 + 4 * ((b >> 1) & 1) + L.lj, k = bz * 8 + 4 * (b & 1) + L.lk;
             if (i <= pmax && j <= pmax) { if (k <= pmax) tile[((size_t)i * P.np + j) * P.np + k] = 0.0f; if (k + 1 <= pmax) tile[((size_t)i * P.np + j) * P.np + k + 1] = 0.0f; }
         }
         return;
@@ -166,19 +127,15 @@ __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A
     __syncwarp();
     if (lane == 0) ss_mbar_arrive_expect_tx(&S.mbar, (uint32_t)C * 16u);
     __syncwarp();
-    if (run_len) ss_bulk_g2s(&S.rec[run_dst], A.rec + run_a, run_len * 16u, &S.mbar);
+    if (run_len) ss_bulk_g2s(&S.rec[run_dst], A.bins.rec + run_a, run_len * 16u, &S.mbar);
     for (int r = 0; r < nruns; ++r) {
         const uint32_t a = __shfl_sync(0xffffffffu, run_a, r), len = __shfl_sync(0xffffffffu, run_len, r), dst = __shfl_sync(0xffffffffu, run_dst, r);
         for (uint32_t t = lane; t < len; t += 32) {
-            S.key[dst + t] = ((unsigned long long)A.pidx[a + t] << 32) | (unsigned long long)(dst + t);
-            S.ks[dst + t] = (uint16_t)max(A.ksplit[a + t], 0);
+            S.key[dst + t] = ((unsigned long long)A.bins.pidx[a + t] << 32) | (unsigned long long)(dst + t);
+            S.ks[dst + t] = (uint16_t)max(A.bins.ksplit[a + t], 0);
         }
     }
-    int npow = 32;
-    while (npow < C) npow <<= 1;
-    for (int t = C + lane; t < npow; t += 32) S.key[t] = ~0ull;
-    __syncwarp();
-    ss_warp_bitonic(S.key, npow, lane);
+    ss_sort_keys<true>(S.key, C);
     ss_mbar_wait(&S.mbar, 0);
     __syncwarp();
 
@@ -186,23 +143,10 @@ __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A
     unsigned hits = 0;
     for (int b = 0; b < 8; ++b) {
         if (!(need8 & (1u << b))) continue;
-        const int ha = (b >> 2) & 1, hb = (b >> 1) & 1, hc = b & 1;
-        const int i0 = bx * 8 + 4 * ha, j0 = by * 8 + 4 * hb, k0 = bz * 8 + 4 * hc;
-        if (i0 > pmax || j0 > pmax || k0 > pmax) continue;
-        const int i = i0 + li, j = j0 + lj, k = k0 + lk;
-        const bool row_ok = i <= pmax && j <= pmax;
-        const bool vA = row_ok && k <= pmax, vB = row_ok && k + 1 <= pmax;
-        const int gi = T.gbase[0] + i, gj = T.gbase[1] + j, gk = T.gbase[2] + k;
-        // grid point coordinates from GLOBAL indices (dense_subdomains.rs:1068, :1101-1102; scalar: uniform_grid.rs:418-425)
-        const float gx = __fadd_rn(__fmul_rn((float)gi, P.c), P.gmin[0]);
-        const float gy = __fadd_rn(__fmul_rn((float)gj, P.c), P.gmin[1]);
-        const float gzA = sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)gk, P.c)) : __fmaf_rn((float)gk, P.c, P.gmin[2]);
-        const float gzB = sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)(gk + 1), P.c)) : __fmaf_rn((float)(gk + 1), P.c, P.gmin[2]);
-        // sub-box in world coordinates (culling only)
-        const int i1 = min(i0 + 3, pmax), j1 = min(j0 + 3, pmax), k1 = min(k0 + 3, pmax);
-        const float bxl = fmaf((float)(T.gbase[0] + i0), P.c, P.gmin[0]), bxh = fmaf((float)(T.gbase[0] + i1), P.c, P.gmin[0]);
-        const float byl = fmaf((float)(T.gbase[1] + j0), P.c, P.gmin[1]), byh = fmaf((float)(T.gbase[1] + j1), P.c, P.gmin[1]);
-        const float bzl = fmaf((float)(T.gbase[2] + k0), P.c, P.gmin[2]), bzh = fmaf((float)(T.gbase[2] + k1), P.c, P.gmin[2]);
+        const SsSubBox X = ss_sub_box(P, T, bx, by, bz, b, L, sparse);
+        if (!X.inside) continue;
+        const int i = X.i, j = X.j, k = X.k, gi = X.gi, gj = X.gj, gk = X.gk, k1 = X.k1;
+        const float gx = X.gx, gy = X.gy, gzA = X.gzA, gzB = X.gzB;
         // ---- candidates within the support of the sub-box, in ascending particle index
         int nlist = 0;
         bool overflow = false;
@@ -213,7 +157,7 @@ __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A
             if (rnk < C) {
                 slot = (int)(S.key[rnk] & 0xffffu);
                 const float4 r = S.rec[slot];
-                keep = ss_axis_d2(r.x, bxl, bxh) + ss_axis_d2(r.y, byl, byh) + ss_axis_d2(r.z, bzl, bzh) < cull2;
+                keep = ss_axis_d2(r.x, X.bxl, X.bxh) + ss_axis_d2(r.y, X.byl, X.byh) + ss_axis_d2(r.z, X.bzl, X.bzh) < cull2;
             }
             const uint32_t mword = __ballot_sync(0xffffffffu, keep);
             const int pos = nlist + __popc(mword & ((1u << lane) - 1u));
@@ -274,8 +218,8 @@ __device__ __forceinline__ void ss_exact_brick(const SsDev &P, const SsXwArgs &A
             }
             ss_unpack(phi, phiA, phiB);
         }
-        if (vA) tile[((size_t)i * P.np + j) * P.np + k] = phiA;
-        if (vB) tile[((size_t)i * P.np + j) * P.np + k + 1] = phiB;
+        if (X.vA) tile[((size_t)i * P.np + j) * P.np + k] = phiA;
+        if (X.vB) tile[((size_t)i * P.np + j) * P.np + k + 1] = phiB;
         __syncwarp();                                           // the list is rebuilt for the next sub-box
     }
     if (COUNT && A.pairs) {

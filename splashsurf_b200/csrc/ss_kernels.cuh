@@ -437,16 +437,10 @@ struct SsTile {
     float smin[3];       // subdomain aabb.min (marching cubes vertex coordinates)
 };
 
+#include "ss_brick.cuh"
+
 struct SsLsArgs {
-    const uint32_t *bin_start;   // [nsub * nbin_sub] run start or 0xffffffff
-    const uint32_t *bin_end;     // [nsub * nbin_sub] run end
-    const float4 *rec;           // bin-sorted records (x, y, z, V)
-    const int *ksplit;
-    const uint32_t *pidx;        // bin-sorted particle indices
-    const uint32_t *sub_flat;    // compressed -> flat
-    const uint8_t *sub_sparse;   // compressed -> sparse flag
-    const SsTile *tile_tab;      // [batch] per-tile constants (host-filled)
-    const int2 *brick_rng;       // [nb] candidate bin range (lo, hi) of brick b along one axis
+    SsBins bins;
     const uint32_t *fix_bricks;  // SS_LS_FIX: list of flagged bricks (global brick index)
     const uint32_t *work_list;   // other modes: list of non-empty bricks to evaluate
     float *tiles;                // [batch][np^3]
@@ -455,22 +449,6 @@ struct SsLsArgs {
     unsigned long long *pairs;   // work counter (in-support evaluations), only with COUNT
     int mode;
 };
-
-// Sorts the staged candidate keys ((pidx << 32) | slot) ascending: bitonic network in shared memory.
-__device__ __forceinline__ void ss_bitonic(unsigned long long *keys, int n /* power of two */) {
-    for (int k = 2; k <= n; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int t = threadIdx.x; t < (n >> 1); t += blockDim.x) {
-                int lo = ((t & ~(j - 1)) << 1) | (t & (j - 1));      // index with bit j clear
-                int hi = lo | j;
-                unsigned long long a = keys[lo], b = keys[hi];
-                bool up = ((lo & k) == 0);
-                if ((a > b) == up) { keys[lo] = b; keys[hi] = a; }
-            }
-            __syncthreads();
-        }
-    }
-}
 
 // One exact accumulation step (the reference's arithmetic) of candidate `r` (x, y, z, V) into phi.
 template <bool SPARSE, bool UNIFORM_FMA>
@@ -727,38 +705,23 @@ k_levelset(SsDev P, SsLsArgs A) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int mode = A.mode;
     const uint32_t brick_lin = (mode == SS_LS_FIX) ? A.fix_bricks[blockIdx.x] : A.work_list[blockIdx.x];
-    int bx, by, bz, tile_idx;
-    {
-        uint32_t q = brick_lin;
-        bz = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-        by = (int)(q % (uint32_t)nb); q /= (uint32_t)nb;
-        bx = (int)(q % (uint32_t)nb); tile_idx = (int)(q / (uint32_t)nb);
-    }
-    const bool ext = P.ext_bricks && mode != SS_LS_FIX;
-    const bool ex = ext && bx == nb - 2, ey = ext && by == nb - 2, ez = ext && bz == nb - 2;
+    const SsBrick B = ss_brick_from_lin(P, brick_lin);
+    const int bx = B.bx, by = B.by, bz = B.bz, tile_idx = B.tile;
     const bool my_flag = (mode != SS_LS_FIX) || (A.wflag[(size_t)brick_lin * SS_LS_WARPS + warp] != 0);
     if (threadIdx.x < 8) s_ext_need[threadIdx.x] = 0;
 
-    const SsTile T = A.tile_tab[tile_idx];
-    const uint32_t s = T.s;
+    const SsTile T = A.bins.tile_tab[tile_idx];
     const bool sparse = GLOBAL || T.sparse != 0;
 
-    // ---- candidate runs: bins overlapping [8b - R, 8b + 7 + R) per axis (+ the extension plane); z contiguous in key order
-    int2 rx = A.brick_rng[bx], ry = A.brick_rng[by], rz = A.brick_rng[bz];
-    if (ex) rx.y = A.brick_rng[bx + 1].y;
-    if (ey) ry.y = A.brick_rng[by + 1].y;
-    if (ez) rz.y = A.brick_rng[bz + 1].y;
-    const int nyr = ry.y - ry.x + 1;
-    const int nruns = (rx.y - rx.x + 1) * nyr;   // host guarantees <= 128
+    // ---- candidate runs (+ the extension plane), one per thread
+    const SsBrickBins K = ss_brick_bins(P, A.bins.brick_rng, bx, by, bz, P.ext_bricks && mode != SS_LS_FIX);
+    const bool ex = K.ex, ey = K.ey, ez = K.ez;
+    const int nyr = K.nyr;
+    const int nruns = K.nruns;                   // host guarantees <= 128
     if ((int)threadIdx.x < nruns) {
-        int X = rx.x + (int)threadIdx.x / nyr, Y = ry.x + (int)threadIdx.x % nyr;
-        uint32_t a = 0xffffffffu, b = 0;
-        uint32_t base = s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        for (int Z = rz.x; Z <= rz.y; ++Z) {
-            uint32_t st = A.bin_start[base + Z];
-            if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[base + Z]; }
-        }
-        s_rng[0][threadIdx.x] = a; s_rng[1][threadIdx.x] = (a == 0xffffffffu) ? 0 : b - a;
+        uint32_t a;
+        const uint32_t len = ss_brick_run(P, A.bins, T.s, K, (int)threadIdx.x, a);
+        s_rng[0][threadIdx.x] = a; s_rng[1][threadIdx.x] = len;
     }
     __syncthreads();
     if (warp == 0) {
@@ -797,7 +760,7 @@ k_levelset(SsDev P, SsLsArgs A) {
                 for (int r = 0; r < nruns; ++r) {
                     uint32_t a = s_rng[0][r], len = s_rng[1][r];
                     for (uint32_t t = lane; t < len; t += 32) {
-                        uint32_t pi = A.pidx[a + t];
+                        uint32_t pi = A.bins.pidx[a + t];
                         if ((long long)pi > last) { unsigned long long kk = ((unsigned long long)pi << 32) | (a + t); if (kk < best) best = kk; }
                     }
                 }
@@ -805,8 +768,8 @@ k_levelset(SsDev P, SsLsArgs A) {
                 if (best == ~0ull) break;
                 last = (long long)(best >> 32);
                 uint32_t src = (uint32_t)(best & 0xffffffffu);
-                float4 r = A.rec[src];
-                int ks = A.ksplit[src];
+                float4 r = A.bins.rec[src];
+                int ks = A.bins.ksplit[src];
                 if (GLOBAL) { int im[3]; float d0[3]; if (ss_global_candidate(P, r, im, d0)) ss_accumulate_global(P, r, im, d0, L.gi, L.gj, L.gk, phi, hits); }
                 else if (sparse) ss_accumulate<true, false>(P, r, ks, L.k, L.gx, L.gy, L.gz, phi, hits);
                 else ss_accumulate<false, false>(P, r, ks, L.k, L.gx, L.gy, L.gz, phi, hits);
@@ -825,10 +788,10 @@ k_levelset(SsDev P, SsLsArgs A) {
         const uint32_t a = s_rng[0][r], len = s_rng[1][r], dst = s_pre[r];
         for (uint32_t t = lane; t < len; t += 32) {
             const uint32_t src = a + t;
-            float4 rc = A.rec[src];
+            float4 rc = A.bins.rec[src];
             if (GLOBAL && !ss_global_candidate(P, rc, s_imin[dst + t], s_dx0[dst + t])) rc.w = 0.0f;   // skipped particle: no volume
-            s_rec[dst + t] = rc; s_ks[dst + t] = A.ksplit[src];
-            s_key[dst + t] = ((unsigned long long)A.pidx[src] << 32) | (dst + t);
+            s_rec[dst + t] = rc; s_ks[dst + t] = A.bins.ksplit[src];
+            s_key[dst + t] = ((unsigned long long)A.bins.pidx[src] << 32) | (dst + t);
         }
     }
     __syncthreads();
@@ -837,7 +800,7 @@ k_levelset(SsDev P, SsLsArgs A) {
     // start the candidate sweep at the run that holds the brick's own bin
     int w0;
     {
-        const int ox = min(max(ss_floor_div(8 * bx, P.be) + P.nlo - rx.x, 0), rx.y - rx.x), oy = min(max(ss_floor_div(8 * by, P.be) + P.nlo - ry.x, 0), nyr - 1);
+        const int ox = min(max(ss_floor_div(8 * bx, P.be) + P.nlo - K.rx.x, 0), K.rx.y - K.rx.x), oy = min(max(ss_floor_div(8 * by, P.be) + P.nlo - K.ry.x, 0), nyr - 1);
         w0 = (int)(s_pre[ox * nyr + oy] >> 5);
         if (w0 >= ((C + 31) >> 5)) w0 = 0;
     }
@@ -870,10 +833,7 @@ k_levelset(SsDev P, SsLsArgs A) {
     }
 
     // ---- exact path: order the candidates by global particle index
-    int npow = 32; while (npow < C) npow <<= 1;
-    for (int t = C + threadIdx.x; t < npow; t += blockDim.x) s_key[t] = ~0ull;
-    __syncthreads();
-    ss_bitonic(s_key, npow);
+    ss_sort_keys<false>(s_key, C);
     for (int pass = 0; pass < 2; ++pass) {
         if (pass == 1 && !has_ext) break;
         const SsLanePoint L = ss_lane_point(P, T, pass ? We : Wm, tile_idx, lane, sparse);
@@ -897,22 +857,14 @@ __global__ void k_brick_worklist(SsDev P, const SsTile *__restrict__ tile_tab, c
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t nb = (uint32_t)P.nb;
     if (b >= ntiles * nb * nb * nb) return;
-    uint32_t q = b;
-    const int bz = (int)(q % nb); q /= nb;
-    const int by = (int)(q % nb); q /= nb;
-    const int bx = (int)(q % nb); const uint32_t tile = q / nb;
-    if (P.ext_bricks && (bx == (int)nb - 1 || by == (int)nb - 1 || bz == (int)nb - 1)) { flag[b] = 0; return; }
-    int2 rx = brick_rng[bx], ry = brick_rng[by], rz = brick_rng[bz];
-    if (P.ext_bricks) {
-        if (bx == (int)nb - 2) rx.y = brick_rng[bx + 1].y;
-        if (by == (int)nb - 2) ry.y = brick_rng[by + 1].y;
-        if (bz == (int)nb - 2) rz.y = brick_rng[bz + 1].y;
-    }
-    const uint32_t s = tile_tab[tile].s;
+    const SsBrick B = ss_brick_from_lin(P, b);
+    if (P.ext_bricks && (B.bx == (int)nb - 1 || B.by == (int)nb - 1 || B.bz == (int)nb - 1)) { flag[b] = 0; return; }
+    const SsBrickBins K = ss_brick_bins(P, brick_rng, B.bx, B.by, B.bz, P.ext_bricks != 0);
+    const uint32_t s = tile_tab[B.tile].s;
     bool any = false;
-    for (int X = rx.x; X <= rx.y && !any; ++X) for (int Y = ry.x; Y <= ry.y && !any; ++Y) {
+    for (int X = K.rx.x; X <= K.rx.y && !any; ++X) for (int Y = K.ry.x; Y <= K.ry.y && !any; ++Y) {
         const uint32_t base = s * (uint32_t)P.nbin_sub + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        for (int Z = rz.x; Z <= rz.y; ++Z) if (bin_start[base + Z] != 0xffffffffu) { any = true; break; }
+        for (int Z = K.rz.x; Z <= K.rz.y; ++Z) if (bin_start[base + Z] != 0xffffffffu) { any = true; break; }
     }
     flag[b] = any ? 1u : 0u;
 }
@@ -922,20 +874,10 @@ __global__ void k_brick_worklist(SsDev P, const SsTile *__restrict__ tile_tab, c
 // per-brick state the level-set kernel records, so that bricks in the bulk (all certified) or in the void (all zero) cost
 // one state lookup instead of a sweep over their 512 grid points.
 #define SS_TP_THREADS 512
-struct SsBrick { int tile, bx, by, bz; uint32_t lin; };
 __device__ __forceinline__ int ss_state_at(const SsDev &P, const uint8_t *__restrict__ bstate, const SsBrick &B, int dx, int dy, int dz) {
     const int x = B.bx + dx, y = B.by + dy, z = B.bz + dz;
     if (x < 0 || y < 0 || z < 0 || x >= P.nb || y >= P.nb || z >= P.nb) return -1;       // outside the tile: no constraint
     return bstate[(((size_t)B.tile * P.nb + x) * P.nb + y) * P.nb + z];
-}
-__device__ __forceinline__ SsBrick ss_brick_from_lin(const SsDev &P, uint32_t lin) {
-    SsBrick B;
-    B.lin = lin;
-    uint32_t q = lin;
-    B.bz = (int)(q % (uint32_t)P.nb); q /= (uint32_t)P.nb;
-    B.by = (int)(q % (uint32_t)P.nb); q /= (uint32_t)P.nb;
-    B.bx = (int)(q % (uint32_t)P.nb); B.tile = (int)(q / (uint32_t)P.nb);
-    return B;
 }
 // the passes run over compacted lists of bricks: blockIdx.x -> list entry
 __device__ __forceinline__ SsBrick ss_brick_of_block(const SsDev &P, const uint32_t *__restrict__ list) {
@@ -1215,8 +1157,7 @@ k_mc_tris(SsDev P, const float *__restrict__ tiles, const uint8_t *__restrict__ 
 struct SsNrmArgs {
     const float *verts; const unsigned long long *vkeys; uint32_t nv;
     const uint32_t *sub_flat; const uint8_t *sub_owned; uint32_t nsub;
-    const uint32_t *bin_start, *bin_end; const float4 *rec; const uint32_t *pidx; const float *rho;
-    const int2 *brick_rng; float sphere_mass; float *normals;
+    SsBins bins; const float *rho; float sphere_mass; float *normals;
 };
 __device__ __forceinline__ float ss_kernel_dq(const SsDev &P, float q) {          // kernel.rs:83-94, constant 3/(4 pi)
     const float k = __fdiv_rn(3.0f, __fmul_rn(4.0f, SS_PI_F));
@@ -1252,25 +1193,19 @@ k_sph_normals(SsDev P, SsNrmArgs A) {
         const float dqdr = __fdiv_rn(2.0f, P.h);
         int2 rng[3];
 #pragma unroll
-        for (int d = 0; d < 3; ++d) { const int lp = g[d] - t[d] * P.S; rng[d] = A.brick_rng[min(lp >> 3, P.nb - 1)]; }
-        const uint32_t base = (uint32_t)found * (uint32_t)P.nbin_sub;
+        for (int d = 0; d < 3; ++d) { const int lp = g[d] - t[d] * P.S; rng[d] = A.bins.brick_rng[min(lp >> 3, P.nb - 1)]; }
         for (int X = rng[0].x; X <= rng[0].y; ++X) for (int Y = rng[1].x; Y <= rng[1].y; ++Y) {
-            uint32_t a = 0xffffffffu, b = 0;
-            const uint32_t row = base + (uint32_t)((X * P.nbin + Y) * P.nbin);
-            for (int Z = rng[2].x; Z <= rng[2].y; ++Z) {
-                const uint32_t st = A.bin_start[row + Z];
-                if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.bin_end[row + Z]; }
-            }
-            if (a == 0xffffffffu) continue;
-            for (uint32_t e = a; e < b; ++e) {
-                const float4 r = A.rec[e];
+            uint32_t a;
+            const uint32_t len = ss_bin_column(P, A.bins.bin_start, A.bins.bin_end, (uint32_t)found, X, Y, rng[2].x, rng[2].y, a);
+            for (uint32_t e = a; e < a + len; ++e) {
+                const float4 r = A.bins.rec[e];
                 const float dx = __fsub_rn(r.x, xi), dy = __fsub_rn(r.y, yi), dz = __fsub_rn(r.z, zi);
                 const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
                 if (!(d2 <= P.h2)) continue;
                 const float rr = __fsqrt_rn(d2);
                 const float q = __fdiv_rn(__fadd_rn(rr, rr), P.h);
                 const float gn = __fmul_rn(__fmul_rn(P.s_sigma, ss_kernel_dq(P, q)), dqdr);
-                const float vol = __fdiv_rn(A.sphere_mass, A.rho[A.pidx[e]]);
+                const float vol = __fdiv_rn(A.sphere_mass, A.rho[A.bins.pidx[e]]);
                 gx = __fadd_rn(gx, __fmul_rn(__fmul_rn(__fdiv_rn(dx, rr), gn), vol));
                 gy = __fadd_rn(gy, __fmul_rn(__fmul_rn(__fdiv_rn(dy, rr), gn), vol));
                 gz = __fadd_rn(gz, __fmul_rn(__fmul_rn(__fdiv_rn(dz, rr), gn), vol));

@@ -23,6 +23,9 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <functional>
+#include <initializer_list>
+#include <type_traits>
 
 // ------------------------------------------------------------------ errors ----
 static thread_local std::string g_last_error;
@@ -110,7 +113,6 @@ struct ss_context {
         sub_flat, sub_off, sub_sparse, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, batch_subs, tiles, vcnt,
         tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
     uint64_t launches = 0;
-    int big_attr_set = 0;            // dynamic shared memory opt-in of k_exact_warp_big done
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
     // the analogue of the reference's ReconstructionWorkspace, workspace.rs:12-79)
@@ -474,10 +476,44 @@ extern "C" int ss_grid_for_reconstruction_f32(ss_context *c, const float *xyz, u
 
 
 // ------------------------------------------------------------------ templated launch helpers ----
+// f(G, C) with G, C std::integral_constant<bool, ...>: the GLOBAL x COUNT instantiation of a kernel for the runtime flags
+template <typename F>
+static void with_global_count(bool global, bool count, F &&f) {
+    if (global) { if (count) f(std::true_type(), std::true_type()); else f(std::true_type(), std::false_type()); }
+    else { if (count) f(std::false_type(), std::true_type()); else f(std::false_type(), std::false_type()); }
+}
+
 static void launch_levelset(ss_context *c, dim3 grid, const SsDev &D, const SsLsArgs &A, bool count, bool global) {
-    void (*kern)(SsDev, SsLsArgs) = global ? (count ? k_levelset<true, true> : k_levelset<false, true>)
-                                           : (count ? k_levelset<true, false> : k_levelset<false, false>);
-    LAUNCH(c, kern, grid, SS_LS_THREADS, D, A);
+    with_global_count(global, count, [&](auto G, auto C) { LAUNCH(c, (k_levelset<C, G>), grid, SS_LS_THREADS, D, A); });
+}
+
+// the splat bins of the last binning stage (context scratch)
+static SsBins context_bins(const ss_context *c) {
+    SsBins B;
+    B.bin_start = c->tab_a.as<uint32_t>(); B.bin_end = c->tab_b.as<uint32_t>(); B.rec = c->rec.as<float4>(); B.ksplit = c->ksplit.as<int>();
+    B.pidx = c->val_a.as<uint32_t>(); B.tile_tab = c->tile_tab.as<SsTile>(); B.brick_rng = c->brick_rng.as<int2>();
+    return B;
+}
+
+// Fallback cascade over a list of n bricks: tier t launches over the bricks tier t - 1 could not take, appending those it cannot
+// take itself to `left` ([0] = count, [1..] = linear brick indices), the next tier's list.  The last tier takes every brick it gets
+// (left = nullptr).  Stops when no brick is left.
+typedef std::function<void(const uint32_t *list, uint32_t n, uint32_t *left)> SsTier;
+static void run_cascade(ss_context *c, const uint32_t *list, uint32_t n, std::initializer_list<SsTier> tiers, uint64_t &ls_launches) {
+    DevBuf *const left_bufs[] = { &c->fallback, &c->fallback2, &c->fallback3 };
+    size_t t = 0;
+    for (const SsTier &tier : tiers) {
+        if (!n) return;
+        if (++t == tiers.size()) { tier(list, n, nullptr); ++ls_launches; return; }
+        DevBuf &left = *left_bufs[t - 1];
+        left.ensure(((size_t)n + 1) * 4);
+        CK(cudaMemsetAsync(left.p, 0, 4, c->stream));
+        tier(list, n, left.as<uint32_t>());
+        ++ls_launches;
+        CK(cudaMemcpyAsync(&n, left.p, 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        list = left.as<uint32_t>() + 1;
+    }
 }
 
 // in-place exclusive scan of the per-particle neighbour counts (n + 1 entries, last = 0) -> CSR offsets; returns the total
@@ -666,56 +702,36 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
     if (!n_bricks) return;
     const bool count = c->count_pairs != 0;
     if (c->ls_variant != 2) { launch_levelset(c, dim3(n_bricks), D, F, count, global_mode); ++ls_launches; return; }
-    cudaStream_t st = c->stream;
-    c->fallback.ensure(((size_t)n_bricks + 1) * 4);
-    CK(cudaMemsetAsync(c->fallback.p, 0, 4, st));
-    SsXwArgs X{};
-    X.bin_start = F.bin_start; X.bin_end = F.bin_end; X.rec = F.rec; X.ksplit = F.ksplit; X.pidx = F.pidx; X.tile_tab = F.tile_tab;
-    X.brick_rng = F.brick_rng; X.bricks = F.fix_bricks; X.n_bricks = n_bricks; X.wflag = F.wflag; X.tiles = F.tiles;
-    X.fallback = c->fallback.as<uint32_t>(); X.pairs = F.pairs;
-    const unsigned grid = (n_bricks + SS_XW_WARPS - 1) / SS_XW_WARPS;
-    if (global_mode) { if (count) LAUNCH(c, (k_exact_warp<true, true>), grid, SS_XW_THREADS, D, X); else LAUNCH(c, (k_exact_warp<true, false>), grid, SS_XW_THREADS, D, X); }
-    else { if (count) LAUNCH(c, (k_exact_warp<false, true>), grid, SS_XW_THREADS, D, X); else LAUNCH(c, (k_exact_warp<false, false>), grid, SS_XW_THREADS, D, X); }
-    ++ls_launches;
-    uint32_t n_fb = 0;
-    CK(cudaMemcpyAsync(&n_fb, c->fallback.p, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    // dense clusters: the same kernel with one warp per CTA and a larger slice -- up to 1024 candidates per brick (27 KB, static;
-    // list: fallback -> leftovers in fallback2), then up to 4096 (108 KB of dynamic shared memory; leftovers in fallback3)
-    for (int stage = 0; stage < 2 && n_fb; ++stage) {
-        DevBuf &in = stage == 0 ? c->fallback : c->fallback2, &left = stage == 0 ? c->fallback2 : c->fallback3;
-        left.ensure(((size_t)n_fb + 1) * 4);
-        CK(cudaMemsetAsync(left.p, 0, 4, st));
-        SsXwArgs Y = X;
-        Y.bricks = in.as<uint32_t>() + 1; Y.n_bricks = n_fb; Y.fallback = left.as<uint32_t>();
-        if (stage == 0) {
-            if (global_mode) { if (count) LAUNCH(c, (k_exact_warp_mid<true, true>), n_fb, 32, D, Y); else LAUNCH(c, (k_exact_warp_mid<true, false>), n_fb, 32, D, Y); }
-            else { if (count) LAUNCH(c, (k_exact_warp_mid<false, true>), n_fb, 32, D, Y); else LAUNCH(c, (k_exact_warp_mid<false, false>), n_fb, 32, D, Y); }
-        } else {
-            const size_t dyn = sizeof(SsXwSliceBig);
-            if (!c->big_attr_set) {
+    const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+        SsXwArgs X{};
+        X.bins = F.bins; X.bricks = list; X.n_bricks = n; X.wflag = F.wflag; X.tiles = F.tiles; X.fallback = left; X.pairs = F.pairs;
+        return X;
+    };
+    // dense clusters: the same kernel with one warp per CTA and a larger slice -- up to 1024 candidates per brick (27 KB, static),
+    // then up to 4096 (108 KB of dynamic shared memory); beyond that k_levelset's O(C^2) selection path (extreme clustering only)
+    run_cascade(c, F.fix_bricks, n_bricks, {
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            with_global_count(global_mode, count, [&](auto G, auto C) {
+                LAUNCH(c, (k_exact_warp<G, C>), (n + SS_XW_WARPS - 1) / SS_XW_WARPS, SS_XW_THREADS, D, args(list, n, left));
+            });
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            with_global_count(global_mode, count, [&](auto G, auto C) { LAUNCH(c, (k_exact_warp_mid<G, C>), n, 32, D, args(list, n, left)); });
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            with_global_count(global_mode, count, [&](auto G, auto C) {
 #ifndef SS_HOST_EMUL
-                CK(cudaFuncSetAttribute(k_exact_warp_big<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-                CK(cudaFuncSetAttribute(k_exact_warp_big<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-                CK(cudaFuncSetAttribute(k_exact_warp_big<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-                CK(cudaFuncSetAttribute(k_exact_warp_big<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+                CK(cudaFuncSetAttribute(k_exact_warp_big<G, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SsXwSliceBig)));
 #endif
-                c->big_attr_set = 1;
-            }
-            if (global_mode) { if (count) LAUNCH_DYN(c, (k_exact_warp_big<true, true>), n_fb, 32, dyn, D, Y); else LAUNCH_DYN(c, (k_exact_warp_big<true, false>), n_fb, 32, dyn, D, Y); }
-            else { if (count) LAUNCH_DYN(c, (k_exact_warp_big<false, true>), n_fb, 32, dyn, D, Y); else LAUNCH_DYN(c, (k_exact_warp_big<false, false>), n_fb, 32, dyn, D, Y); }
-        }
-        ++ls_launches;
-        CK(cudaMemcpyAsync(&n_fb, left.p, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    if (n_fb) {
-        // beyond 4096 candidates: k_levelset's O(C^2) selection path (extreme clustering only)
-        SsLsArgs G = F;
-        G.fix_bricks = c->fallback3.as<uint32_t>() + 1;
-        launch_levelset(c, dim3(n_fb), D, G, count, global_mode);
-        ++ls_launches;
-    }
+                LAUNCH_DYN(c, (k_exact_warp_big<G, C>), n, 32, sizeof(SsXwSliceBig), D, args(list, n, left));
+            });
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *) {
+            SsLsArgs G = F;
+            G.fix_bricks = list;
+            launch_levelset(c, dim3(n), D, G, count, global_mode);
+        },
+    }, ls_launches);
 }
 
 // Anisotropic level set of one batch (ss_aniso.cuh): work list of non-empty bricks without extension tasks (the single-point
@@ -725,35 +741,19 @@ static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nb
     SsDev Dw = D;
     Dw.ext_bricks = 0;
     const uint32_t n_work = build_worklist(c, Dw, nbatch);
-    if (!n_work) return 0;
-    cudaStream_t st = c->stream;
-    SsAnArgs A{};
-    A.bin_start = c->tab_a.as<uint32_t>(); A.bin_end = c->tab_b.as<uint32_t>(); A.rec = c->rec.as<float4>(); A.grec = c->an_grec.as<float4>();
-    A.pidx = c->val_a.as<uint32_t>(); A.tile_tab = c->tile_tab.as<SsTile>(); A.brick_rng = c->brick_rng.as<int2>();
-    A.bricks = c->list_ls.as<uint32_t>(); A.n_bricks = n_work; A.tiles = c->tiles.as<float>(); A.bstate = c->bstate.as<uint8_t>();
-    c->fallback.ensure(((size_t)n_work + 1) * 4);
-    CK(cudaMemsetAsync(c->fallback.p, 0, 4, st));
-    A.fallback = c->fallback.as<uint32_t>();
-    LAUNCH(c, (k_aniso_levelset<SS_AN_CAP, SS_AN_WARPS>), (n_work + SS_AN_WARPS - 1) / SS_AN_WARPS, SS_AN_WARPS * 32, Dw, A);
-    ++ls_launches;
-    uint32_t n_fb = 0;
-    CK(cudaMemcpyAsync(&n_fb, c->fallback.p, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (n_fb) {
-        c->fallback2.ensure(((size_t)n_fb + 1) * 4);
-        CK(cudaMemsetAsync(c->fallback2.p, 0, 4, st));
-        SsAnArgs B = A;
-        B.bricks = c->fallback.as<uint32_t>() + 1; B.n_bricks = n_fb; B.bstate = nullptr; B.fallback = c->fallback2.as<uint32_t>();
-        LAUNCH(c, (k_aniso_levelset<SS_AN_BIG_CAP, 1>), n_fb, 32, Dw, B);
-        ++ls_launches;
-        CK(cudaMemcpyAsync(&n_fb, c->fallback2.p, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        if (n_fb) {
-            B.bricks = c->fallback2.as<uint32_t>() + 1; B.n_bricks = n_fb; B.fallback = nullptr;
-            LAUNCH(c, k_aniso_select, n_fb, 32, Dw, B);
-            ++ls_launches;
-        }
-    }
+    const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left, uint8_t *bstate) {
+        SsAnArgs A{};
+        A.bins = context_bins(c); A.grec = c->an_grec.as<float4>(); A.bricks = list; A.n_bricks = n; A.tiles = c->tiles.as<float>();
+        A.bstate = bstate; A.fallback = left;
+        return A;
+    };
+    run_cascade(c, c->list_ls.as<uint32_t>(), n_work, {
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            LAUNCH(c, (k_aniso_levelset<SS_AN_CAP, SS_AN_WARPS>), (n + SS_AN_WARPS - 1) / SS_AN_WARPS, SS_AN_WARPS * 32, Dw, args(list, n, left, c->bstate.as<uint8_t>()));
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_aniso_levelset<SS_AN_BIG_CAP, 1>), n, 32, Dw, args(list, n, left, nullptr)); },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_aniso_select, n, 32, Dw, args(list, n, left, nullptr)); },
+    }, ls_launches);
     return n_work;
 }
 
@@ -764,9 +764,7 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
                           ss_surface *out, uint64_t &ls_launches, uint64_t &fix_points, uint32_t *n_mc_out) {
     cudaStream_t st = c->stream;
     SsLsArgs A{};
-    A.bin_start = c->tab_a.as<uint32_t>(); A.bin_end = c->tab_b.as<uint32_t>(); A.rec = c->rec.as<float4>();
-    A.ksplit = c->ksplit.as<int>(); A.pidx = c->val_a.as<uint32_t>();
-    A.tile_tab = c->tile_tab.as<SsTile>(); A.brick_rng = c->brick_rng.as<int2>(); A.tiles = c->tiles.as<float>();
+    A.bins = context_bins(c); A.tiles = c->tiles.as<float>();
     A.pairs = c->count_pairs ? c->pairs.as<unsigned long long>() : nullptr;
     A.mode = exact_all ? SS_LS_EXACT_ALL : SS_LS_CERTIFY;
     A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = c->bstate.as<uint8_t>();
@@ -782,13 +780,11 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
         CK(cudaMemsetAsync(c->wstate.p, 0, (size_t)nbr_c * SS_LS_WARPS, st));
         LAUNCH(c, k_compact_desc, nblk(nbr_c, 256), 256, D, c->flag_ls.as<uint32_t>(), c->off_ls.as<uint32_t>(), nbr_c, c->desc_ls.as<uint4>());
         SsCertArgs CA{};
-        CA.bin_start = A.bin_start; CA.bin_end = A.bin_end; CA.rec = A.rec; CA.tile_tab = A.tile_tab; CA.brick_rng = A.brick_rng;
-        CA.work_desc = c->desc_ls.as<uint4>(); CA.tiles = A.tiles; CA.wstate = c->wstate.as<uint8_t>();
+        CA.bins = A.bins; CA.work_desc = c->desc_ls.as<uint4>(); CA.tiles = A.tiles; CA.wstate = c->wstate.as<uint8_t>();
         if (c->ls_variant == 2) {
             // warp-per-brick certification: TMA-staged candidates, paired FP32 (ss_certify.cuh, variant 2)
             SsCwArgs W{};
-            W.bin_start = A.bin_start; W.bin_end = A.bin_end; W.rec = A.rec; W.tile_tab = A.tile_tab; W.brick_rng = A.brick_rng;
-            W.work_desc = c->desc_ls.as<uint4>(); W.n_work = n_work; W.tiles = A.tiles; W.wstate = c->wstate.as<uint8_t>();
+            W.bins = A.bins; W.work_desc = c->desc_ls.as<uint4>(); W.n_work = n_work; W.tiles = A.tiles; W.wstate = c->wstate.as<uint8_t>();
             W.evals = c->count_pairs ? c->pairs.as<unsigned long long>() + 1 : nullptr;
             c->nflag.ensure(8);                                  // work-list counter of the persistent warps (the fix-up sweep re-zeroes it)
             CK(cudaMemsetAsync(c->nflag.p, 0, 4, st));
@@ -800,11 +796,10 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
             // persistent warps: one wave of CTAs (20 warps per SM), fewer when the work list is short
             const unsigned grid_s = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * (20 / SS_CW_WARPS_S), (n_work + SS_CW_WARPS_S - 1) / SS_CW_WARPS_S);
             const unsigned grid_l = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * (20 / SS_CW_WARPS_L), (n_work + SS_CW_WARPS_L - 1) / SS_CW_WARPS_L);
-#define SS_CW_GO(G_, C_) do { if (cw_small) LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_S, SS_CW_WARPS_S>), grid_s, SS_CW_WARPS_S * 32, D, W); \
-                                 else LAUNCH(c, (k_certify_warp<G_, C_, SS_CW_CAP_L, SS_CW_WARPS_L>), grid_l, SS_CW_WARPS_L * 32, D, W); } while (0)
-            if (global_mode) { if (c->count_pairs) SS_CW_GO(true, true); else SS_CW_GO(true, false); }
-            else { if (c->count_pairs) SS_CW_GO(false, true); else SS_CW_GO(false, false); }
-#undef SS_CW_GO
+            with_global_count(global_mode, c->count_pairs != 0, [&](auto G, auto C) {
+                if (cw_small) LAUNCH(c, (k_certify_warp<G, C, SS_CW_CAP_S, SS_CW_WARPS_S>), grid_s, SS_CW_WARPS_S * 32, D, W);
+                else LAUNCH(c, (k_certify_warp<G, C, SS_CW_CAP_L, SS_CW_WARPS_L>), grid_l, SS_CW_WARPS_L * 32, D, W);
+            });
         } else if (global_mode) LAUNCH(c, k_certify<true>, n_work, SS_LS_THREADS, D, CA);
         else LAUNCH(c, k_certify<false>, n_work, SS_LS_THREADS, D, CA);
         ++ls_launches;
@@ -1293,8 +1288,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         SsNrmArgs NA{};
         NA.verts = out->verts.as<float>(); NA.vkeys = out->vkeys.as<unsigned long long>(); NA.nv = (uint32_t)nv_final;
         NA.sub_flat = c->sub_flat.as<uint32_t>(); NA.sub_owned = part.enabled ? c->sub_owned.as<uint8_t>() : nullptr; NA.nsub = nsub;
-        NA.bin_start = c->tab_a.as<uint32_t>(); NA.bin_end = c->tab_b.as<uint32_t>(); NA.rec = c->rec.as<float4>(); NA.pidx = c->val_a.as<uint32_t>();
-        NA.rho = d_rho; NA.brick_rng = c->brick_rng.as<int2>();
+        NA.bins = context_bins(c); NA.rho = d_rho;
         const float r3 = fmulr(fmulr(p->particle_radius, p->particle_radius), p->particle_radius);
         const float frac_pi_3 = 1.04719755119659774615f;
         NA.sphere_mass = fmulr(fmulr(fmulr(4.0f, frac_pi_3), r3), p->rest_density);
@@ -1388,9 +1382,7 @@ extern "C" int ss_levelset_tile_f32(ss_context *c, const float *xyz, const float
             CK(cudaMemcpyAsync(c->tile_tab.p, &T, sizeof(SsTile), cudaMemcpyHostToDevice, st));
             CK(cudaMemcpyAsync(c->brick_rng.p, h_rng.data(), (size_t)D.nb * sizeof(int2), cudaMemcpyHostToDevice, st));
             SsLsArgs A{};
-            A.bin_start = c->tab_a.as<uint32_t>(); A.bin_end = c->tab_b.as<uint32_t>(); A.rec = c->rec.as<float4>();
-            A.ksplit = c->ksplit.as<int>(); A.pidx = c->val_a.as<uint32_t>();
-            A.tile_tab = c->tile_tab.as<SsTile>(); A.brick_rng = c->brick_rng.as<int2>(); A.tiles = c->tiles.as<float>();
+            A.bins = context_bins(c); A.tiles = c->tiles.as<float>();
             A.pairs = nullptr; A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = nullptr; A.mode = SS_LS_EXACT_ALL;
             const uint32_t n_work = build_worklist(c, D, 1);
             A.work_list = c->list_ls.as<uint32_t>();

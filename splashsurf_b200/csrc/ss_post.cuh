@@ -47,16 +47,10 @@ __device__ __forceinline__ void ss_particles_near(const SsDev &P, const SsQuery 
         b0[d] = min(max((int)floorf((u - reach) / (float)P.be) + P.nlo, 0), P.nbin - 1);
         b1[d] = min(max((int)floorf((u + reach) / (float)P.be) + P.nlo, 0), P.nbin - 1);
     }
-    const uint32_t base = lo * (uint32_t)P.nbin_sub;
     for (int X = b0[0]; X <= b1[0]; ++X) for (int Y = b0[1]; Y <= b1[1]; ++Y) {
-        const uint32_t row = base + (uint32_t)((X * P.nbin + Y) * P.nbin);
-        uint32_t a = 0xffffffffu, b = 0;                          // bins along z are contiguous in the sorted records
-        for (int Z = b0[2]; Z <= b1[2]; ++Z) {
-            const uint32_t st = Q.bin_start[row + Z];
-            if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = Q.bin_end[row + Z]; }
-        }
-        if (a == 0xffffffffu) continue;
-        for (uint32_t e = a; e < b; ++e) visit(e, Q.rec[e]);
+        uint32_t a;
+        const uint32_t len = ss_bin_column(P, Q.bin_start, Q.bin_end, lo, X, Y, b0[2], b1[2], a);
+        for (uint32_t e = a; e < a + len; ++e) visit(e, Q.rec[e]);
     }
 }
 
