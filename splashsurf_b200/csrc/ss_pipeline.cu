@@ -34,13 +34,39 @@ static int ss_fail(int code, const std::string &msg) { g_last_error = msg; retur
 struct SsCudaError { cudaError_t e; const char *what; const char *file; int line; };
 #define CK(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) throw SsCudaError{ _e, #call, __FILE__, __LINE__ }; } while (0)
 
+// Runs an entry's body and turns a failure it throws into the entry's status: a CUDA error is cleared from the runtime and
+// reported with its call site, a failed device or host allocation as SS_ERR_OUT_OF_MEMORY.
+template <typename F>
+static int ss_guard(F &&body) {
+    try {
+        return body();
+    } catch (const SsCudaError &err) {
+        cudaGetLastError();
+        char buf[512];
+        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
+        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
+    } catch (const std::bad_alloc &) {
+        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
+    }
+}
+
 // ------------------------------------------------------------------ device buffers ----
 // Growth slack of the pooled buffers in eighths of the request: 1 (12.5 %) for whole-domain runs; partitioned (multi-GPU) runs use 4
 // (50 %), because the slab plan -- and with it every per-rank size -- moves a little from frame to frame while it balances, and
 // re-allocating the scratch costs far more than the memory it saves (each rank holds 1/N of the data anyway).
 static int g_devbuf_slack_eighths = 1;
+// A device allocation with one owner: freed when the owner goes, handed on with std::move / std::swap.
 struct DevBuf {
     void *p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+        return *this;
+    }
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { release(); }
     template <typename T> T *as() const { return (T *)p; }
     void ensure(size_t bytes) {
 #ifdef SS_EMUL_GUARD                      // tests/emul: exact-size allocations in front of a guard page (overrun detection)
@@ -86,7 +112,6 @@ struct PostScratch {
     uint32_t nsub = 0, M = 0;
     float sphere_mass = 0.f;         // 4/3 pi r^3 rho0 (reconstruct.rs:1126-1129)
     DevBuf keys_a, keys_b, flag, scan, vals, out, tmpv;
-    void release_all() { for (DevBuf *b : { &keys_a, &keys_b, &flag, &scan, &vals, &out, &tmpv }) b->release(); }
 };
 
 struct ss_context {
@@ -110,7 +135,7 @@ struct ss_context {
     cudaEvent_t ev_an[2] = { nullptr, nullptr };
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
-        sub_flat, sub_off, sub_sparse, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, batch_subs, tiles, vcnt,
+        sub_flat, sub_off, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, tiles, vcnt,
         tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
@@ -205,27 +230,51 @@ static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t -
 #endif
 #define LAUNCH_DYN(ctx, kern, grid, block, smem, ...) do { SS_LAUNCH_DYN(kern, grid, block, smem, (ctx)->stream, __VA_ARGS__); (ctx)->launches++; } while (0)
 
-static void cub_sort_pairs(ss_context *c, const uint32_t *kin, uint32_t *kout, const uint32_t *vin, uint32_t *vout,
-                           uint32_t n, int end_bit) {
-    size_t tmp = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kin, kout, vin, vout, (int)n, 0, end_bit, c->stream));
-    c->cub_tmp.ensure(tmp);
-    CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tmp, kin, kout, vin, vout, (int)n, 0, end_bit, c->stream));
+// Radix sort of n keys on bits [0, end_bit), carrying the values vin -> vout when given (V = void: keys only).
+template <typename K, typename V = void>
+static void cub_sort(ss_context *c, const K *kin, K *kout, uint32_t n, int end_bit, const V *vin = nullptr, V *vout = nullptr) {
+    const auto cub_radix_sort = [&](void *tmp, size_t &bytes) {
+        if constexpr (std::is_void<V>::value) return cub::DeviceRadixSort::SortKeys(tmp, bytes, kin, kout, (int)n, 0, end_bit, c->stream);
+        else return cub::DeviceRadixSort::SortPairs(tmp, bytes, kin, kout, vin, vout, (int)n, 0, end_bit, c->stream);
+    };
+    size_t bytes = 0;
+    CK(cub_radix_sort(nullptr, bytes));
+    c->cub_tmp.ensure(bytes);
+    CK(cub_radix_sort(c->cub_tmp.p, bytes));
     c->launches += 1 + (uint64_t)((end_bit + 7) / 8) * 2;   // upsweep/onesweep histogram + per-digit passes (approx.)
 }
-static void cub_excl_scan(ss_context *c, const uint32_t *in, uint32_t *out, uint32_t n) {
-    size_t tmp = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, in, out, (int)n, c->stream));
-    c->cub_tmp.ensure(tmp);
-    CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tmp, in, out, (int)n, c->stream));
+// Exclusive (or inclusive) prefix sum of n entries.
+template <bool INCLUSIVE = false, typename In, typename Out>
+static void cub_scan(ss_context *c, In in, Out out, uint64_t n) {
+    const auto cub_device_scan = [&](void *tmp, size_t &bytes) {
+        if constexpr (INCLUSIVE) return cub::DeviceScan::InclusiveSum(tmp, bytes, in, out, (int)n, c->stream);
+        else return cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, (int)n, c->stream);
+    };
+    size_t bytes = 0;
+    CK(cub_device_scan(nullptr, bytes));
+    c->cub_tmp.ensure(bytes);
+    CK(cub_device_scan(c->cub_tmp.p, bytes));
     c->launches += 2;
 }
-static void cub_incl_scan(ss_context *c, const uint32_t *in, uint32_t *out, uint32_t n) {
-    size_t tmp = 0;
-    CK(cub::DeviceScan::InclusiveSum(nullptr, tmp, in, out, (int)n, c->stream));
-    c->cub_tmp.ensure(tmp);
-    CK(cub::DeviceScan::InclusiveSum(c->cub_tmp.p, tmp, in, out, (int)n, c->stream));
-    c->launches += 2;
+// Exclusive scan of n >= 1 entries, and the read-back of its total out[n - 1] + in[n - 1] into last[0] + last[1]: the caller adds
+// them after its next synchronisation of the stream.
+static void scan_with_total(ss_context *c, const uint32_t *in, uint32_t *out, uint32_t n, uint32_t last[2]) {
+    cub_scan(c, in, out, n);
+    CK(cudaMemcpyAsync(&last[0], out + (n - 1), 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(&last[1], in + (n - 1), 4, cudaMemcpyDeviceToHost, c->stream));
+}
+// ... synchronised: returns the total
+static uint64_t scan_total(ss_context *c, const uint32_t *in, uint32_t *out, uint32_t n) {
+    uint32_t last[2] = { 0, 0 };
+    scan_with_total(c, in, out, n, last);
+    CK(cudaStreamSynchronize(c->stream));
+    return (uint64_t)last[0] + last[1];
+}
+// Exclusive scan of n 0/1 flags and the list of the flagged indices (k_compact_list); `last` as in scan_with_total, if given.
+static void scan_compact(ss_context *c, const uint32_t *flag, uint32_t *off, uint32_t n, uint32_t *list, uint32_t *last = nullptr) {
+    if (last) scan_with_total(c, flag, off, n, last);
+    else cub_scan(c, flag, off, n);
+    LAUNCH(c, k_compact_list, nblk(n, 256), 256, flag, off, n, list);
 }
 static int bits_for(uint64_t maxval) { int b = 1; while (b < 64 && (maxval >> b)) ++b; return b; }
 
@@ -240,7 +289,7 @@ extern "C" int ss_context_create(int device, ss_context **out) {
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)
         return ss_fail(SS_ERR_NO_DEVICE, std::string("no CUDA device available (") + cudaGetErrorString(e) + "); this library has no CPU path");
-    try {
+    return ss_guard([&]() -> int {
         if (device < 0) CK(cudaGetDevice(&device));
         if (device >= ndev) return ss_fail(SS_ERR_INVALID_PARAMETER, "device index out of range");
         CK(cudaSetDevice(device));
@@ -264,23 +313,14 @@ extern "C" int ss_context_create(int device, ss_context **out) {
         { std::lock_guard<std::mutex> lk(g_ctx_mutex); g_live_contexts.insert(c); }
         *out = c;
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        return ss_fail(SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 extern "C" void ss_context_destroy(ss_context *c) {
     if (!c) return;
     { std::lock_guard<std::mutex> lk(g_ctx_mutex); g_live_contexts.erase(c); }
     cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->stream);
-    DevBuf *bufs[] = { &c->xyz, &c->xyz_f, &c->filt_flag, &c->filt_flag32, &c->filt_off, &c->aabb, &c->cnt, &c->off, &c->key_a, &c->key_b,
-                       &c->val_a, &c->val_b, &c->cid, &c->cub_tmp, &c->sub_flat, &c->sub_off, &c->sub_sparse, &c->sub_owned, &c->gkey_a, &c->gkey_b, &c->gval_a, &c->gval_b, &c->flags, &c->scan,
-                       &c->spos, &c->rho, &c->tab_a, &c->tab_b, &c->rec, &c->ksplit, &c->batch_subs, &c->tiles, &c->vcnt, &c->tcnt,
-                       &c->vmask, &c->voff, &c->vblk_off, &c->tblk_off, &c->tile_tab, &c->brick_rng, &c->bstate, &c->flag_ls, &c->off_ls, &c->list_ls, &c->flag_mc, &c->flag_fix, &c->off_mc, &c->off_fix, &c->list_mc, &c->list_fix, &c->wflag, &c->wstate, &c->desc_ls, &c->dflag, &c->doff, &c->dlist, &c->fallback, &c->fallback2, &c->fallback3, &c->pack_cnt, &c->pack_off, &c->brick_seen, &c->fix_list, &c->nflag, &c->bkeys_a, &c->bkeys_b, &c->bids_a, &c->bids_b, &c->bcount, &c->remap, &c->keep, &c->newid,
-                       &c->err, &c->pairs, &c->an_det, &c->an_grec, &c->o_verts, &c->o_tris, &c->o_vkeys, &c->o_rho, &c->o_verts2, &c->o_vkeys2, &c->o_normals };
-    for (DevBuf *b : bufs) b->release();
-    c->post.release_all();
+    cudaStreamSynchronize(c->stream);                  // the device buffers are freed with the context below
     for (auto &ev : c->ev) cudaEventDestroy(ev);
     for (auto &ev : c->ev_stage) if (ev) cudaEventDestroy(ev);
     for (auto &ev : c->ev_an) if (ev) cudaEventDestroy(ev);
@@ -407,12 +447,7 @@ static int prepare_particles(ss_context *c, const float *xyz, uint64_t n_in, con
         float3 mn = make_float3(p->particle_aabb_min[0], p->particle_aabb_min[1], p->particle_aabb_min[2]);
         float3 mx = make_float3(p->particle_aabb_max[0], p->particle_aabb_max[1], p->particle_aabb_max[2]);
         LAUNCH(c, k_filter_flags, nblk(n_in, 256), 256, d_in, n_in, mn, mx, c->filt_flag.as<uint8_t>(), c->filt_flag32.as<uint32_t>());
-        cub_excl_scan(c, c->filt_flag32.as<uint32_t>(), c->filt_off.as<uint32_t>(), (uint32_t)n_in);
-        uint32_t last_off = 0, last_flag = 0;
-        CK(cudaMemcpyAsync(&last_off, c->filt_off.as<uint32_t>() + (n_in - 1), 4, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaMemcpyAsync(&last_flag, c->filt_flag32.as<uint32_t>() + (n_in - 1), 4, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaStreamSynchronize(c->stream));
-        uint64_t nf = (uint64_t)last_off + last_flag;
+        const uint64_t nf = scan_total(c, c->filt_flag32.as<uint32_t>(), c->filt_off.as<uint32_t>(), (uint32_t)n_in);
         c->xyz_f.ensure(std::max<uint64_t>(nf, 1) * 12);
         LAUNCH(c, k_filter_scatter, nblk(n_in, 256), 256, d_in, n_in, c->filt_flag.as<uint8_t>(), c->filt_off.as<uint32_t>(), c->xyz_f.as<float>());
         P.d_xyz = c->xyz_f.as<float>(); P.n = nf;
@@ -461,17 +496,14 @@ extern "C" int ss_grid_for_reconstruction_f32(ss_context *c, const float *xyz, u
     if (!c || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     int rc = validate_params(p);
     if (rc) return rc;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         Prepared P;
-        rc = prepare_particles(c, xyz, n, p, P, nullptr);
+        const int rc = prepare_particles(c, xyz, n, p, P, nullptr);
         if (rc) return rc;
         grid_to_abi(P.grid, out);
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA,
-                       std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 
@@ -518,11 +550,7 @@ static void run_cascade(ss_context *c, const uint32_t *list, uint32_t n, std::in
 
 // in-place exclusive scan of the per-particle neighbour counts (n + 1 entries, last = 0) -> CSR offsets; returns the total
 static uint64_t scan_neighbor_counts(ss_context *c, unsigned long long *cnt, uint64_t n) {
-    size_t tmp = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, cnt, (int)(n + 1), c->stream));
-    c->cub_tmp.ensure(tmp);
-    CK(cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tmp, cnt, cnt, (int)(n + 1), c->stream));
-    c->launches += 2;
+    cub_scan(c, cnt, cnt, n + 1);
     unsigned long long total = 0;
     CK(cudaMemcpyAsync(&total, cnt + n, 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
@@ -534,13 +562,35 @@ static uint32_t build_worklist(ss_context *c, const SsDev &D, uint32_t ntiles) {
     const uint32_t nbr = ntiles * (uint32_t)(D.nb * D.nb * D.nb);
     c->flag_ls.ensure((size_t)nbr * 4); c->off_ls.ensure((size_t)nbr * 4 + 4); c->list_ls.ensure((size_t)nbr * 4);
     LAUNCH(c, k_brick_worklist, nblk(nbr, 256), 256, D, c->tile_tab.as<SsTile>(), c->brick_rng.as<int2>(), c->tab_a.as<uint32_t>(), ntiles, c->flag_ls.as<uint32_t>());
-    cub_excl_scan(c, c->flag_ls.as<uint32_t>(), c->off_ls.as<uint32_t>(), nbr);
-    LAUNCH(c, k_compact_list, nblk(nbr, 256), 256, c->flag_ls.as<uint32_t>(), c->off_ls.as<uint32_t>(), nbr, c->list_ls.as<uint32_t>());
     uint32_t lc[2] = { 0, 0 };
-    CK(cudaMemcpyAsync(&lc[0], c->off_ls.as<uint32_t>() + (nbr - 1), 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(&lc[1], c->flag_ls.as<uint32_t>() + (nbr - 1), 4, cudaMemcpyDeviceToHost, c->stream));
+    scan_compact(c, c->flag_ls.as<uint32_t>(), c->off_ls.as<uint32_t>(), nbr, c->list_ls.as<uint32_t>(), lc);
     CK(cudaStreamSynchronize(c->stream));
     return lc[0] + lc[1];
+}
+
+// Candidate bin range of each brick along one axis (bins overlapping [8b - R, 8b + 7 + R)) -> c->brick_rng.
+static void upload_brick_ranges(ss_context *c, const SsDev &D) {
+    std::vector<int2> h_rng(D.nb);
+    for (int bb = 0; bb < D.nb; ++bb) {
+        h_rng[bb].x = std::max(ss_floor_div(8 * bb - D.R, D.be) + D.nlo, 0);
+        h_rng[bb].y = std::min(ss_floor_div(8 * bb + 6 + D.R, D.be) + D.nlo, D.nbin - 1);
+    }
+    c->brick_rng.ensure((size_t)D.nb * sizeof(int2));
+    CK(cudaMemcpyAsync(c->brick_rng.p, h_rng.data(), (size_t)D.nb * sizeof(int2), cudaMemcpyHostToDevice, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+}
+
+// (i, j, k) of the flat index f of a subdomain in a grid of nsd subdomains (k fastest).
+static void subdomain_ijk(int64_t f, const int64_t nsd[3], int64_t ijk[3]) {
+    ijk[0] = f / (nsd[1] * nsd[2]); ijk[1] = (f - ijk[0] * nsd[1] * nsd[2]) / nsd[2]; ijk[2] = f - ijk[0] * nsd[1] * nsd[2] - ijk[1] * nsd[2];
+}
+
+// The tile of subdomain ijk (S cubes per axis, `sub_size` = c * S): its first global grid point and lower corner.
+static SsTile make_tile(const int64_t ijk[3], int64_t S, const float gmin[3], float sub_size, uint32_t s, bool sparse) {
+    SsTile T{};
+    for (int d = 0; d < 3; ++d) { T.gbase[d] = (int)(ijk[d] * S); T.smin[d] = faddr(gmin[d], fmulr((float)ijk[d], sub_size)); }
+    T.s = s; T.sparse = sparse ? 1u : 0u;
+    return T;
 }
 
 // kernel.rs:327-336 (AVX-path constants) and :61-66 (scalar normalisation), evaluated in f32 like the reference
@@ -564,6 +614,23 @@ static void fill_bins(SsDev &D, float cs) {
     D.nbin_sub = D.nbin * D.nbin * D.nbin;
     D.inv_c = (float)(1.0 / (double)cs);
     D.rr_cells = (float)D.R + 0.01f;
+}
+// Tiles of S cubes of size cs, kernel of compact support h: the grid, kernel and bin constants of the level set (dense_subdomains.rs:89-244)
+static void fill_tile_geometry(SsDev &D, float cs, int64_t S, float h, float rest_mass) {
+    D.c = cs; D.h = h; D.h2 = fmulr(h, h); D.h2m = fmulr(D.h2, 1.01f); D.rest_mass = rest_mass;
+    D.sub_size = fmulr(cs, (float)S); D.S = (int)S; D.np = (int)S + 1; D.np_magic = (uint32_t)(4294967296ull / (uint64_t)D.np) + 1u;
+    D.R = (int)ceilf(fdivr(h, cs));
+    fill_kernel_consts(D, h);
+    fill_bins(D, cs);
+}
+// Membership (ghost) margin of the subdomain decomposition for a kernel reach r: ceil(r / cs) cubes plus 1 % (dense_subdomains.rs:89-244)
+static float member_margin(float r, float cs) { return fmulr(fmulr(ceilf(fdivr(r, cs)), cs), 1.01f); }
+// D.margin and the number of subdomains it spans, D.srad (D.sub_size set)
+static int set_member_margin(SsDev &D, float margin) {
+    D.margin = margin;
+    D.srad = (int)ceilf(fdivr(margin, D.sub_size));
+    if (D.srad > 8) return ss_fail(SS_ERR_INVALID_PARAMETER, "ghost margin spans more than 8 subdomains; increase subdomain_num_cubes_per_dim");
+    return SS_OK;
 }
 
 // ------------------------------------------------------------------ the subdomain-grid pipeline ----
@@ -597,7 +664,7 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
            c->key_a.as<uint32_t>(), c->err.as<int>());
     const uint64_t ns_keys = (uint64_t)nsub * D.ns_stride;
     // anisotropic mode: members outside the neighbourhood-search grid carry key 0xffffffff and sort behind every cell
-    cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>(), M, D.aniso ? 32 : bits_for(ns_keys));
+    cub_sort(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), M, D.aniso ? 32 : bits_for(ns_keys), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>());
     c->tab_a.ensure(ns_keys * 4); c->tab_b.ensure(ns_keys * 4);
     CK(cudaMemsetAsync(c->tab_a.p, 0xff, ns_keys * 4, st));
     LAUNCH(c, k_mark_starts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_a.as<uint32_t>(), (uint32_t)ns_keys);
@@ -612,8 +679,7 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
         // cell-cooperative kernel (ss_density.cuh): one warp per h-cell that holds a particle inside its subdomain (<= n cells), persistent grid
         LAUNCH(c, k_density_cell_flags, nblk(M, 256), 256, D, M, c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
                c->tab_b.as<uint32_t>(), c->dflag.as<uint32_t>());
-        cub_excl_scan(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M);
-        LAUNCH(c, k_compact_list, nblk(M, 256), 256, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
+        scan_compact(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
         SsDcArgs DA{};
         DA.m = M; DA.list = c->dlist.as<uint32_t>(); DA.list_off = c->doff.as<uint32_t>(); DA.list_flag = c->dflag.as<uint32_t>();
         DA.key = c->key_b.as<uint32_t>(); DA.spos = c->spos.as<float4>(); DA.sub_flat = c->sub_flat.as<uint32_t>();
@@ -623,8 +689,7 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
         else LAUNCH(c, k_density_cells<false>, std::max(grid, 1u), SS_DC_WARPS * 32, D, DA);
     } else {
     LAUNCH(c, k_density_flags, nblk(M, 256), 256, D, M, c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(), c->dflag.as<uint32_t>());
-    cub_excl_scan(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M);
-    LAUNCH(c, k_compact_list, nblk(M, 256), 256, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
+    scan_compact(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
     LAUNCH(c, k_density<false>, nblk(n, 128), 128, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
            c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
            c->tab_a.as<uint32_t>(), c->tab_b.as<uint32_t>(), d_rho, d_ncnt, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
@@ -642,7 +707,7 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
         const uint32_t n32 = (uint32_t)n;
         c->gkey_a.ensure((size_t)n32 * 4); c->gkey_b.ensure((size_t)n32 * 4); c->gval_a.ensure((size_t)n32 * 4); c->gval_b.ensure((size_t)n32 * 4);
         LAUNCH(c, k_ns_keys_global, nblk(n32, 256), 256, D, d_xyz, n32, c->gkey_a.as<uint32_t>(), c->gval_a.as<uint32_t>(), c->err.as<int>());
-        cub_sort_pairs(c, c->gkey_a.as<uint32_t>(), c->gkey_b.as<uint32_t>(), c->gval_a.as<uint32_t>(), c->gval_b.as<uint32_t>(), n32, bits_for(g_ns_cells));
+        cub_sort(c, c->gkey_a.as<uint32_t>(), c->gkey_b.as<uint32_t>(), n32, bits_for(g_ns_cells), c->gval_a.as<uint32_t>(), c->gval_b.as<uint32_t>());
         c->tab_a.ensure(g_ns_cells * 4); c->tab_b.ensure(g_ns_cells * 4);
         CK(cudaMemsetAsync(c->tab_a.p, 0xff, g_ns_cells * 4, st));
         LAUNCH(c, k_mark_starts, nblk(n32, 256), 256, c->gkey_b.as<uint32_t>(), n32, c->tab_a.as<uint32_t>(), (uint32_t)g_ns_cells);
@@ -673,7 +738,7 @@ static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, cons
     cudaStream_t st = c->stream;
     LAUNCH(c, k_bin_keys, nblk(M, 256), 256, D, d_xyz, M, c->cid.as<uint32_t>(), c->sub_flat.as<uint32_t>(), c->val_b.as<uint32_t>(),
            partitioned ? c->sub_owned.as<uint8_t>() : nullptr, c->key_a.as<uint32_t>());
-    cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>(), M, 32);
+    cub_sort(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), M, 32, c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>());
     const uint64_t bin_keys = (uint64_t)nsub * D.nbin_sub;
     c->tab_a.ensure(bin_keys * 4); c->tab_b.ensure(bin_keys * 4);
     CK(cudaMemsetAsync(c->tab_a.p, 0xff, bin_keys * 4, st));
@@ -805,11 +870,8 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
         ++ls_launches;
         LAUNCH(c, k_wstate_reduce, nblk(nbr_c, 256), 256, c->wstate.as<uint8_t>(), nbr_c, c->bstate.as<uint8_t>(), c->flag_fix.as<uint32_t>(),
                c->wflag.as<uint8_t>());
-        cub_excl_scan(c, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_c);
-        LAUNCH(c, k_compact_list, nblk(nbr_c, 256), 256, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_c, c->fix_list.as<uint32_t>());
         uint32_t ln[2] = { 0, 0 };
-        CK(cudaMemcpyAsync(&ln[0], c->off_fix.as<uint32_t>() + (nbr_c - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&ln[1], c->flag_fix.as<uint32_t>() + (nbr_c - 1), 4, cudaMemcpyDeviceToHost, st));
+        scan_compact(c, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_c, c->fix_list.as<uint32_t>(), ln);
         CK(cudaStreamSynchronize(st));
         if (ln[0] + ln[1]) {
             SsLsArgs F = A;
@@ -823,18 +885,12 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     c->flag_mc.ensure((size_t)nbr_b * 4); c->flag_fix.ensure((size_t)nbr_b * 4); c->off_mc.ensure((size_t)nbr_b * 4 + 4); c->off_fix.ensure((size_t)nbr_b * 4 + 4);
     c->list_mc.ensure((size_t)nbr_b * 4); c->list_fix.ensure((size_t)nbr_b * 4);
     LAUNCH(c, k_brick_classify, nblk(nbr_b, 256), 256, D, c->bstate.as<uint8_t>(), nbr_b, c->flag_mc.as<uint32_t>(), c->flag_fix.as<uint32_t>());
-    cub_excl_scan(c, c->flag_mc.as<uint32_t>(), c->off_mc.as<uint32_t>(), nbr_b);
-    cub_excl_scan(c, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_b);
-    LAUNCH(c, k_compact_list, nblk(nbr_b, 256), 256, c->flag_mc.as<uint32_t>(), c->off_mc.as<uint32_t>(), nbr_b, c->list_mc.as<uint32_t>());
-    LAUNCH(c, k_compact_list, nblk(nbr_b, 256), 256, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_b, c->list_fix.as<uint32_t>());
+    uint32_t lc[4] = { 0, 0, 0, 0 };
+    scan_compact(c, c->flag_mc.as<uint32_t>(), c->off_mc.as<uint32_t>(), nbr_b, c->list_mc.as<uint32_t>(), &lc[0]);
+    scan_compact(c, c->flag_fix.as<uint32_t>(), c->off_fix.as<uint32_t>(), nbr_b, c->list_fix.as<uint32_t>(), &lc[2]);
     if (c->ls_variant == 2 && split_certify && !global_mode)       // the tiles were not zero-filled: untouched bricks a later pass can read
         LAUNCH(c, k_zero_untouched, nblk((uint64_t)nbr_b * 32, 256), 256, D, c->bstate.as<uint8_t>(), c->flag_mc.as<uint32_t>(), c->flag_fix.as<uint32_t>(),
                nbr_b, c->tiles.as<float>());
-    uint32_t lc[4] = { 0, 0, 0, 0 };
-    CK(cudaMemcpyAsync(&lc[0], c->off_mc.as<uint32_t>() + (nbr_b - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&lc[1], c->flag_mc.as<uint32_t>() + (nbr_b - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&lc[2], c->off_fix.as<uint32_t>() + (nbr_b - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&lc[3], c->flag_fix.as<uint32_t>() + (nbr_b - 1), 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     const uint32_t n_mc = lc[0] + lc[1], n_fixscan = lc[2] + lc[3];
     out->tm.bricks_total += nbr_b; out->tm.bricks_mc += n_mc; out->tm.bricks_fixscan += n_fixscan;
@@ -869,28 +925,20 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
 // the surface's mesh buffers and to the boundary-vertex list.
 static int marching_cubes_batch(ss_context *c, const SsDev &D, bool global_mode, uint32_t n_mc, ss_surface *out, uint64_t &vtotal, uint64_t &ttotal) {
     cudaStream_t st = c->stream;
-    uint64_t bv = 0, bt = 0;
     const bool warp_mc = c->mc_variant == 1 && !global_mode;       // ss_mc.cuh: one warp per brick, count + emit
+    uint32_t lv[2] = { 0, 0 }, lt[2] = { 0, 0 };                  // vertex / triangle totals of the batch
     if (n_mc) {
         if (warp_mc) LAUNCH(c, k_mc_count_warp, (n_mc + SS_MW_WARPS - 1) / SS_MW_WARPS, SS_MW_WARPS * 32, D, c->tiles.as<float>(), c->list_mc.as<uint32_t>(), n_mc,
                             c->vmask.as<uint8_t>(), c->voff.as<uint32_t>(), c->vcnt.as<uint32_t>(), c->tcnt.as<uint32_t>());
         else if (global_mode) LAUNCH(c, k_mc_count<true>, n_mc, SS_TP_THREADS, D, c->tiles.as<float>(), c->list_mc.as<uint32_t>(), c->vmask.as<uint8_t>(), c->vcnt.as<uint32_t>(), c->tcnt.as<uint32_t>());
         else LAUNCH(c, k_mc_count<false>, n_mc, SS_TP_THREADS, D, c->tiles.as<float>(), c->list_mc.as<uint32_t>(), c->vmask.as<uint8_t>(), c->vcnt.as<uint32_t>(), c->tcnt.as<uint32_t>());
-        cub_excl_scan(c, c->vcnt.as<uint32_t>(), c->vblk_off.as<uint32_t>(), n_mc);
-        cub_excl_scan(c, c->tcnt.as<uint32_t>(), c->tblk_off.as<uint32_t>(), n_mc);
+        scan_with_total(c, c->vcnt.as<uint32_t>(), c->vblk_off.as<uint32_t>(), n_mc, lv);
+        scan_with_total(c, c->tcnt.as<uint32_t>(), c->tblk_off.as<uint32_t>(), n_mc, lt);
     }
     uint32_t bc = 0;
     CK(cudaMemcpyAsync(&bc, c->bcount.p, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    if (n_mc) {
-        uint32_t lv[2] = { 0, 0 }, lt[2] = { 0, 0 };
-        CK(cudaMemcpyAsync(&lv[1], c->vcnt.as<uint32_t>() + (n_mc - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&lt[1], c->tcnt.as<uint32_t>() + (n_mc - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&lv[0], c->vblk_off.as<uint32_t>() + (n_mc - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&lt[0], c->tblk_off.as<uint32_t>() + (n_mc - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        bv = (uint64_t)lv[0] + lv[1]; bt = (uint64_t)lt[0] + lt[1];
-    }
+    const uint64_t bv = (uint64_t)lv[0] + lv[1], bt = (uint64_t)lt[0] + lt[1];
     if (vtotal + bv >= 0xfffffff0ull || ttotal + bt >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "mesh too large for 32-bit vertex / triangle ids");
     if (bv || bt) {
         out->verts.grow_keep((vtotal + bv) * 12, vtotal * 12, st);
@@ -923,6 +971,24 @@ static int marching_cubes_batch(ss_context *c, const SsDev &D, bool global_mode,
     return SS_OK;
 }
 
+// Welds the vertices that carry the same MC edge key: c->bkeys_a holds the keys of the `bc` candidate vertices `ids`.  The kept
+// vertices of verts / keys (nv) go to nverts / nkeys in order, the nt triangles are renumbered in place; returns how many are kept.
+static uint64_t weld_vertices(ss_context *c, const uint32_t *ids, uint32_t bc, const float *verts, const unsigned long long *keys, uint64_t nv,
+                              uint32_t *tris, uint64_t nt, DevBuf &nverts, DevBuf &nkeys) {
+    c->bkeys_b.ensure((size_t)bc * 8); c->bids_b.ensure((size_t)bc * 4);
+    cub_sort(c, c->bkeys_a.as<unsigned long long>(), c->bkeys_b.as<unsigned long long>(), bc, 64, ids, c->bids_b.as<uint32_t>());
+    c->remap.ensure(nv * 4); c->keep.ensure(nv * 4); c->newid.ensure(nv * 4 + 4);
+    LAUNCH(c, k_iota_keep, nblk(nv, 256), 256, (uint32_t)nv, c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
+    LAUNCH(c, k_weld_runs, nblk(bc, 256), 256, c->bkeys_b.as<unsigned long long>(), c->bids_b.as<uint32_t>(), bc,
+           c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
+    const uint64_t nv_final = scan_total(c, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(), (uint32_t)nv);
+    nverts.ensure(std::max<uint64_t>(nv, 1) * 12); nkeys.ensure(std::max<uint64_t>(nv, 1) * 8);
+    LAUNCH(c, k_compact_verts, nblk(nv, 256), 256, (uint32_t)nv, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(), verts, keys,
+           nverts.as<float>(), nkeys.as<unsigned long long>());
+    if (nt) LAUNCH(c, k_remap_tris, nblk(nt * 3, 256), 256, nt * 3, c->remap.as<uint32_t>(), c->newid.as<uint32_t>(), tris);
+    return nv_final;
+}
+
 // Stitching: weld duplicated boundary vertices (same MC edge key), compact the vertices, remap the triangle indices.
 static int weld_boundary_vertices(ss_context *c, ss_surface *out, uint64_t vtotal, uint64_t ttotal, uint64_t &nv_final_out, uint32_t &bc_out) {
     cudaStream_t st = c->stream;
@@ -931,34 +997,11 @@ static int weld_boundary_vertices(ss_context *c, ss_surface *out, uint64_t vtota
     CK(cudaStreamSynchronize(st));
     uint64_t nv_final = vtotal;
     if (vtotal && bc) {
-        c->bkeys_b.ensure((size_t)bc * 8); c->bids_b.ensure((size_t)bc * 4);
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, c->bkeys_a.as<unsigned long long>(), c->bkeys_b.as<unsigned long long>(),
-                                           c->bids_a.as<uint32_t>(), c->bids_b.as<uint32_t>(), (int)bc, 0, 64, st));
-        c->cub_tmp.ensure(tmp);
-        CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tmp, c->bkeys_a.as<unsigned long long>(), c->bkeys_b.as<unsigned long long>(),
-                                           c->bids_a.as<uint32_t>(), c->bids_b.as<uint32_t>(), (int)bc, 0, 64, st));
-        c->launches += 17;
-        c->remap.ensure(vtotal * 4); c->keep.ensure(vtotal * 4); c->newid.ensure(vtotal * 4 + 4);
-        LAUNCH(c, k_iota_keep, nblk(vtotal, 256), 256, (uint32_t)vtotal, c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
-        LAUNCH(c, k_weld_runs, nblk(bc, 256), 256, c->bkeys_b.as<unsigned long long>(), c->bids_b.as<uint32_t>(), bc,
-               c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
-        cub_excl_scan(c, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(), (uint32_t)vtotal);
-        uint32_t lk = 0, ln = 0;
-        CK(cudaMemcpyAsync(&lk, c->keep.as<uint32_t>() + (vtotal - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&ln, c->newid.as<uint32_t>() + (vtotal - 1), 4, cudaMemcpyDeviceToHost, st));
+        // compact into the context's spare mesh buffers, which keep the pre-weld buffers for the next frame
+        nv_final = weld_vertices(c, c->bids_a.as<uint32_t>(), bc, out->verts.as<float>(), out->vkeys.as<unsigned long long>(), vtotal,
+                                 out->tris.as<uint32_t>(), ttotal, c->o_verts2, c->o_vkeys2);
         CK(cudaStreamSynchronize(st));
-        nv_final = (uint64_t)lk + ln;
-        // compact into fresh buffers (swap)
-        DevBuf nverts = c->o_verts2, nkeys = c->o_vkeys2;
-        c->o_verts2 = DevBuf(); c->o_vkeys2 = DevBuf();
-        nverts.ensure(std::max<uint64_t>(vtotal, 1) * 12); nkeys.ensure(std::max<uint64_t>(vtotal, 1) * 8);
-        LAUNCH(c, k_compact_verts, nblk(vtotal, 256), 256, (uint32_t)vtotal, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(),
-               out->verts.as<float>(), out->vkeys.as<unsigned long long>(), nverts.as<float>(), nkeys.as<unsigned long long>());
-        LAUNCH(c, k_remap_tris, nblk(ttotal * 3, 256), 256, ttotal * 3, c->remap.as<uint32_t>(), c->newid.as<uint32_t>(), out->tris.as<uint32_t>());
-        CK(cudaStreamSynchronize(st));
-        c->o_verts2 = out->verts; c->o_vkeys2 = out->vkeys;     // keep the pre-weld buffers for the next frame
-        out->verts = nverts; out->vkeys = nkeys;
+        std::swap(out->verts, c->o_verts2); std::swap(out->vkeys, c->o_vkeys2);
     }
     nv_final_out = nv_final; bc_out = bc;
     return SS_OK;
@@ -977,11 +1020,11 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     const float r2 = faddr(p->particle_radius, p->particle_radius);
     const float rest_mass = fmulr(fmulr(fmulr(r2, r2), r2), p->rest_density);
     const float ns_margin = global_mode ? fmulr(cs, ceilf(fdivr(h, cs)) + 2.0f)      // stencil reach (R + 1 cells) + slack
-                                        : fmulr(fmulr(ceilf(fdivr(h, cs)), cs), 1.01f);
+                                        : member_margin(h, cs);
     // anisotropic kernels (ss_aniso.cuh): a kernel centre moves up to smoothing * h < h from its particle, so memberships need a
     // margin of 2h; the neighbourhood-search grids and cell lists stay on the standard margin (bit-identical densities)
     const bool aniso = c->an_on && !global_mode && !part.enabled && !part.given_rho;
-    const float margin = aniso ? fmulr(fmulr(ceilf(fdivr(fmulr(2.0f, h), cs)), cs), 1.01f) : ns_margin;
+    const float margin = aniso ? member_margin(fmulr(2.0f, h), cs) : ns_margin;
     int64_t nsd[3], ncg[3];
     for (int d = 0; d < 3; ++d) { nsd[d] = (PP.grid.nc[d] + S - 1) / S; ncg[d] = nsd[d] * S; }
     HostGrid gg, sg;
@@ -1000,16 +1043,12 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
 
     SsDev D{};
     for (int d = 0; d < 3; ++d) { D.gmin[d] = gg.mn[d]; D.nsd[d] = (int)nsd[d]; }
-    D.c = cs; D.h = h; D.h2 = fmulr(h, h); D.h2m = fmulr(D.h2, 1.01f); D.thr = p->iso_surface_threshold;
-    D.rest_mass = rest_mass; D.sub_size = sub_size; D.margin = margin; D.grow = fmulr(ns_margin, 1.5f);
-    D.S = (int)S; D.np = (int)S + 1; D.np_magic = (uint32_t)(4294967296ull / (uint64_t)D.np) + 1u;
-    D.R = (int)ceilf(fdivr(h, cs));
-    D.srad = (int)ceilf(fdivr(margin, sub_size));
-    if (D.srad > 8) return ss_fail(SS_ERR_INVALID_PARAMETER, "ghost margin spans more than 8 subdomains; increase subdomain_num_cubes_per_dim");
-    fill_kernel_consts(D, h);
+    fill_tile_geometry(D, cs, S, h, rest_mass);
+    rc = set_member_margin(D, margin);
+    if (rc) return rc;
+    D.thr = p->iso_surface_threshold; D.grow = fmulr(ns_margin, 1.5f);
     D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)ns_margin) / (double)h) + 3;
     D.ns_stride = D.nsD * D.nsD * D.nsD;
-    fill_bins(D, cs);
     D.simd = p->enable_simd ? 1 : 0;
     D.gmode = global_mode ? 1 : 0;
     D.aniso = aniso ? 1 : 0;
@@ -1046,8 +1085,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     out->nv = out->nt = 0; out->nsub = 0;
     out->owner = c;
     c->post.valid = 0; out->frame = ++c->frame;
-    out->rho = c->o_rho; c->o_rho = DevBuf(); out->verts = c->o_verts; c->o_verts = DevBuf();
-    out->tris = c->o_tris; c->o_tris = DevBuf(); out->vkeys = c->o_vkeys; c->o_vkeys = DevBuf();
+    out->rho = std::move(c->o_rho); out->verts = std::move(c->o_verts); out->tris = std::move(c->o_tris); out->vkeys = std::move(c->o_vkeys);
     out->rho.ensure(std::max<uint64_t>(n, 1) * 4);
     float *d_rho = out->rho.as<float>();
     CK(cudaMemsetAsync(d_rho, 0, std::max<uint64_t>(n, 1) * 4, st));
@@ -1056,44 +1094,36 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         if (n) LAUNCH(c, k_aniso_init, nblk(n, 256), 256, d_xyz, (uint32_t)n, out->an_xbar.as<float>(), out->an_g.as<float>(), c->an_det.as<float>());
         out->has_aniso = 1;
     }
-    // NOTE (multi-GPU): the max-reduce callback is a collective -- every rank must call it exactly once per
-    // reconstruction, also ranks that received no particles or own no subdomain.
-    if (n == 0) {
+    // Early end without a mesh: the remaining stage events are recorded (the entries read the stage times).  NOTE (multi-GPU): the
+    // max-reduce callback is a collective -- every rank must call it exactly once per reconstruction, also ranks that received no
+    // particles or own no subdomain.
+    const auto finish_early = [&](bool reduce) {
         for (int e = 3; e <= 9; ++e) CK(cudaEventRecord(c->ev[e], st));
         CK(cudaStreamSynchronize(st));
-        if (part.enabled && part.max_reduce) part.max_reduce(0, part.max_reduce_user);
+        if (reduce && part.enabled && part.max_reduce) part.max_reduce(0, part.max_reduce_user);
         return SS_OK;
-    }
+    };
+    if (n == 0) return finish_early(true);
 
     // ---- decomposition: memberships (owner + ghosts), stable sort by subdomain
     c->cnt.ensure(n * 4); c->off.ensure(n * 4 + 4);
     LAUNCH(c, k_classify_count, nblk(n, 256), 256, D, d_xyz, (uint32_t)n, c->cnt.as<uint32_t>());
-    cub_excl_scan(c, c->cnt.as<uint32_t>(), c->off.as<uint32_t>(), (uint32_t)n);
-    uint32_t lo = 0, lc = 0;
-    CK(cudaMemcpyAsync(&lo, c->off.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&lc, c->cnt.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const uint64_t M64 = (uint64_t)lo + lc;
+    const uint64_t M64 = scan_total(c, c->cnt.as<uint32_t>(), c->off.as<uint32_t>(), (uint32_t)n);
     if (M64 >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "more than 2^32 subdomain memberships");
     const uint32_t M = (uint32_t)M64;
-    if (M == 0) {
-        for (int e = 3; e <= 9; ++e) CK(cudaEventRecord(c->ev[e], st));
-        CK(cudaStreamSynchronize(st));
-        if (part.enabled && part.max_reduce) part.max_reduce(0, part.max_reduce_user);
-        return SS_OK;
-    }
+    if (M == 0) return finish_early(true);
     c->key_a.ensure((size_t)M * 4); c->key_b.ensure((size_t)M * 4); c->val_a.ensure((size_t)M * 4); c->val_b.ensure((size_t)M * 4);
     LAUNCH(c, k_classify_fill, nblk(n, 256), 256, D, d_xyz, (uint32_t)n, c->off.as<uint32_t>(), c->key_a.as<uint32_t>(), c->val_a.as<uint32_t>());
     const uint64_t nslots = (uint64_t)nsd[0] * nsd[1] * nsd[2];
-    cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(), c->val_b.as<uint32_t>(), M, bits_for(nslots));
+    cub_sort(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), M, bits_for(nslots), c->val_a.as<uint32_t>(), c->val_b.as<uint32_t>());
     // key_b = flat subdomain per membership (sorted), val_b = particle index (ascending inside a subdomain)
     c->flags.ensure((size_t)M * 4); c->scan.ensure((size_t)M * 4); c->cid.ensure((size_t)M * 4);
     LAUNCH(c, k_seg_flags, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->flags.as<uint32_t>());
-    cub_incl_scan(c, c->flags.as<uint32_t>(), c->scan.as<uint32_t>(), M);
+    cub_scan<true>(c, c->flags.as<const uint32_t>(), c->scan.as<uint32_t>(), M);
     uint32_t nsub = 0;
     CK(cudaMemcpyAsync(&nsub, c->scan.as<uint32_t>() + (M - 1), 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    c->sub_flat.ensure((size_t)nsub * 4); c->sub_off.ensure((size_t)(nsub + 1) * 4); c->sub_sparse.ensure(nsub);
+    c->sub_flat.ensure((size_t)nsub * 4); c->sub_off.ensure((size_t)(nsub + 1) * 4);
     LAUNCH(c, k_seg_finish, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->scan.as<uint32_t>(), c->cid.as<uint32_t>(),
            c->sub_flat.as<uint32_t>(), c->sub_off.as<uint32_t>());
     std::vector<uint32_t> h_flat(nsub), h_off(nsub + 1);
@@ -1115,18 +1145,16 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         out->sub_flat[s] = h_flat[s]; out->sub_count[s] = h_off[s + 1] - h_off[s];
         out->sub_sparse[s] = (!global_mode && out->sub_count[s] <= sparse_limit) ? 1 : 0;
         if (part.enabled) {
-            const int64_t f = h_flat[s];
             int64_t ijk[3];
-            ijk[0] = f / (nsd[1] * nsd[2]); ijk[1] = (f - ijk[0] * nsd[1] * nsd[2]) / nsd[2]; ijk[2] = f - ijk[0] * nsd[1] * nsd[2] - ijk[1] * nsd[2];
+            subdomain_ijk(h_flat[s], nsd, ijk);
             h_owned[s] = (ijk[part.axis] >= part.own_lo && ijk[part.axis] < part.own_hi) ? 1 : 0;
         }
         if (h_owned[s]) owned_list.push_back(s);
     }
     out->sub_owned = h_owned;
-    if (part.enabled && part.stop_after_decomposition) { for (int e = 3; e <= 9; ++e) CK(cudaEventRecord(c->ev[e], st)); CK(cudaStreamSynchronize(st)); return SS_OK; }
+    if (part.enabled && part.stop_after_decomposition) return finish_early(false);   // (the max-reduce ran above)
     c->sub_owned.ensure(nsub);
     CK(cudaMemcpyAsync(c->sub_owned.p, h_owned.data(), nsub, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->sub_sparse.p, out->sub_sparse.data(), nsub, cudaMemcpyHostToDevice, st));
     CK(cudaEventRecord(c->ev[3], st));
 
     if (part.given_rho) {
@@ -1188,19 +1216,11 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     const size_t nblk_max = max_tiles * nbricks;
     c->tiles.ensure(max_tiles * np3 * 4); c->voff.ensure(max_tiles * np3 * 4); c->vmask.ensure(max_tiles * np3);
     c->vcnt.ensure(nblk_max * 4 + 4); c->tcnt.ensure(nblk_max * 4 + 4); c->vblk_off.ensure(nblk_max * 4 + 4); c->tblk_off.ensure(nblk_max * 4 + 4);
-    c->tile_tab.ensure(max_tiles * sizeof(SsTile)); c->brick_rng.ensure((size_t)D.nb * sizeof(int2)); c->bstate.ensure(nblk_max);
+    c->tile_tab.ensure(max_tiles * sizeof(SsTile)); c->bstate.ensure(nblk_max);
     c->bcount.ensure(4); c->pairs.ensure(16);
     CK(cudaMemsetAsync(c->bcount.p, 0, 4, st));
     CK(cudaMemsetAsync(c->pairs.p, 0, 16, st));
-    {   // candidate bin range of brick b along one axis: bins overlapping [8b - R, 8b + 7 + R)
-        std::vector<int2> h_rng(D.nb);
-        for (int bb = 0; bb < D.nb; ++bb) {
-            h_rng[bb].x = std::max(ss_floor_div(8 * bb - D.R, D.be) + D.nlo, 0);
-            h_rng[bb].y = std::min(ss_floor_div(8 * bb + 6 + D.R, D.be) + D.nlo, D.nbin - 1);
-        }
-        CK(cudaMemcpyAsync(c->brick_rng.p, h_rng.data(), (size_t)D.nb * sizeof(int2), cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));
-    }
+    upload_brick_ranges(c, D);
     std::vector<SsTile> h_tiles(max_tiles);
     uint64_t vtotal = 0, ttotal = 0;
     size_t bcap = std::max<size_t>(1 << 16, c->hint_bc + c->hint_bc / 8);
@@ -1214,13 +1234,10 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     for (uint32_t s0 = 0; s0 < nown; s0 += (uint32_t)max_tiles) {
         const uint32_t nbatch = std::min<uint32_t>((uint32_t)max_tiles, nown - s0);
         for (uint32_t q = 0; q < nbatch; ++q) {
-            SsTile &T = h_tiles[q];
             const uint32_t sid = owned_list[s0 + q];
-            const int64_t f = h_flat[sid];
             int64_t ijk[3];
-            ijk[0] = f / (nsd[1] * nsd[2]); ijk[1] = (f - ijk[0] * nsd[1] * nsd[2]) / nsd[2]; ijk[2] = f - ijk[0] * nsd[1] * nsd[2] - ijk[1] * nsd[2];
-            for (int d = 0; d < 3; ++d) { T.gbase[d] = (int)(ijk[d] * S); T.smin[d] = faddr(gg.mn[d], fmulr((float)ijk[d], sub_size)); }
-            T.s = sid; T.sparse = (out->sub_sparse[sid] || !D.simd) ? 1u : 0u;
+            subdomain_ijk(h_flat[sid], nsd, ijk);
+            h_tiles[q] = make_tile(ijk, S, gg.mn, sub_size, sid, out->sub_sparse[sid] || !D.simd);
         }
         CK(cudaMemcpyAsync(c->tile_tab.p, h_tiles.data(), (size_t)nbatch * sizeof(SsTile), cudaMemcpyHostToDevice, st));
         // level-set variant 2 writes every value a later pass reads (markers, exact values, exact zeros) and fills the untouched
@@ -1283,7 +1300,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     if (c->sph_normals && nv_final) {
         // SPH normals at the vertices (pipeline post-processing step, splashsurf/src/reconstruct.rs:1287-1294); sphere rest mass
         // 4/3 pi r^3 rho0 as in reconstruct.rs:1126-1129
-        out->normals = c->o_normals; c->o_normals = DevBuf();
+        out->normals = std::move(c->o_normals);
         out->normals.ensure(nv_final * 12);
         SsNrmArgs NA{};
         NA.verts = out->verts.as<float>(); NA.vkeys = out->vkeys.as<unsigned long long>(); NA.nv = (uint32_t)nv_final;
@@ -1316,6 +1333,33 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     return SS_OK;
 }
 
+// The frame of an entry that creates a surface: body(s) runs on a fresh surface of context c, which goes to *out when body returns
+// SS_OK and is freed when it returns an error or throws.  The surface records the kernel launches of the call.
+template <typename F>
+static int with_new_surface(ss_context *c, ss_surface **out, F &&body) {
+    ss_surface *s = nullptr;
+    const int rc = ss_guard([&]() -> int {
+        CK(cudaSetDevice(c->device));
+        s = new ss_surface();
+        s->device = c->device;
+        c->launches = 0;
+        const int rc = body(s);
+        s->tm.kernel_launches = c->launches;
+        return rc;
+    });
+    if (rc) ss_surface_free(s);
+    else *out = s;
+    return rc;
+}
+
+// times of the upload, of the AABB and grid, and of the whole device pass of a reconstruction
+static void front_timings(const ss_context *c, ss_surface *s) {
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, c->ev[0], c->ev[1])); s->tm.upload = ms;
+    CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[2])); s->tm.aabb_and_grid = ms;
+    CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[9])); s->tm.total_device = ms;
+}
+
 // ------------------------------------------------------------------ stage-level entry: one level-set tile ----
 // density_grid_loop_auto / density_grid_loop_scalar (dense_subdomains.rs:715-847, both `pub`): the level-set tile of
 // ONE subdomain from an explicit particle list (in list order == ascending index) and explicit densities.
@@ -1331,17 +1375,13 @@ extern "C" int ss_levelset_tile_f32(ss_context *c, const float *xyz, const float
     if (!(cube_size > 0.0f) || !(h > 0.0f) || S < 1 || S > 1024) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad tile parameters");
     if (n >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many particles");
     for (int d = 0; d < 3; ++d) if (subdomain_ijk[d] < 0 || subdomain_ijk[d] > 1000) return ss_fail(SS_ERR_INVALID_PARAMETER, "subdomain_ijk out of range");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         c->post.valid = 0; ++c->frame;                       // this entry rewrites the bins in the scratch
         SsDev D{};
         for (int d = 0; d < 3; ++d) { D.gmin[d] = global_min[d]; D.nsd[d] = (int)subdomain_ijk[d] + 1; }
-        D.c = cube_size; D.h = h; D.h2 = fmulr(h, h); D.h2m = fmulr(D.h2, 1.01f); D.rest_mass = rest_mass;
-        D.sub_size = fmulr(cube_size, (float)S); D.S = (int)S; D.np = (int)S + 1; D.np_magic = (uint32_t)(4294967296ull / (uint64_t)D.np) + 1u;
-        D.R = (int)ceilf(fdivr(h, cube_size));
-        fill_kernel_consts(D, h);
-        fill_bins(D, cube_size);
+        fill_tile_geometry(D, cube_size, S, h, rest_mass);
         D.simd = mode == 0 ? 1 : 0;
         const size_t np3 = (size_t)D.np * D.np * D.np;
         c->tiles.ensure(np3 * 4);
@@ -1353,34 +1393,16 @@ extern "C" int ss_levelset_tile_f32(ss_context *c, const float *xyz, const float
             CK(cudaMemcpyAsync(c->xyz.p, xyz, n * 12, cudaMemcpyDefault, st));
             CK(cudaMemcpyAsync(c->rho.p, rho, n * 4, cudaMemcpyDefault, st));
             c->key_a.ensure((size_t)M * 4); c->key_b.ensure((size_t)M * 4); c->val_a.ensure((size_t)M * 4); c->val_b.ensure((size_t)M * 4);
-            c->cid.ensure((size_t)M * 4); c->sub_flat.ensure(4); c->sub_sparse.ensure(1); c->batch_subs.ensure(4);
+            c->cid.ensure((size_t)M * 4); c->sub_flat.ensure(4); c->err.ensure(4);
             LAUNCH(c, k_iota2, nblk(M, 256), 256, M, c->val_b.as<uint32_t>(), c->cid.as<uint32_t>());
-            uint32_t zero = 0; uint8_t z8 = 0;
             CK(cudaMemcpyAsync(c->sub_flat.p, &flat, 4, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->sub_sparse.p, &z8, 1, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->batch_subs.p, &zero, 4, cudaMemcpyHostToDevice, st));
-            LAUNCH(c, k_bin_keys, nblk(M, 256), 256, D, c->xyz.as<float>(), M, c->cid.as<uint32_t>(), c->sub_flat.as<uint32_t>(),
-                   c->val_b.as<uint32_t>(), (const uint8_t *)nullptr, c->key_a.as<uint32_t>());
-            cub_sort_pairs(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>(), M, 32);
-            const uint64_t bin_keys = (uint64_t)D.nbin_sub;
-            c->tab_a.ensure(bin_keys * 4); c->tab_b.ensure(bin_keys * 4);
-            CK(cudaMemsetAsync(c->tab_a.p, 0xff, bin_keys * 4, st));
-            LAUNCH(c, k_mark_starts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_a.as<uint32_t>(), (uint32_t)bin_keys);
-            LAUNCH(c, k_run_counts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_b.as<uint32_t>(), (uint32_t)bin_keys);
-            c->rec.ensure((size_t)M * 16); c->ksplit.ensure((size_t)M * 4);
-            LAUNCH(c, k_records, nblk(M, 256), 256, D, c->xyz.as<float>(), c->rho.as<float>(), M, c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(),
-                   c->sub_flat.as<uint32_t>(), c->rec.as<float4>(), c->ksplit.as<int>());
-            SsTile T{};
-            for (int d = 0; d < 3; ++d) { T.gbase[d] = (int)(subdomain_ijk[d] * (int64_t)S); T.smin[d] = faddr(global_min[d], fmulr((float)subdomain_ijk[d], D.sub_size)); }
-            T.s = 0; T.sparse = D.simd ? 0u : 1u;
-            std::vector<int2> h_rng(D.nb);
-            for (int bb = 0; bb < D.nb; ++bb) {
-                h_rng[bb].x = std::max(ss_floor_div(8 * bb - D.R, D.be) + D.nlo, 0);
-                h_rng[bb].y = std::min(ss_floor_div(8 * bb + 6 + D.R, D.be) + D.nlo, D.nbin - 1);
-            }
-            c->tile_tab.ensure(sizeof(SsTile)); c->brick_rng.ensure((size_t)D.nb * sizeof(int2));
+            CK(cudaMemsetAsync(c->err.p, 0, 4, st));
+            const int rc = stage_binning(c, D, c->xyz.as<float>(), c->rho.as<float>(), M, 1, false, nullptr, nullptr, /*record_event=*/false);
+            if (rc) return rc;
+            const SsTile T = make_tile(subdomain_ijk, S, global_min, D.sub_size, 0, !D.simd);
+            c->tile_tab.ensure(sizeof(SsTile));
             CK(cudaMemcpyAsync(c->tile_tab.p, &T, sizeof(SsTile), cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->brick_rng.p, h_rng.data(), (size_t)D.nb * sizeof(int2), cudaMemcpyHostToDevice, st));
+            upload_brick_ranges(c, D);
             SsLsArgs A{};
             A.bins = context_bins(c); A.tiles = c->tiles.as<float>();
             A.pairs = nullptr; A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = nullptr; A.mode = SS_LS_EXACT_ALL;
@@ -1392,10 +1414,7 @@ extern "C" int ss_levelset_tile_f32(ss_context *c, const float *xyz, const float
         CK(cudaMemcpyAsync(tile_out, c->tiles.p, np3 * 4, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // ------------------------------------------------------------------ multi-GPU: plan statistics + halo packing ----
@@ -1422,7 +1441,7 @@ extern "C" int ss_partition_stats_f32(ss_context *c, const float *xyz, uint64_t 
                                       uint32_t *hist, uint32_t *occ) {
     if (!c || !grid || !hist || !occ || (n && !xyz) || axis < 0 || axis > 2 || S < 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad argument");
     if (n >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many particles");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         int3 nsd;
         nsd.x = (int)((grid->cells_per_dim[0] + S - 1) / S); nsd.y = (int)((grid->cells_per_dim[1] + S - 1) / S); nsd.z = (int)((grid->cells_per_dim[2] + S - 1) / S);
@@ -1436,10 +1455,7 @@ extern "C" int ss_partition_stats_f32(ss_context *c, const float *xyz, uint64_t 
         }
         CK(cudaStreamSynchronize(c->stream));
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // Plan statistics with the EXACT classifier: `members[slot]` = number of particles of this rank's input that are members (owner or
@@ -1467,16 +1483,14 @@ extern "C" int ss_partition_members_f32(ss_context *c, const float *xyz, uint64_
     int rc = validate_params(p);
     if (rc) return rc;
     if (n >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many particles");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
-        // the decomposition parameters exactly as run_subdomain_grid derives them (dense_subdomains.rs:89-244)
         const int64_t S = (int64_t)p->subdomain_num_cubes_per_dim;
         const float h = p->compact_support_radius, cs = p->cube_size;
         SsDev D{};
         D.sub_size = fmulr(cs, (float)S);
-        D.margin = fmulr(fmulr(ceilf(fdivr(h, cs)), cs), 1.01f);
-        D.srad = (int)ceilf(fdivr(D.margin, D.sub_size));
-        if (D.srad > 8) return ss_fail(SS_ERR_INVALID_PARAMETER, "ghost margin spans more than 8 subdomains; increase subdomain_num_cubes_per_dim");
+        const int rc = set_member_margin(D, member_margin(h, cs));
+        if (rc) return rc;
         uint64_t nslots = 1;
         for (int d = 0; d < 3; ++d) { D.gmin[d] = grid->aabb_min[d]; D.nsd[d] = (int)((grid->cells_per_dim[d] + S - 1) / S); nslots *= (uint64_t)D.nsd[d]; }
         if (nslots >= 2147483647ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many subdomain slots");
@@ -1489,10 +1503,7 @@ extern "C" int ss_partition_members_f32(ss_context *c, const float *xyz, uint64_
         }
         CK(cudaStreamSynchronize(c->stream));
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // Halo packing: destination d takes the particles with lo[d] <= coordinate < hi[d] along the partition axis (one particle may
@@ -1537,7 +1548,7 @@ extern "C" int ss_partition_pack_f32(ss_context *c, const float *xyz, uint64_t n
                                      uint64_t *counts_out, float *send) {
     if (!c || !lo || !hi || !counts_out || (n && !xyz) || axis < 0 || axis > 2 || world < 1 || world > SS_PACK_MAXW) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad argument");
     if (n >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many particles");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nchunks = (uint32_t)((n + SS_PACK_CHUNK - 1) / SS_PACK_CHUNK);
@@ -1550,11 +1561,10 @@ extern "C" int ss_partition_pack_f32(ss_context *c, const float *xyz, uint64_t n
         const unsigned blocks = nblk((uint64_t)nchunks * 32, 128);
         if (!send) {
             LAUNCH(c, k_part_pack<false>, blocks, 128, xyz, (uint32_t)n, axis, iv, (int)world, nchunks, c->pack_cnt.as<uint32_t>(), (float *)nullptr);
-            cub_excl_scan(c, c->pack_cnt.as<uint32_t>(), c->pack_off.as<uint32_t>(), (uint32_t)tab);
-            std::vector<uint32_t> h_off(world), h_last(2);
+            uint32_t h_last[2] = { 0, 0 };
+            scan_with_total(c, c->pack_cnt.as<uint32_t>(), c->pack_off.as<uint32_t>(), (uint32_t)tab, h_last);
+            std::vector<uint32_t> h_off(world);
             for (uint32_t d = 0; d < world; ++d) CK(cudaMemcpyAsync(&h_off[d], c->pack_off.as<uint32_t>() + (size_t)d * nchunks, 4, cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(&h_last[0], c->pack_off.as<uint32_t>() + (tab - 1), 4, cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(&h_last[1], c->pack_cnt.as<uint32_t>() + (tab - 1), 4, cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
             const uint64_t total = (uint64_t)h_last[0] + h_last[1];
             for (uint32_t d = 0; d < world; ++d) counts_out[d] = (d + 1 < world ? h_off[d + 1] : total) - h_off[d];
@@ -1566,10 +1576,7 @@ extern "C" int ss_partition_pack_f32(ss_context *c, const float *xyz, uint64_t n
             c->pack_n = 0;
         }
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // ------------------------------------------------------------------ multi-GPU: one rank's slab of subdomains ----
@@ -1606,40 +1613,22 @@ static int reconstruct_partition_impl(ss_context *c, const float *xyz, uint64_t 
     if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "partitioned reconstruction requires the subdomain grid");
     if (axis < 0 || axis > 2 || own_lo < 0 || own_hi < own_lo || halo < 0) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad partition");
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
-        s = new ss_surface();
-        s->device = c->device; s->n_in = n_in;
-        c->launches = 0;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        s->n_in = n_in;
         Prepared P;
         g_devbuf_slack_eighths = 4;
-        rc = prepare_particles(c, xyz, n_in, p, P, nullptr, grid);
-        if (rc) { ss_surface_free(s); return rc; }
+        int rc = prepare_particles(c, xyz, n_in, p, P, nullptr, grid);
+        if (rc) return rc;
         s->n = P.n; s->grid = P.grid; s->used_decomposition = 1;
         Partition part;
         part.enabled = 1; part.axis = axis; part.own_lo = own_lo; part.own_hi = own_hi; part.halo = halo;
         part.global_max_particles = global_max_particles; part.stop_after_decomposition = stop_after_decomposition;
         part.max_reduce = max_reduce ? &ReduceOnce::call : nullptr; part.max_reduce_user = &once;
         rc = run_subdomain_grid(c, P, p, s, part);
-        if (rc) { ss_surface_free(s); return rc; }
-        float ms = 0.f;
-        CK(cudaEventElapsedTime(&ms, c->ev[0], c->ev[1])); s->tm.upload = ms;
-        CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[2])); s->tm.aabb_and_grid = ms;
-        CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[9])); s->tm.total_device = ms;
-        s->tm.kernel_launches = c->launches;
-        *out = s;
+        if (rc) return rc;
+        front_timings(c, s);
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        char buf[512];
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
-    } catch (const std::bad_alloc &) {
-        if (s) ss_surface_free(s);
-        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
-    }
+    });
 }
 extern "C" uint64_t ss_surface_max_subdomain_particles(const ss_surface *s) { return s ? s->max_particles : 0; }
 
@@ -1653,43 +1642,20 @@ extern "C" int ss_weld_meshes(ss_context *c, float *verts, unsigned long long *k
     *nv_out = nv;
     if (!nv || !n_cand) return SS_OK;
     if (nv >= 0xfffffff0ull || n_cand >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "mesh too large");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t bc = (uint32_t)n_cand;
-        c->bkeys_a.ensure((size_t)bc * 8); c->bkeys_b.ensure((size_t)bc * 8); c->bids_b.ensure((size_t)bc * 4);
+        c->bkeys_a.ensure((size_t)bc * 8);
         LAUNCH(c, k_gather_keys, nblk(bc, 256), 256, keys, cand, bc, c->bkeys_a.as<unsigned long long>());
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, c->bkeys_a.as<unsigned long long>(), c->bkeys_b.as<unsigned long long>(),
-                                           cand, c->bids_b.as<uint32_t>(), (int)bc, 0, 64, st));
-        c->cub_tmp.ensure(tmp);
-        CK(cub::DeviceRadixSort::SortPairs(c->cub_tmp.p, tmp, c->bkeys_a.as<unsigned long long>(), c->bkeys_b.as<unsigned long long>(),
-                                           cand, c->bids_b.as<uint32_t>(), (int)bc, 0, 64, st));
-        c->remap.ensure(nv * 4); c->keep.ensure(nv * 4); c->newid.ensure(nv * 4 + 4);
-        LAUNCH(c, k_iota_keep, nblk(nv, 256), 256, (uint32_t)nv, c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
-        LAUNCH(c, k_weld_runs, nblk(bc, 256), 256, c->bkeys_b.as<unsigned long long>(), c->bids_b.as<uint32_t>(), bc,
-               c->remap.as<uint32_t>(), c->keep.as<uint32_t>());
-        cub_excl_scan(c, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(), (uint32_t)nv);
-        uint32_t lk = 0, ln = 0;
-        CK(cudaMemcpyAsync(&lk, c->keep.as<uint32_t>() + (nv - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&ln, c->newid.as<uint32_t>() + (nv - 1), 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        const uint64_t nv_final = (uint64_t)lk + ln;
-        DevBuf nverts, nkeys;
-        nverts.ensure(nv_final * 12 + 16); nkeys.ensure(nv_final * 8 + 16);
-        LAUNCH(c, k_compact_verts, nblk(nv, 256), 256, (uint32_t)nv, c->keep.as<uint32_t>(), c->newid.as<uint32_t>(), verts, keys,
-               nverts.as<float>(), nkeys.as<unsigned long long>());
-        if (nt) LAUNCH(c, k_remap_tris, nblk(nt * 3, 256), 256, nt * 3, c->remap.as<uint32_t>(), c->newid.as<uint32_t>(), tris);
+        DevBuf nverts, nkeys;                                // compacted copies, written back over verts / keys
+        const uint64_t nv_final = weld_vertices(c, cand, bc, verts, keys, nv, tris, nt, nverts, nkeys);
         CK(cudaMemcpyAsync(verts, nverts.p, nv_final * 12, cudaMemcpyDeviceToDevice, st));
         CK(cudaMemcpyAsync(keys, nkeys.p, nv_final * 8, cudaMemcpyDeviceToDevice, st));
         CK(cudaStreamSynchronize(st));
-        nverts.release(); nkeys.release();
         *nv_out = nv_final;
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 extern "C" const unsigned long long *ss_surface_device_vertex_keys(const ss_surface *s) { return s ? s->vkeys.as<unsigned long long>() : nullptr; }
 extern "C" int ss_surface_copy_subdomain_owned(const ss_surface *s, uint8_t *dst) {
@@ -1705,21 +1671,17 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
     int rc = validate_params(p);
     if (rc) return rc;
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
-        s = new ss_surface();
-        s->device = c->device; s->n_in = n_in;
-        c->launches = 0;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        s->n_in = n_in;
         Prepared P;
-        rc = prepare_particles(c, xyz, n_in, p, P, &s->inside_aabb);
-        if (rc) { ss_surface_free(s); return rc; }
+        int rc = prepare_particles(c, xyz, n_in, p, P, &s->inside_aabb);
+        if (rc) return rc;
         s->n = P.n; s->grid = P.grid;
         // decomposition decision, lib.rs:421-464
         int use_dec = 0;
         if (c->an_on) {
             // anisotropic kernels: subdomain path only, always decomposed (no auto-disable)
-            if (p->spatial_decomposition != 1) { ss_surface_free(s); return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels require the subdomain grid (spatial_decomposition = UniformGrid)"); }
+            if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels require the subdomain grid (spatial_decomposition = UniformGrid)");
             use_dec = 1;
         } else if (p->spatial_decomposition == 1) {
             if (p->auto_disable) {
@@ -1730,31 +1692,15 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
         }
         s->used_decomposition = use_dec;
         rc = run_subdomain_grid(c, P, p, s, Partition(), /*global_mode=*/!use_dec);
-        if (rc) { ss_surface_free(s); return rc; }
-        float ms = 0.f;
-        CK(cudaEventElapsedTime(&ms, c->ev[0], c->ev[1])); s->tm.upload = ms;
-        CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[2])); s->tm.aabb_and_grid = ms;
-        CK(cudaEventElapsedTime(&ms, c->ev[1], c->ev[9])); s->tm.total_device = ms;
-        s->tm.kernel_launches = c->launches;
-        *out = s;
+        if (rc) return rc;
+        front_timings(c, s);
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        char buf[512];
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
-    } catch (const std::bad_alloc &) {
-        if (s) ss_surface_free(s);
-        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
-    }
+    });
 }
 
+// a result buffer of a freed surface goes back to the context's pool when the pool's is smaller (or missing)
 static void give_back(DevBuf &slot, DevBuf &buf) {
-    if (!buf.p) return;
-    if (!slot.p) { slot = buf; buf.p = nullptr; buf.cap = 0; }
-    else if (slot.cap < buf.cap) { cudaFree(slot.p); slot = buf; buf.p = nullptr; buf.cap = 0; }
-    else buf.release();
+    if (buf.p && (!slot.p || slot.cap < buf.cap)) slot = std::move(buf);
 }
 extern "C" void ss_surface_free(ss_surface *s) {
     if (!s) return;
@@ -1767,10 +1713,7 @@ extern "C" void ss_surface_free(ss_surface *s) {
             give_back(c->o_normals, s->normals);
         }
     }
-    s->verts.release(); s->tris.release(); s->vkeys.release(); s->rho.release(); s->normals.release(); s->nbr_off.release(); s->nbr_idx.release();
-    s->weights.release(); s->adj_row.release(); s->adj_idx.release(); s->inc_row.release(); s->inc_idx.release();
-    s->an_xbar.release(); s->an_g.release();
-    delete s;
+    delete s;                                          // frees the buffers the pool did not take
 }
 
 // ------------------------------------------------------------------ accessors ----
@@ -1813,7 +1756,7 @@ static int copy_out(const ss_surface *s, void *dst, const void *src, size_t byte
         scatter_chunk(static_cast<char *>(dst), reinterpret_cast<const char *>(tmp.data()), bytes, true);
         return SS_OK;
     }
-    try {
+    return ss_guard([&]() -> int {
         for (int q = 0; q < 2; ++q) if (!c->h_stage[q]) {
             if (cudaHostAlloc(&c->h_stage[q], SS_STAGE_BYTES_MAX, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); c->h_stage[q] = nullptr; }
         }
@@ -1837,10 +1780,7 @@ static int copy_out(const ss_surface *s, void *dst, const void *src, size_t byte
             scatter_chunk(static_cast<char *>(dst) + (widen ? 2 * off : off), static_cast<const char *>(c->h_stage[k & 1]), n, widen);
         }
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 extern "C" int ss_surface_copy_vertices(const ss_surface *s, float *dst) { return copy_out(s, dst, s ? s->verts.p : nullptr, s ? s->nv * 12 : 0); }
 extern "C" int ss_surface_copy_triangles_u32(const ss_surface *s, uint32_t *dst) { return copy_out(s, dst, s ? s->tris.p : nullptr, s ? s->nt * 12 : 0); }

@@ -232,14 +232,6 @@ __global__ void k_pp_area_normals(uint32_t nv, const float *__restrict__ verts, 
 
 // ------------------------------------------------------------------ host side ----
 #ifndef SS_POST_KERNELS_ONLY          // (tests/emul steps the kernels above on the CPU and skips the rest)
-static void cub_sort_keys64(ss_context *c, const unsigned long long *in, unsigned long long *out, uint32_t n, int end_bit) {
-    size_t tmp = 0;
-    CK(cub::DeviceRadixSort::SortKeys(nullptr, tmp, in, out, (int)n, 0, end_bit, c->stream));
-    c->cub_tmp.ensure(tmp);
-    CK(cub::DeviceRadixSort::SortKeys(c->cub_tmp.p, tmp, in, out, (int)n, 0, end_bit, c->stream));
-    c->launches += 1 + (uint64_t)((end_bit + 7) / 8) * 2;
-}
-
 // Sorted unique low words per high word: row[nv + 1], idx[total].  `keys_a` holds n keys on entry (destroyed).
 static uint32_t pp_build_csr(ss_context *c, uint32_t n, uint32_t nv, int key_bits, DevBuf &row, DevBuf &idx) {
     cudaStream_t st = c->stream;
@@ -250,14 +242,9 @@ static uint32_t pp_build_csr(ss_context *c, uint32_t n, uint32_t nv, int key_bit
         return 0;
     }
     S.keys_b.ensure((size_t)n * 8); S.flag.ensure((size_t)n * 4); S.scan.ensure((size_t)n * 4 + 4);
-    cub_sort_keys64(c, S.keys_a.as<unsigned long long>(), S.keys_b.as<unsigned long long>(), n, key_bits);
+    cub_sort(c, S.keys_a.as<unsigned long long>(), S.keys_b.as<unsigned long long>(), n, key_bits);
     LAUNCH(c, k_pp_flag_unique, nblk(n, 256), 256, S.keys_b.as<unsigned long long>(), n, S.flag.as<uint32_t>());
-    cub_excl_scan(c, S.flag.as<uint32_t>(), S.scan.as<uint32_t>(), n);
-    uint32_t lf = 0, ls = 0;
-    CK(cudaMemcpyAsync(&lf, S.flag.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ls, S.scan.as<uint32_t>() + (n - 1), 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const uint32_t total = lf + ls;
+    const uint32_t total = (uint32_t)scan_total(c, S.flag.as<uint32_t>(), S.scan.as<uint32_t>(), n);
     row.ensure(((size_t)nv + 1) * 4); idx.ensure(std::max<size_t>(total, 1) * 4);
     LAUNCH(c, k_pp_compact_low, nblk(n, 256), 256, S.keys_b.as<unsigned long long>(), S.flag.as<uint32_t>(), S.scan.as<uint32_t>(), n,
            idx.as<uint32_t>());
@@ -309,13 +296,6 @@ static SsQuery pp_query(const ss_context *c, const ss_surface *s) {
     Q.rec = c->rec.as<float4>(); Q.rho = s->rho.as<float>(); Q.sphere_mass = c->post.sphere_mass;
     return Q;
 }
-#define PP_CATCH                                                                                                              \
-    catch (const SsCudaError &err) {                                                                                          \
-        cudaGetLastError();                                                                                                   \
-        char buf[512];                                                                                                        \
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));        \
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);                         \
-    }
 
 // SphInterpolator::interpolate_scalar_quantity / interpolate_vector_quantity at the mesh vertices (sph_interpolation.rs:141-258;
 // pipeline hook reconstruct.rs:1345-1391).  values: [num_particles * dim] (filtered particles, host or device), out: [nv * dim].
@@ -324,7 +304,7 @@ extern "C" int ss_surface_interpolate_quantity_f32(ss_surface *s, const float *v
     if (!c) return rc;
     if (!values || !out || (dim != 1 && dim != 3)) return ss_fail(SS_ERR_INVALID_PARAMETER, "values/out must be non-NULL and dim 1 or 3");
     if (!s->nv) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nv = (uint32_t)s->nv;
@@ -336,7 +316,7 @@ extern "C" int ss_surface_interpolate_quantity_f32(ss_surface *s, const float *v
         CK(cudaMemcpyAsync(out, c->post.out.p, (size_t)nv * dim * 4, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // ------------------------------------------------------------------ SphInterpolator at arbitrary points ----
@@ -355,33 +335,16 @@ extern "C" int ss_sph_interpolator_create_f32(ss_context *c, const float *xyz, u
     p.particle_radius = compact_support_radius * 0.25f; p.rest_density = 1000.0f; p.compact_support_radius = compact_support_radius;
     p.cube_size = compact_support_radius * 0.5f; p.iso_surface_threshold = 0.6f; p.enable_multi_threading = 1; p.enable_simd = 1;
     p.spatial_decomposition = 1; p.subdomain_num_cubes_per_dim = 64; p.auto_disable = 0;
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
-        s = new ss_surface();
-        s->device = c->device; s->n_in = n;
-        c->launches = 0;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        s->n_in = n;
         Prepared P;
         int rc = prepare_particles(c, xyz, n, &p, P, nullptr);
-        if (rc) { ss_surface_free(s); return rc; }
+        if (rc) return rc;
         s->n = P.n; s->grid = P.grid; s->used_decomposition = 1;
         Partition opt;
         opt.given_rho = densities; opt.given_mass = particle_rest_mass;
-        rc = run_subdomain_grid(c, P, &p, s, opt, /*global_mode=*/false);
-        if (rc) { ss_surface_free(s); return rc; }
-        s->tm.kernel_launches = c->launches;
-        *out = s;
-        return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        char buf[512];
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
-    } catch (const std::bad_alloc &) {
-        if (s) ss_surface_free(s);
-        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
-    }
+        return run_subdomain_grid(c, P, &p, s, opt, /*global_mode=*/false);
+    });
 }
 
 __global__ void k_pp_fill(uint32_t n, float value, float *__restrict__ out) {
@@ -415,7 +378,7 @@ extern "C" int ss_sph_interpolate_quantity_at_f32(ss_surface *s, const float *va
     if ((dim != 1 && dim != 3) || (m && (!points || !out)) || (s->n && !values)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or dim not 1 / 3");
     if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many interpolation points for one call");
     if (!m) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t np = (uint32_t)m;
@@ -435,7 +398,7 @@ extern "C" int ss_sph_interpolate_quantity_at_f32(ss_surface *s, const float *va
         CK(cudaMemcpyAsync(out, c->post.out.p, (size_t)np * dim * 4, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // SphInterpolator::interpolate_normals (sph_interpolation.rs:82-133) at `m` points: normalised SPH gradient of the indicator function
@@ -446,7 +409,7 @@ extern "C" int ss_sph_interpolate_normals_at_f32(ss_surface *s, const float *poi
     if (m && (!points || !out)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many interpolation points for one call");
     if (!m) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t np = (uint32_t)m;
@@ -460,7 +423,7 @@ extern "C" int ss_sph_interpolate_normals_at_f32(ss_surface *s, const float *poi
         CK(cudaMemcpyAsync(out, c->post.out.p, (size_t)np * 12, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // ------------------------------------------------------------------ stand-alone neighbourhood search ----
@@ -487,26 +450,21 @@ extern "C" int ss_neighborhood_search_f32(ss_context *c, const float *xyz, uint6
     ss_grid_f32 g{};                                    // only keeps prepare_particles from reducing a bounding box nobody needs
     for (int d = 0; d < 3; ++d) { g.aabb_min[d] = ns.mn[d]; g.aabb_max[d] = ns.mx[d]; g.points_per_dim[d] = ns.np[d]; g.cells_per_dim[d] = ns.nc[d]; }
     g.cell_size = search_radius;
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
-        s = new ss_surface();
-        s->device = c->device; s->n_in = n;
-        c->launches = 0;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        s->n_in = n;
         Prepared P;
         int rc = prepare_particles(c, xyz, n, &p, P, nullptr, &g);
-        if (rc) { ss_surface_free(s); return rc; }
+        if (rc) return rc;
         s->n = P.n; s->grid = ns;
         s->owner = c; c->post.valid = 0; s->frame = ++c->frame;
         cudaStream_t st = c->stream;
-        s->rho = c->o_rho; c->o_rho = DevBuf();
+        s->rho = std::move(c->o_rho);
         s->rho.ensure(std::max<uint64_t>(n, 1) * 4);
         s->nbr_off.ensure((n + 1) * 8);
         if (n == 0) {
             CK(cudaMemsetAsync(s->nbr_off.p, 0, 8, st));
             CK(cudaStreamSynchronize(st));
             s->has_neighbors = 1; s->n_neighbors = 0;
-            *out = s;
             return SS_OK;
         }
         SsDev D{};
@@ -514,24 +472,13 @@ extern "C" int ss_neighborhood_search_f32(ss_context *c, const float *xyz, uint6
         fill_kernel_consts(D, search_radius);
         for (int d = 0; d < 3; ++d) { D.g_ns_amin[d] = ns.mn[d]; D.g_ns_nc[d] = (int)ns.nc[d]; D.gmin[d] = ns.mn[d]; }
         rc = stage_densities(c, D, P.d_xyz, n, 0, 0, cells, /*global_mode=*/true, /*want_nbrs=*/true, s, s->rho.as<float>());
-        if (rc) { ss_surface_free(s); return rc; }
+        if (rc) return rc;
         int h_err = 0;
         CK(cudaMemcpyAsync(&h_err, c->err.p, 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-        if (h_err) { ss_surface_free(s); return ss_fail(SS_ERR_INVALID_PARAMETER, "particle outside of the domain of the neighbourhood search (reference: panic)"); }
-        s->tm.kernel_launches = c->launches;
-        *out = s;
+        if (h_err) return ss_fail(SS_ERR_INVALID_PARAMETER, "particle outside of the domain of the neighbourhood search (reference: panic)");
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        char buf[512];
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
-    } catch (const std::bad_alloc &) {
-        if (s) ss_surface_free(s);
-        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
-    }
+    });
 }
 
 // ------------------------------------------------------------------ marching cubes on caller-supplied level-set tiles ----
@@ -558,24 +505,20 @@ extern "C" int ss_marching_cubes_tiles_f32(ss_context *c, const float *tiles, ui
     if ((uint64_t)ntiles * nbricks >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many tiles for one call");
     std::vector<SsTile> h_tiles(ntiles);
     for (uint32_t t = 0; t < ntiles; ++t) {
-        SsTile &T = h_tiles[t];
+        int64_t ijk[3];
         for (int d = 0; d < 3; ++d) {
-            const int32_t q = tile_ijk[3 * (size_t)t + d];
-            if (q < 0 || (int64_t)q * 64 + 64 >= (1 << 20)) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "tile index out of range (2^20 grid points per dimension)");
-            T.gbase[d] = q * 64; T.smin[d] = faddr(grid_min[d], fmulr((float)q, D.sub_size));
+            ijk[d] = tile_ijk[3 * (size_t)t + d];
+            if (ijk[d] < 0 || ijk[d] * 64 + 64 >= (1 << 20)) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "tile index out of range (2^20 grid points per dimension)");
         }
-        T.s = t; T.sparse = 1u;
+        h_tiles[t] = make_tile(ijk, 64, grid_min, D.sub_size, t, true);
     }
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
         cudaStream_t st = c->stream;
-        s = new ss_surface();
-        s->device = c->device; s->owner = c; s->S = 64;
-        c->launches = 0; c->post.valid = 0; s->frame = ++c->frame;
+        s->owner = c; s->S = 64;
+        c->post.valid = 0; s->frame = ++c->frame;
         for (int d = 0; d < 3; ++d) { s->grid.mn[d] = s->grid.mx[d] = grid_min[d]; s->grid.np[d] = s->grid.nc[d] = 0; }
         s->grid.cell = cube_size;
-        s->verts = c->o_verts; c->o_verts = DevBuf(); s->tris = c->o_tris; c->o_tris = DevBuf(); s->vkeys = c->o_vkeys; c->o_vkeys = DevBuf();
+        s->verts = std::move(c->o_verts); s->tris = std::move(c->o_tris); s->vkeys = std::move(c->o_vkeys);
         s->verts.ensure(1 << 16); s->vkeys.ensure(1 << 16); s->tris.ensure(1 << 16);
         uint64_t vtotal = 0, ttotal = 0, nv_final = 0;
         uint32_t bc = 0;
@@ -592,26 +535,15 @@ extern "C" int ss_marching_cubes_tiles_f32(ss_context *c, const float *tiles, ui
             LAUNCH(c, k_iota2, nblk(n_mc, 256), 256, n_mc, c->list_mc.as<uint32_t>(), c->vcnt.as<uint32_t>());      // every brick of every tile
             CK(cudaStreamSynchronize(st));                                                                          // h_tiles is read by the copy above
             int rc = marching_cubes_batch(c, D, /*global_mode=*/true, n_mc, s, vtotal, ttotal);
-            if (rc) { ss_surface_free(s); return rc; }
+            if (rc) return rc;
             nv_final = vtotal;
             rc = weld_boundary_vertices(c, s, vtotal, ttotal, nv_final, bc);
-            if (rc) { ss_surface_free(s); return rc; }
+            if (rc) return rc;
         }
         s->nv = nv_final; s->nt = ttotal;
         CK(cudaStreamSynchronize(st));
-        s->tm.kernel_launches = c->launches;
-        *out = s;
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        char buf[512];
-        snprintf(buf, sizeof(buf), "%s failed at %s:%d: %s", err.what, err.file, err.line, cudaGetErrorString(err.e));
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, buf);
-    } catch (const std::bad_alloc &) {
-        if (s) ss_surface_free(s);
-        return ss_fail(SS_ERR_OUT_OF_MEMORY, "host allocation failed");
-    }
+    });
 }
 
 // Smoothing weights of the mesh vertices (reconstruct.rs:1159-1258): distance-weighted neighbour count per particle,
@@ -622,7 +554,7 @@ extern "C" int ss_surface_compute_smoothing_weights_f32(ss_surface *s, float nor
     int rc; ss_context *c = pp_context(s, true, &rc);
     if (!c) return rc;
     if (!s->nv) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nv = (uint32_t)s->nv;
@@ -637,7 +569,7 @@ extern "C" int ss_surface_compute_smoothing_weights_f32(ss_surface *s, float nor
         CK(cudaStreamSynchronize(st));
         s->has_weights = 1;
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // par_laplacian_smoothing_inplace (postprocessing.rs:17-53) on the surface's vertices.  weights: [nv] host or device; NULL
@@ -646,7 +578,7 @@ extern "C" int ss_surface_laplacian_smoothing_f32(ss_surface *s, uint32_t iterat
     int rc; ss_context *c = pp_context(s, false, &rc);
     if (!c) return rc;
     if (!s->nv || !iterations) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nv = (uint32_t)s->nv;
@@ -667,7 +599,7 @@ extern "C" int ss_surface_laplacian_smoothing_f32(ss_surface *s, uint32_t iterat
         if (cur != s->verts.as<float>()) CK(cudaMemcpyAsync(s->verts.p, cur, (size_t)nv * 12, cudaMemcpyDeviceToDevice, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // Vertex normals at the surface's current (possibly smoothed) vertices, stored as the surface's normals:
@@ -677,7 +609,7 @@ extern "C" int ss_surface_compute_normals_f32(ss_surface *s, int sph) {
     int rc; ss_context *c = pp_context(s, sph != 0, &rc);
     if (!c) return rc;
     if (!s->nv) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nv = (uint32_t)s->nv;
@@ -692,7 +624,7 @@ extern "C" int ss_surface_compute_normals_f32(ss_surface *s, int sph) {
         CK(cudaStreamSynchronize(st));
         s->has_normals = 1;
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // par_laplacian_smoothing_normals_inplace (postprocessing.rs:56-97) on the surface's normals.
@@ -701,7 +633,7 @@ extern "C" int ss_surface_smooth_normals_f32(ss_surface *s, uint32_t iterations)
     if (!c) return rc;
     if (!s->has_normals) return ss_fail(SS_ERR_INVALID_PARAMETER, "the surface has no normals to smooth");
     if (!s->nv || !iterations) return SS_OK;
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t nv = (uint32_t)s->nv;
@@ -715,7 +647,7 @@ extern "C" int ss_surface_smooth_normals_f32(ss_surface *s, uint32_t iterations)
         if (a != s->normals.as<float>()) CK(cudaMemcpyAsync(s->normals.p, a, (size_t)nv * 12, cudaMemcpyDeviceToDevice, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // Wraps a caller-supplied triangle mesh (host or device pointers: verts nv x 3 f32, tris nt x 3 u32) in a surface so that the
@@ -727,23 +659,15 @@ extern "C" int ss_surface_from_mesh_f32(ss_context *c, const float *verts, uint6
     if (!c || !out || (nv && !verts) || (nt && !tris)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     *out = nullptr;
     if (nv >= 0x7fffffffull || nt * 6 >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "mesh too large for device post-processing");
-    ss_surface *s = nullptr;
-    try {
-        CK(cudaSetDevice(c->device));
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
         cudaStream_t st = c->stream;
-        s = new ss_surface();
-        s->owner = c; s->device = c->device; s->nv = nv; s->nt = nt; s->frame = 0;       // frame 0 never matches a reconstruction
+        s->owner = c; s->nv = nv; s->nt = nt; s->frame = 0;       // frame 0 never matches a reconstruction
         s->verts.ensure(std::max<uint64_t>(nv, 1) * 12); s->tris.ensure(std::max<uint64_t>(nt, 1) * 12);
         if (nv) CK(cudaMemcpyAsync(s->verts.p, verts, nv * 12, cudaMemcpyDefault, st));
         if (nt) CK(cudaMemcpyAsync(s->tris.p, tris, nt * 12, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
-        *out = s;
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        if (s) ss_surface_free(s);
-        cudaGetLastError();
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // Replaces the mesh of a surface (host or device arrays), e.g. after the host-side clean-up / decimation of SURVEY 8(f.4), and keeps
@@ -754,7 +678,7 @@ extern "C" int ss_surface_replace_mesh_f32(ss_surface *s, const float *verts, ui
     if (!c) return rc;
     if ((nv && !verts) || (nt && !tris)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     if (nv >= 0x7fffffffull || nt * 6 >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "mesh too large for device post-processing");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         s->verts.ensure(std::max<uint64_t>(nv, 1) * 12); s->tris.ensure(std::max<uint64_t>(nt, 1) * 12);
@@ -765,10 +689,7 @@ extern "C" int ss_surface_replace_mesh_f32(ss_surface *s, const float *verts, ui
         s->has_adj = s->has_inc = s->has_weights = s->has_normals = 0;
         s->vkeys.release();
         return SS_OK;
-    } catch (const SsCudaError &err) {
-        cudaGetLastError();
-        return ss_fail(err.e == cudaErrorMemoryAllocation ? SS_ERR_OUT_OF_MEMORY : SS_ERR_CUDA, std::string(err.what) + ": " + cudaGetErrorString(err.e));
-    }
+    });
 }
 
 // Replaces the surface's normals by caller-supplied ones ([nv * 3], host or device), e.g. to smooth an arbitrary normal field
@@ -777,14 +698,14 @@ extern "C" int ss_surface_set_normals_f32(ss_surface *s, const float *normals) {
     int rc; ss_context *c = pp_context(s, false, &rc);
     if (!c) return rc;
     if (!normals && s->nv) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         s->normals.ensure(std::max<uint64_t>(s->nv, 1) * 12);
         if (s->nv) CK(cudaMemcpyAsync(s->normals.p, normals, s->nv * 12, cudaMemcpyDefault, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         s->has_normals = 1;
         return SS_OK;
-    } PP_CATCH
+    });
 }
 
 // Vertex -> vertex connectivity of the mesh as CSR (TriMesh3d::vertex_vertex_connectivity, mesh.rs:290-306; neighbours in
@@ -795,7 +716,7 @@ extern "C" int ss_surface_vertex_connectivity(ss_surface *s, uint64_t *offsets, 
     if (!n_indices) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     *n_indices = 0;
     if (!s->nv) { if (offsets) offsets[0] = 0; return SS_OK; }
-    try {
+    return ss_guard([&]() -> int {
         CK(cudaSetDevice(c->device));
         pp_vertex_adjacency(c, s);
         std::vector<uint32_t> row(s->nv + 1);
@@ -804,6 +725,6 @@ extern "C" int ss_surface_vertex_connectivity(ss_surface *s, uint64_t *offsets, 
         if (offsets) for (uint64_t i = 0; i <= s->nv; ++i) offsets[i] = row[i];
         if (indices && row[s->nv]) CK(cudaMemcpy(indices, s->adj_idx.p, (size_t)row[s->nv] * 4, cudaMemcpyDeviceToHost));
         return SS_OK;
-    } PP_CATCH
+    });
 }
 #endif  // SS_POST_KERNELS_ONLY
