@@ -222,6 +222,36 @@ int ss_surface_copy_levelset_tile(const ss_surface *s, float *dst);
 /* Timings / launch counts of the reconstruction that produced `s`. */
 int ss_surface_timings(const ss_surface *s, ss_timings *out);
 
+/* Level-set launch paths of the reconstruction that produced `s`, summed over its tile batches: how many bricks each kernel of
+ * the stage received.  Writes min(n, SS_LSP_N) counters to out[SS_LSP_*] and returns SS_LSP_N (negative: NULL surface).
+ * Host bookkeeping of values the stage reads back anyway (no device work, no synchronisation).
+ * - fallback cascades, bricks each tier received (tier t + 1 receives what tier t could not take; the last tier takes all):
+ *   exact pass, fix-up pass (variant 2) and anisotropic level set;
+ * - certification: work bricks of k_certify_warp with the 384- or 576-candidate slice (variant 2), of k_certify (variant 1), or
+ *   of the fused k_levelset (variant 0, exact everywhere, or more than 32 candidate bin runs per brick);
+ * - the GLOBAL and COUNT template flags of the launches (0 / 1), R = ceil(h / cube_size) and the bin width in cells. */
+#define SS_LSP_EXACT_512      0
+#define SS_LSP_EXACT_1024     1
+#define SS_LSP_EXACT_4096     2
+#define SS_LSP_EXACT_SELECT   3
+#define SS_LSP_FIXUP_512      4
+#define SS_LSP_FIXUP_1024     5
+#define SS_LSP_FIXUP_4096     6
+#define SS_LSP_FIXUP_SELECT   7
+#define SS_LSP_ANISO_512      8
+#define SS_LSP_ANISO_4096     9
+#define SS_LSP_ANISO_SELECT  10
+#define SS_LSP_CERT_WARP_384 11
+#define SS_LSP_CERT_WARP_576 12
+#define SS_LSP_CERT_CTA      13
+#define SS_LSP_CERT_FUSED    14
+#define SS_LSP_GLOBAL        15
+#define SS_LSP_COUNT_PAIRS   16
+#define SS_LSP_R             17
+#define SS_LSP_BIN_CELLS     18
+#define SS_LSP_N             19
+int ss_surface_levelset_paths(const ss_surface *s, uint64_t *out, int n);
+
 /* Tuning knobs (do not change results).
  * - maximum number of subdomain tiles resident at once;
  * - level-set evaluation: by default grid points that are provably inside the fluid (a partial sum of the

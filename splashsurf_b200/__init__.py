@@ -73,6 +73,12 @@ class _Timings(C.Structure):
                 ("levelset_cert_evals", C.c_double), ("tile_setup", C.c_double)]
 
 
+# ss_surface_levelset_paths: counter names in index order (SS_LSP_* of include/splashsurf_b200.h)
+LEVELSET_PATHS = ("exact_512", "exact_1024", "exact_4096", "exact_select", "fixup_512", "fixup_1024", "fixup_4096", "fixup_select",
+                  "aniso_512", "aniso_4096", "aniso_select", "cert_warp_384", "cert_warp_576", "cert_cta", "cert_fused",
+                  "global", "count_pairs", "R", "bin_cells")
+
+
 class _Anisotropy(C.Structure):
     """ss_anisotropy_f32 (include/splashsurf_b200.h)."""
     _fields_ = [("smoothing", C.c_float), ("max_stretch", C.c_float), ("min_neighbors", C.c_uint32)]
@@ -134,6 +140,7 @@ def _bind(L):
     L.ss_surface_copy_neighbor_lists.argtypes = [vp, vp, vp]
     L.ss_context_keep_levelset_tile.argtypes = [vp, i64]
     L.ss_surface_timings.argtypes = [vp, C.POINTER(_Timings)]
+    L.ss_surface_levelset_paths.argtypes = [vp, vp, C.c_int]
     L.ss_context_set_tile_batch.argtypes = [vp, C.c_uint32]
     L.ss_context_set_levelset_exact_everywhere.argtypes = [vp, C.c_int]
     L.ss_context_set_levelset_variant.argtypes = [vp, C.c_int]
@@ -582,6 +589,8 @@ class SurfaceReconstruction:
     timings: Optional[dict] = None
     vertex_edge_keys: Optional[np.ndarray] = None
     subdomains: Optional[dict] = None
+    # with_debug: bricks per level-set kernel and the launch flags (ss_surface_levelset_paths; names in LEVELSET_PATHS)
+    levelset_paths: Optional[dict] = None
     levelset_tile: Optional[np.ndarray] = None
     normals: Optional[np.ndarray] = None       # (V, 3) unit SPH normals when requested
     # with anisotropic kernels (``anisotropy=Anisotropy()``): kernel centres x_bar (N, 3) and matrices G (N, 3, 3) of the particles
@@ -1079,6 +1088,11 @@ def _collect(ctx: Context, s, n_in: int, p: _Params, debug: bool, tile: bool) ->
         flat, cnt, sp = np.empty(ns, np.int64), np.empty(ns, np.uint64), np.empty(ns, np.uint8)
         _check(L, L.ss_surface_copy_subdomains(s, flat.ctypes.data, cnt.ctypes.data, sp.ctypes.data))
         res.subdomains = {"flat": flat, "count": cnt, "sparse": sp.astype(bool)}
+        lp = np.zeros(64, np.uint64)
+        k = L.ss_surface_levelset_paths(s, lp.ctypes.data, len(lp))
+        if k != len(LEVELSET_PATHS):
+            raise SplashsurfError(-k if k < 0 else 6, f"ss_surface_levelset_paths returned {k}")
+        res.levelset_paths = {name: int(v) for name, v in zip(LEVELSET_PATHS, lp)}
     if tile:
         S = int(p.subdomain_num_cubes_per_dim)
         t = np.empty((S + 1,) * 3, dtype=np.float32)

@@ -687,6 +687,13 @@ __device__ __forceinline__ int ss_ext_group(int t) { return t < 6 ? (t >> 1) : t
 // Launch: SS_LS_CERTIFY / SS_LS_EXACT_ALL run over a work list of non-empty bricks (k_brick_worklist); with
 // P.ext_bricks the list only holds bricks 0 .. nb-2 per axis and the last one also evaluates the np-1 planes
 // (extension tasks).  SS_LS_FIX runs over the flagged bricks (any index, no extension).
+// adds a warp's in-support evaluations to the work counter (COUNT instantiations)
+__device__ __forceinline__ void ss_flush_hits(unsigned long long *pairs, unsigned hits, int lane) {
+    unsigned long long np_ = hits;
+    for (int o = 16; o > 0; o >>= 1) np_ += __shfl_xor_sync(0xffffffffu, np_, o);
+    if (lane == 0 && np_) atomicAdd(pairs, np_);
+}
+
 template <bool COUNT, bool GLOBAL>
 __global__ void __launch_bounds__(SS_LS_THREADS, 3)
 k_levelset(SsDev P, SsLsArgs A) {
@@ -780,6 +787,7 @@ k_levelset(SsDev P, SsLsArgs A) {
             if (threadIdx.x == 0) A.bstate[brick_lin] = 2;
             if (has_ext && lane == 0) A.bstate[(((size_t)tile_idx * nb + vbx) * nb + vby) * nb + vbz] = 2;
         }
+        if (COUNT && A.pairs) ss_flush_hits(A.pairs, hits, lane);
         return;
     }
 
@@ -843,11 +851,7 @@ k_levelset(SsDev P, SsLsArgs A) {
         const float phi = ss_exact_box<GLOBAL>(P, L, sparse, s_rec, s_ks, s_key, s_list[warp], s_imin, s_dx0, C, lane, hits);
         if (L.valid) A.tiles[L.out_idx] = phi;
     }
-    if (COUNT && A.pairs) {
-        unsigned long long np_ = hits;
-        for (int o = 16; o > 0; o >>= 1) np_ += __shfl_xor_sync(0xffffffffu, np_, o);
-        if (lane == 0 && np_) atomicAdd(A.pairs, np_);
-    }
+    if (COUNT && A.pairs) ss_flush_hits(A.pairs, hits, lane);
 }
 
 // Work list of the level-set launch: one thread per brick; listed when any of its candidate bins holds particles

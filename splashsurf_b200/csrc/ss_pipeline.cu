@@ -172,6 +172,7 @@ struct ss_surface {
     uint64_t max_particles = 0;
     std::vector<float> tile;
     ss_timings tm{};
+    uint64_t ls_paths[SS_LSP_N] = {};                        // ss_surface_levelset_paths
 };
 
 // ------------------------------------------------------------------ host grid math (exact f32) ----
@@ -529,13 +530,15 @@ static SsBins context_bins(const ss_context *c) {
 
 // Fallback cascade over a list of n bricks: tier t launches over the bricks tier t - 1 could not take, appending those it cannot
 // take itself to `left` ([0] = count, [1..] = linear brick indices), the next tier's list.  The last tier takes every brick it gets
-// (left = nullptr).  Stops when no brick is left.
+// (left = nullptr).  Stops when no brick is left.  received[t] accumulates the length of tier t's list.
 typedef std::function<void(const uint32_t *list, uint32_t n, uint32_t *left)> SsTier;
-static void run_cascade(ss_context *c, const uint32_t *list, uint32_t n, std::initializer_list<SsTier> tiers, uint64_t &ls_launches) {
+static void run_cascade(ss_context *c, const uint32_t *list, uint32_t n, std::initializer_list<SsTier> tiers, uint64_t &ls_launches,
+                        uint64_t *received) {
     DevBuf *const left_bufs[] = { &c->fallback, &c->fallback2, &c->fallback3 };
     size_t t = 0;
     for (const SsTier &tier : tiers) {
         if (!n) return;
+        received[t] += n;
         if (++t == tiers.size()) { tier(list, n, nullptr); ++ls_launches; return; }
         DevBuf &left = *left_bufs[t - 1];
         left.ensure(((size_t)n + 1) * 4);
@@ -763,7 +766,9 @@ static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, cons
 
 // Exact values for the flagged boxes of `n_bricks` listed bricks.  Variant 2: warp-per-brick kernel (ss_exact.cuh), bricks it
 // cannot take come back in a fallback list and go through k_levelset (SS_LS_FIX) like in the other variants.
-static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint32_t n_bricks, bool global_mode, uint64_t &ls_launches) {
+// received: the cascade's tier counters in ss_surface::ls_paths (exact or fix-up pass).
+static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint32_t n_bricks, bool global_mode, uint64_t &ls_launches,
+                         uint64_t *received) {
     if (!n_bricks) return;
     const bool count = c->count_pairs != 0;
     if (c->ls_variant != 2) { launch_levelset(c, dim3(n_bricks), D, F, count, global_mode); ++ls_launches; return; }
@@ -796,13 +801,13 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
             G.fix_bricks = list;
             launch_levelset(c, dim3(n), D, G, count, global_mode);
         },
-    }, ls_launches);
+    }, ls_launches, received);
 }
 
 // Anisotropic level set of one batch (ss_aniso.cuh): work list of non-empty bricks without extension tasks (the single-point
 // planes of the last brick are bricks of their own), warp-per-brick kernel, then the 4096-slot slice, then selection.  Every
 // listed brick gets state 2 (exact values).  Returns the length of the work list.
-static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, uint64_t &ls_launches) {
+static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, uint64_t &ls_launches, uint64_t *received) {
     SsDev Dw = D;
     Dw.ext_bricks = 0;
     const uint32_t n_work = build_worklist(c, Dw, nbatch);
@@ -818,7 +823,7 @@ static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nb
         },
         [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_aniso_levelset<SS_AN_BIG_CAP, 1>), n, 32, Dw, args(list, n, left, nullptr)); },
         [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_aniso_select, n, 32, Dw, args(list, n, left, nullptr)); },
-    }, ls_launches);
+    }, ls_launches, received);
     return n_work;
 }
 
@@ -833,10 +838,14 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     A.pairs = c->count_pairs ? c->pairs.as<unsigned long long>() : nullptr;
     A.mode = exact_all ? SS_LS_EXACT_ALL : SS_LS_CERTIFY;
     A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = c->bstate.as<uint8_t>();
-    const uint32_t n_work = D.aniso ? launch_aniso_levelset(c, D, nbatch, ls_launches) : build_worklist(c, D, nbatch);
+    uint64_t *const paths = out->ls_paths;
+    const uint32_t n_work = D.aniso ? launch_aniso_levelset(c, D, nbatch, ls_launches, paths + SS_LSP_ANISO_512) : build_worklist(c, D, nbatch);
     A.work_list = c->list_ls.as<uint32_t>();
     const bool split_certify = !D.aniso && c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
-    if (n_work && !split_certify && !D.aniso) { launch_levelset(c, dim3(n_work), D, A, c->count_pairs != 0, global_mode); ++ls_launches; }
+    if (n_work && !split_certify && !D.aniso) {
+        launch_levelset(c, dim3(n_work), D, A, c->count_pairs != 0, global_mode); ++ls_launches;
+        paths[SS_LSP_CERT_FUSED] += n_work;
+    }
     if (n_work && split_certify) {
         // variant 1 (ss_certify.cuh): certification kernel, then the exact pass over the boxes it could not certify
         const uint32_t nbr_c = nbatch * nbricks;
@@ -865,8 +874,12 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
                 if (cw_small) LAUNCH(c, (k_certify_warp<G, C, SS_CW_CAP_S, SS_CW_WARPS_S>), grid_s, SS_CW_WARPS_S * 32, D, W);
                 else LAUNCH(c, (k_certify_warp<G, C, SS_CW_CAP_L, SS_CW_WARPS_L>), grid_l, SS_CW_WARPS_L * 32, D, W);
             });
-        } else if (global_mode) LAUNCH(c, k_certify<true>, n_work, SS_LS_THREADS, D, CA);
-        else LAUNCH(c, k_certify<false>, n_work, SS_LS_THREADS, D, CA);
+            paths[cw_small ? SS_LSP_CERT_WARP_384 : SS_LSP_CERT_WARP_576] += n_work;
+        } else {
+            if (global_mode) LAUNCH(c, k_certify<true>, n_work, SS_LS_THREADS, D, CA);
+            else LAUNCH(c, k_certify<false>, n_work, SS_LS_THREADS, D, CA);
+            paths[SS_LSP_CERT_CTA] += n_work;
+        }
         ++ls_launches;
         LAUNCH(c, k_wstate_reduce, nblk(nbr_c, 256), 256, c->wstate.as<uint8_t>(), nbr_c, c->bstate.as<uint8_t>(), c->flag_fix.as<uint32_t>(),
                c->wflag.as<uint8_t>());
@@ -876,7 +889,7 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
         if (ln[0] + ln[1]) {
             SsLsArgs F = A;
             F.mode = SS_LS_FIX; F.wflag = c->wflag.as<uint8_t>(); F.fix_bricks = c->fix_list.as<uint32_t>();
-            launch_exact(c, D, F, ln[0] + ln[1], global_mode, ls_launches);
+            launch_exact(c, D, F, ln[0] + ln[1], global_mode, ls_launches, paths + SS_LSP_EXACT_512);
         }
     }
     out->tm.bricks_levelset += n_work;
@@ -912,7 +925,7 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
         CK(cudaStreamSynchronize(st));
         if (nfl[0]) {
             A.mode = SS_LS_FIX; A.wflag = c->wflag.as<uint8_t>(); A.fix_bricks = c->fix_list.as<uint32_t>();
-            if (split_certify) launch_exact(c, D, A, nfl[0], global_mode, ls_launches);
+            if (split_certify) launch_exact(c, D, A, nfl[0], global_mode, ls_launches, paths + SS_LSP_FIXUP_512);
             else { launch_levelset(c, dim3(nfl[0]), D, A, c->count_pairs != 0, global_mode); ++ls_launches; }
             fix_points += nfl[1];
         }
@@ -1079,6 +1092,8 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         if (per_axis * per_axis > 128) return ss_fail(SS_ERR_INVALID_PARAMETER, "internal: too many candidate bin runs per brick");
         certify_runs = per_axis * per_axis;
     }
+    out->ls_paths[SS_LSP_GLOBAL] = global_mode ? 1 : 0; out->ls_paths[SS_LSP_COUNT_PAIRS] = c->count_pairs ? 1 : 0;
+    out->ls_paths[SS_LSP_R] = (uint64_t)D.R; out->ls_paths[SS_LSP_BIN_CELLS] = (uint64_t)D.be;
 
     const bool want_nbrs = p->global_neighborhood_list != 0 && !part.enabled;
     CK(cudaEventRecord(c->ev[2], st));
@@ -1843,6 +1858,11 @@ extern "C" int ss_surface_copy_neighbor_lists(const ss_surface *s, uint64_t *off
     return rc;
 }
 extern "C" int ss_surface_timings(const ss_surface *s, ss_timings *o) { if (!s || !o) return SS_ERR_INVALID_PARAMETER; *o = s->tm; return SS_OK; }
+extern "C" int ss_surface_levelset_paths(const ss_surface *s, uint64_t *out, int n) {
+    if (!s) return -SS_ERR_INVALID_PARAMETER;
+    for (int i = 0; i < std::min(n, (int)SS_LSP_N); ++i) out[i] = s->ls_paths[i];
+    return SS_LSP_N;
+}
 extern "C" float ss_surface_anisotropy_ms(const ss_surface *s) { return (s && s->has_aniso) ? s->an_ms : 0.0f; }
 extern "C" int ss_surface_copy_anisotropy(const ss_surface *s, float *xbar, float *g) {
     if (!s) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL surface");

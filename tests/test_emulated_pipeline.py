@@ -142,14 +142,21 @@ def test_emulated_warp_per_brick_certification(emu, oracle_mod, name, gen, kw, o
     _check_bit_exact(emu, oracle_mod, gen(), kw, variant=2, **opts)
 
 
-@pytest.mark.parametrize("n,sigma", [(600, 0.004), (1500, 0.004), (400, 0.02), (260, 0.01), (4500, 0.004)],
+@pytest.mark.parametrize("n,sigma,finishes", [(600, 0.004, "exact_1024"), (1500, 0.004, "exact_4096"), (400, 0.02, None), (260, 0.01, None),
+                                               (4500, 0.004, "exact_select")],
                          ids=["oversized_brick_1024_variant", "oversized_brick_4096_variant", "list_overflow", "dense_cluster", "extreme_cluster"])
-def test_emulated_warp_per_brick_clustered_particles(emu, oracle_mod, n, sigma):
-    """Variant 2 on pathological clustering: more candidates than a warp's slice holds (brick goes to the 4096-candidate variant of
-    the exact kernel), more candidates in the support of one sub-box than its list holds, a dense cluster that still fits, and
-    more than 4096 candidates around one brick (last resort: k_levelset's selection path)."""
+def test_emulated_warp_per_brick_clustered_particles(emu, oracle_mod, n, sigma, finishes):
+    """Variant 2 on pathological clustering: more candidates than a warp's slice holds (the 1024- and 4096-candidate tiers of the
+    exact kernel finish the bricks), more candidates in the support of one sub-box than its list holds, a dense cluster that still
+    fits, and more than 4096 candidates around one brick (last resort: k_levelset's selection path).  The tier named by `finishes`
+    must finish every brick of the exact pass (tests/test_zzz_gpu_levelset_paths.py holds the whole path matrix)."""
     kw = dict(BASE, cube_size=0.5, subdomain_grid_auto_disable=False)
-    _check_bit_exact(emu, oracle_mod, np.random.default_rng(n).normal(0, sigma, (n, 3)).astype(np.float32), kw, variant=2)
+    g, _ = _check_bit_exact(emu, oracle_mod, np.random.default_rng(n).normal(0, sigma, (n, 3)).astype(np.float32), kw, variant=2)
+    if finishes:
+        lp = g.levelset_paths
+        tiers = ["exact_512", "exact_1024", "exact_4096", "exact_select"]
+        t = tiers.index(finishes)
+        assert lp[finishes] == lp["exact_512"] > 0 and (t + 1 == len(tiers) or lp[tiers[t + 1]] == 0), lp
 
 
 @pytest.mark.parametrize("case", ["certify_default", "scalar_arithmetic", "clump_rounds_and_pool_overflow", "clump_oversized_cell", "clumps_in_a_cube"])

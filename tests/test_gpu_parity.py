@@ -108,13 +108,16 @@ def test_cuda_edge_cases(ss, oracle_mod):
     g = ss.reconstruct_surface(p, with_debug=True, **kw)
     o = oracle_mod.reconstruct(p, **kw)
     assert _parity(oracle_mod, g, o)["triangles_equal"] and g.mesh.nvertices == 252
-    # 3000 particles inside one brick's reach: exercises the oversized-candidate path of the level-set kernel
+    # 3000 particles inside one brick's reach: more candidates per brick than the 1024-candidate tier of the exact pass holds; the
+    # 4096 tier finishes some bricks, k_levelset's selection path the rest
     p = np.random.default_rng(1).normal(0, 0.004, (3000, 3)).astype(np.float32)
     g = ss.reconstruct_surface(p, with_debug=True, **kw)
     o = oracle_mod.reconstruct(p, **kw)
     assert np.array_equal(g.particle_densities, o["particle_densities"])
     m = _parity(oracle_mod, g, o)
     assert m["keys_equal"] and m["triangles_equal"] and m["n_not_bitexact"] == 0, m
+    lp = g.levelset_paths
+    assert lp["exact_1024"] == lp["exact_512"] > 0 and 0 < lp["exact_select"] < lp["exact_4096"] == lp["exact_1024"], lp
     # error behaviour (uniform_grid.rs:147-169, lib.rs:289-314)
     with pytest.raises(ss.SplashsurfError) as e:
         ss.reconstruct_surface(np.zeros((4, 3), np.float32), particle_radius=0.025, smoothing_length=2.0, cube_size=0.0)

@@ -45,7 +45,9 @@ def test_cuda_split_certification_bit_exact_vs_oracle(ss, oracle_mod, name, gen,
 
 @pytest.mark.parametrize("n,sigma", [(3000, 0.004), (400, 0.02), (260, 0.01), (6000, 0.004)], ids=["oversized_brick", "list_overflow", "dense_cluster", "extreme_cluster"])
 def test_cuda_warp_per_brick_clustered_particles(ss, oracle_mod, n, sigma):
-    """Variant 2 on pathological clustering (fallback of whole bricks to k_levelset, sub-box list overflow)."""
+    """Variant 2 on pathological clustering (fallback of whole bricks to k_levelset, sub-box list overflow).  oversized_brick: the
+    1024-candidate tier finishes no brick, the 4096 tier some, k_levelset's selection path the rest; extreme_cluster: every brick of
+    the exact pass ends in the selection path (tests/test_zzz_gpu_levelset_paths.py holds the whole path matrix)."""
     kw = dict(BASE, cube_size=0.5, subdomain_grid_auto_disable=False)
     p = np.random.default_rng(n).normal(0, sigma, (n, 3)).astype(np.float32)
     o = oracle_mod.reconstruct(p, **kw)
@@ -58,6 +60,11 @@ def test_cuda_warp_per_brick_clustered_particles(ss, oracle_mod, n, sigma):
     assert np.array_equal(g.particle_densities, o["particle_densities"])
     m = oracle_mod.mesh_parity(g.mesh.vertices, g.mesh.triangles, g.vertex_edge_keys, o["vertices"], o["triangles"], o["vertex_keys"], 64)
     assert m["keys_equal"] and m["triangles_equal"] and m["n_not_bitexact"] == 0, m
+    lp = g.levelset_paths
+    if n == 3000:
+        assert lp["exact_1024"] == lp["exact_512"] > 0 and 0 < lp["exact_select"] < lp["exact_4096"] == lp["exact_1024"], lp
+    if n == 6000:
+        assert lp["exact_select"] == lp["exact_512"] > 0, lp
 
 
 @pytest.mark.parametrize("case", ["cube24", "splash_scalar", "dam_small", "clump_rounds_and_pool_overflow", "clump_oversized_cell"])
