@@ -244,9 +244,13 @@ def canonicalize(vertices, triangles, keys):
     return v, t, k
 
 
-def resolve_keys(vertices, grid_min, cell_size, known_keys, triangles=None, known_triangles=None):
+def resolve_keys(vertices, grid_min, cell_size, known_keys, triangles=None, known_triangles=None, known_vertices=None):
     """Edge keys for a mesh whose keys are unknown (the reference binary's output), disambiguated with a
     trusted mesh (keys + triangles).
+
+    With `known_vertices` (the trusted mesh's positions), a vertex whose f32 bits equal those of exactly one trusted vertex
+    takes that vertex's key first.  Far from the origin a vertex close to a lattice point lies within the coordinates'
+    rounding of it, so its position alone no longer tells its edge (two vertices near one lattice point come out swapped).
 
     A vertex with interpolation weight ~0 or ~1 sits on a lattice point, where `edge_keys_from_positions`
     cannot tell which of the six incident edges carries it (several such vertices usually share the point).
@@ -260,7 +264,19 @@ def resolve_keys(vertices, grid_min, cell_size, known_keys, triangles=None, know
     known = {tuple(k): i for i, k in enumerate(known_keys.tolist())}
     used = {}
     pending = []
+    exact = set()
+    if known_vertices is not None:
+        by_bits = {}
+        for j, b in enumerate(map(tuple, np.ascontiguousarray(known_vertices, dtype=np.float32).view(np.uint32).tolist())):
+            by_bits.setdefault(b, []).append(j)
+        for i, b in enumerate(map(tuple, np.ascontiguousarray(vertices, dtype=np.float32).view(np.uint32).tolist())):
+            js = by_bits.get(b, [])
+            k = tuple(known_keys[js[0]].tolist()) if len(js) == 1 else None
+            if k is not None and k not in used:
+                keys[i] = k; used[k] = i; exact.add(i)
     for i, k in enumerate(map(tuple, keys.tolist())):
+        if i in exact:
+            continue
         if k in known and k not in used:
             used[k] = i
         else:
@@ -269,6 +285,8 @@ def resolve_keys(vertices, grid_min, cell_size, known_keys, triangles=None, know
         return keys
     v = np.asarray(vertices, dtype=np.float64)
     q = (v - np.asarray(grid_min, dtype=np.float64)[None]) / float(cell_size)
+    # "on a lattice point": within 1e-3 cells, or within the f32 rounding of the coordinates where that is coarser
+    near = max(1e-3, 4.0 * float(np.spacing(np.float32(np.abs(v).max()))) / float(cell_size)) if len(v) else 1e-3
     groups = {}
     for i in pending:
         groups.setdefault(tuple(np.rint(q[i]).astype(np.int64).tolist()), []).append(i)
@@ -287,9 +305,9 @@ def resolve_keys(vertices, grid_min, cell_size, known_keys, triangles=None, know
                 k = list(P); k[a] += off
                 cands.append((k[0], k[1], k[2], a))
         for k in cands:
-            if k in used and used[k] not in members:
+            if k in used and used[k] not in members and used[k] not in exact:
                 qi = q[used[k]]
-                if np.abs(qi - np.rint(qi)).max() < 1e-3:
+                if np.abs(qi - np.rint(qi)).max() < near:
                     members.append(used.pop(k))
         free = [k for k in cands if k in known and k not in used]
         if len(free) < len(members):

@@ -95,6 +95,15 @@ __device__ __forceinline__ void ss_sort_keys(unsigned long long *keys, int n) {
     }
 }
 
+// Coordinate of the grid point with GLOBAL index g, by the reference's expressions: x, y mul then add, z fused unless `sparse`
+// (dense_subdomains.rs:1068, :1101-1102; scalar: uniform_grid.rs:418-425).  Both are monotonic in g, so a box whose bounds come from
+// the same expression contains every point it spans, however large the coordinates' rounding is against the cell size; the culls
+// with a relative slack on h^2 rely on this.
+__device__ __forceinline__ float ss_grid_xy(const SsDev &P, int g, int d) { return __fadd_rn(__fmul_rn((float)g, P.c), P.gmin[d]); }
+__device__ __forceinline__ float ss_grid_z(const SsDev &P, int g, bool sparse) {
+    return sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)g, P.c)) : __fmaf_rn((float)g, P.c, P.gmin[2]);
+}
+
 // lane -> its two grid points (li, lj, lk) and (li, lj, lk + 1) within a 4x4x4-point sub-box; pmax: the tile's last point index
 struct SsSubLane { int li, lj, lk, pmax; };
 __device__ __forceinline__ SsSubLane ss_sub_lane(const SsDev &P, int lane) { return SsSubLane{ lane >> 3, (lane >> 1) & 3, (lane & 1) * 2, P.np - 1 }; }
@@ -118,14 +127,14 @@ __device__ __forceinline__ SsSubBox ss_sub_box(const SsDev &P, const SsTile &T, 
     const bool row_ok = G.i <= pmax && G.j <= pmax;
     G.vA = row_ok && G.k <= pmax; G.vB = row_ok && G.k + 1 <= pmax;
     G.gi = T.gbase[0] + G.i; G.gj = T.gbase[1] + G.j; G.gk = T.gbase[2] + G.k;
-    G.gx = __fadd_rn(__fmul_rn((float)G.gi, P.c), P.gmin[0]);
-    G.gy = __fadd_rn(__fmul_rn((float)G.gj, P.c), P.gmin[1]);
-    G.gzA = sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)G.gk, P.c)) : __fmaf_rn((float)G.gk, P.c, P.gmin[2]);
-    G.gzB = sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)(G.gk + 1), P.c)) : __fmaf_rn((float)(G.gk + 1), P.c, P.gmin[2]);
+    G.gx = ss_grid_xy(P, G.gi, 0);
+    G.gy = ss_grid_xy(P, G.gj, 1);
+    G.gzA = ss_grid_z(P, G.gk, sparse);
+    G.gzB = ss_grid_z(P, G.gk + 1, sparse);
     const int i1 = min(i0 + 3, pmax), j1 = min(j0 + 3, pmax), k1 = min(k0 + 3, pmax);
     G.k1 = k1;
-    G.bxl = fmaf((float)(T.gbase[0] + i0), P.c, P.gmin[0]); G.bxh = fmaf((float)(T.gbase[0] + i1), P.c, P.gmin[0]);
-    G.byl = fmaf((float)(T.gbase[1] + j0), P.c, P.gmin[1]); G.byh = fmaf((float)(T.gbase[1] + j1), P.c, P.gmin[1]);
-    G.bzl = fmaf((float)(T.gbase[2] + k0), P.c, P.gmin[2]); G.bzh = fmaf((float)(T.gbase[2] + k1), P.c, P.gmin[2]);
+    G.bxl = ss_grid_xy(P, T.gbase[0] + i0, 0); G.bxh = ss_grid_xy(P, T.gbase[0] + i1, 0);
+    G.byl = ss_grid_xy(P, T.gbase[1] + j0, 1); G.byh = ss_grid_xy(P, T.gbase[1] + j1, 1);
+    G.bzl = ss_grid_z(P, T.gbase[2] + k0, sparse); G.bzh = ss_grid_z(P, T.gbase[2] + k1, sparse);
     return G;
 }

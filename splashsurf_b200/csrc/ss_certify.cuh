@@ -179,8 +179,9 @@ struct SsCwArgs {
     uint8_t *wstate;                   // [batch][nb^3][16]
     unsigned long long *evals;         // optional work counter: candidate evaluations of the certification (lane-level)
     uint32_t *taken;                   // work-list entries handed out beyond the first wave (zero at launch)
-    float g1, g2, g3;                  // cubic bound in d^2: g = G0 + g1 d2 + g2 d2^2 + g3 d2^3 (G_k / h^(2k), host-computed)
-    float r0sq, r1sq;                  // ring radii squared: (0.55 h)^2, (0.76 h)^2
+    float cs;                          // coordinate scale of the bound: 2^-e with h cs in [1, 2) (exact in f32)
+    float g1, g2, g3;                  // cubic bound in scaled d^2: g = G0 + g1 d2 + g2 d2^2 + g3 d2^3 (G_k / (h cs)^(2k), host-computed)
+    float r0sq, r1sq;                  // ring radii squared, unscaled: (0.55 h)^2, (0.76 h)^2
 };
 
 #define SS_CW_PAIRS 24                 // capacity of one sub-box's ring-0 list in candidate PAIRS (bulk fluid: ~13); extra candidates are dropped (sound)
@@ -201,12 +202,14 @@ __device__ __forceinline__ float ss_axis_d2(float u, float lo, float hi) { const
 
 // Folds the candidates flagged in `mword` (bit = index into wrec) into the two running lower bounds of a lane (points k, k + 1):
 //   d^2 = (dz, dz')^2 + (dx^2 + dy^2),  sum += max(g(d^2), 0) * V   with g = G0 + g1 d2 + g2 d2^2 + g3 d2^3 <= W / sigma.
+// Distances are in coordinates scaled by cs (SsCwArgs): the point is stored scaled, a staged record is scaled by the fused
+// multiply-add that takes the difference (r cs is exact, so this rounds like (r - g) cs).
 // Two candidates per iteration (independent accumulators); an odd tail re-reads the last record with zero volume.
-struct SsCwPoint { float gx, gy; ss_f2 ngz; float g1, g2, g3; };
+struct SsCwPoint { float gx, gy; ss_f2 ngz; float cs, g1, g2, g3; };
 __device__ __forceinline__ void ss_cw_eval(const SsCwPoint &Q, const float4 r, const float vol, ss_f2 &sum) {
-    const float dx = r.x - Q.gx, dy = r.y - Q.gy;
+    const float dx = fmaf(r.x, Q.cs, -Q.gx), dy = fmaf(r.y, Q.cs, -Q.gy);
     const float t = fmaf(dx, dx, dy * dy);
-    const ss_f2 dz = ss_add2(ss_pack(r.z, r.z), Q.ngz);
+    const ss_f2 dz = ss_fma2(ss_pack(r.z, r.z), ss_pack(Q.cs, Q.cs), Q.ngz);
     const ss_f2 d2 = ss_fma2(dz, dz, ss_pack(t, t));
     ss_f2 g = ss_fma2(d2, ss_pack(Q.g3, Q.g3), ss_pack(Q.g2, Q.g2));
     g = ss_fma2(d2, g, ss_pack(Q.g1, Q.g1));
@@ -329,16 +332,17 @@ __device__ __forceinline__ unsigned long long ss_cw_brick(const SsDev &P, const 
     // ---- level 1: per candidate, ring-0 membership for the eight sub-boxes (bit b = a * 4 + bb * 2 + cc: upper half in x, y, z)
     const int nwords = (C + 31) >> 5;
     const int pmax = P.np - 1;
-    // world coordinates of the half-brick point intervals [lo, hi] per axis (culling only; same expression as ss_lane_point's box)
+    // world coordinates of the half-brick point intervals [lo, hi] per axis (culling only; the grid points' own expressions, so
+    // that the intervals contain the points: ss_grid_xy / ss_grid_z)
     float xl0, xl1, xh0, xh1, yl0, yl1, yh0, yh1, zl0, zl1, zh0, zh1;
     {
         const int ox = bx * 8, oy = by * 8, oz = bz * 8;
-        xl0 = fmaf((float)(T.gbase[0] + min(ox, pmax)), P.c, P.gmin[0]);     xh0 = fmaf((float)(T.gbase[0] + min(ox + 3, pmax)), P.c, P.gmin[0]);
-        xl1 = fmaf((float)(T.gbase[0] + min(ox + 4, pmax)), P.c, P.gmin[0]); xh1 = fmaf((float)(T.gbase[0] + min(ox + 7, pmax)), P.c, P.gmin[0]);
-        yl0 = fmaf((float)(T.gbase[1] + min(oy, pmax)), P.c, P.gmin[1]);     yh0 = fmaf((float)(T.gbase[1] + min(oy + 3, pmax)), P.c, P.gmin[1]);
-        yl1 = fmaf((float)(T.gbase[1] + min(oy + 4, pmax)), P.c, P.gmin[1]); yh1 = fmaf((float)(T.gbase[1] + min(oy + 7, pmax)), P.c, P.gmin[1]);
-        zl0 = fmaf((float)(T.gbase[2] + min(oz, pmax)), P.c, P.gmin[2]);     zh0 = fmaf((float)(T.gbase[2] + min(oz + 3, pmax)), P.c, P.gmin[2]);
-        zl1 = fmaf((float)(T.gbase[2] + min(oz + 4, pmax)), P.c, P.gmin[2]); zh1 = fmaf((float)(T.gbase[2] + min(oz + 7, pmax)), P.c, P.gmin[2]);
+        xl0 = ss_grid_xy(P, T.gbase[0] + min(ox, pmax), 0);     xh0 = ss_grid_xy(P, T.gbase[0] + min(ox + 3, pmax), 0);
+        xl1 = ss_grid_xy(P, T.gbase[0] + min(ox + 4, pmax), 0); xh1 = ss_grid_xy(P, T.gbase[0] + min(ox + 7, pmax), 0);
+        yl0 = ss_grid_xy(P, T.gbase[1] + min(oy, pmax), 1);     yh0 = ss_grid_xy(P, T.gbase[1] + min(oy + 3, pmax), 1);
+        yl1 = ss_grid_xy(P, T.gbase[1] + min(oy + 4, pmax), 1); yh1 = ss_grid_xy(P, T.gbase[1] + min(oy + 7, pmax), 1);
+        zl0 = ss_grid_z(P, T.gbase[2] + min(oz, pmax), sparse);     zh0 = ss_grid_z(P, T.gbase[2] + min(oz + 3, pmax), sparse);
+        zl1 = ss_grid_z(P, T.gbase[2] + min(oz + 4, pmax), sparse); zh1 = ss_grid_z(P, T.gbase[2] + min(oz + 7, pmax), sparse);
     }
     // ---- pre-filter: candidates within ring 0 of the whole brick, compacted (sub-box distances are never smaller)
     int n0 = 0;
@@ -386,7 +390,7 @@ __device__ __forceinline__ unsigned long long ss_cw_brick(const SsDev &P, const 
                 const int pos = cnt_ + __popc(bal & ((1u << lane) - 1u));                                                \
                 if (((m >> (s4)) & 1u) && pos < 2 * SS_CW_PAIRS) {                                                       \
                     SsCwPair &E = S.list[s4][pos >> 1];                                                                  \
-                    E.x[pos & 1] = r.x; E.y[pos & 1] = r.y; E.z[pos & 1] = r.z; E.v[pos & 1] = r.w;                      \
+                    E.x[pos & 1] = r.x * A.cs; E.y[pos & 1] = r.y * A.cs; E.z[pos & 1] = r.z * A.cs; E.v[pos & 1] = r.w; \
                 }                                                                                                        \
                 cnt_ = min(cnt_ + __popc(bal), 2 * SS_CW_PAIRS);                                                         \
             }
@@ -408,14 +412,13 @@ __device__ __forceinline__ unsigned long long ss_cw_brick(const SsDev &P, const 
             const int i = i0 + li, j = j0 + lj, k = k0 + lk;
             const bool row_ok = i <= pmax && j <= pmax;
             const bool vA = row_ok && k <= pmax, vB = row_ok && k + 1 <= pmax;
-            // grid point coordinates from GLOBAL indices, the reference's expressions (ss_lane_point)
-            const float gx = __fadd_rn(__fmul_rn((float)(T.gbase[0] + i), P.c), P.gmin[0]);
-            const float gy = __fadd_rn(__fmul_rn((float)(T.gbase[1] + j), P.c), P.gmin[1]);
-            const float fkA = (float)(T.gbase[2] + k), fkB = (float)(T.gbase[2] + k + 1);
-            const float gzA = sparse ? __fadd_rn(P.gmin[2], __fmul_rn(fkA, P.c)) : __fmaf_rn(fkA, P.c, P.gmin[2]);
-            const float gzB = sparse ? __fadd_rn(P.gmin[2], __fmul_rn(fkB, P.c)) : __fmaf_rn(fkB, P.c, P.gmin[2]);
+            // grid point coordinates from GLOBAL indices, the reference's expressions, scaled like the list entries
+            const float gx = ss_grid_xy(P, T.gbase[0] + i, 0) * A.cs;
+            const float gy = ss_grid_xy(P, T.gbase[1] + j, 1) * A.cs;
+            const float gzA = ss_grid_z(P, T.gbase[2] + k, sparse) * A.cs;
+            const float gzB = ss_grid_z(P, T.gbase[2] + k + 1, sparse) * A.cs;
             SsCwPoint Q;
-            Q.gx = gx; Q.gy = gy; Q.ngz = ss_pack(-gzA, -gzB); Q.g1 = A.g1; Q.g2 = A.g2; Q.g3 = A.g3;
+            Q.gx = gx; Q.gy = gy; Q.ngz = ss_pack(-gzA, -gzB); Q.cs = A.cs; Q.g1 = A.g1; Q.g2 = A.g2; Q.g3 = A.g3;
             const int ns4 = s4 == 0 ? cnt0 : (s4 == 1 ? cnt1 : (s4 == 2 ? cnt2 : cnt3));
             const int npairs = (ns4 + 1) >> 1;
             ss_f2 sumA = ss_pack(0.0f, 0.0f), sumB = ss_pack(0.0f, 0.0f);

@@ -528,14 +528,14 @@ __device__ __forceinline__ SsLanePoint ss_lane_point(const SsDev &P, const SsTil
     L.gi = T.gbase[0] + L.i; L.gj = T.gbase[1] + L.j; L.gk = T.gbase[2] + L.k;
     // grid point coordinates from GLOBAL indices: x, y = mul then add, z fused in the AVX path
     // (dense_subdomains.rs:1068, :1101-1102); scalar path: point_coordinates (uniform_grid.rs:418-425)
-    L.gx = __fadd_rn(__fmul_rn((float)L.gi, P.c), P.gmin[0]);
-    L.gy = __fadd_rn(__fmul_rn((float)L.gj, P.c), P.gmin[1]);
-    L.gz = sparse ? __fadd_rn(P.gmin[2], __fmul_rn((float)L.gk, P.c)) : __fmaf_rn((float)L.gk, P.c, P.gmin[2]);
+    L.gx = ss_grid_xy(P, L.gi, 0);
+    L.gy = ss_grid_xy(P, L.gj, 1);
+    L.gz = ss_grid_z(P, L.gk, sparse);
     const int i1 = min(W.i0 + W.dx - 1, P.np - 1), j1 = min(W.j0 + W.dy - 1, P.np - 1), k1 = min(W.k0 + W.dz - 1, P.np - 1);
     L.k1 = k1;
-    L.bxl = fmaf((float)(T.gbase[0] + W.i0), P.c, P.gmin[0]); L.bxh = fmaf((float)(T.gbase[0] + i1), P.c, P.gmin[0]);
-    L.byl = fmaf((float)(T.gbase[1] + W.j0), P.c, P.gmin[1]); L.byh = fmaf((float)(T.gbase[1] + j1), P.c, P.gmin[1]);
-    L.bzl = fmaf((float)(T.gbase[2] + W.k0), P.c, P.gmin[2]); L.bzh = fmaf((float)(T.gbase[2] + k1), P.c, P.gmin[2]);
+    L.bxl = ss_grid_xy(P, T.gbase[0] + W.i0, 0); L.bxh = ss_grid_xy(P, T.gbase[0] + i1, 0);
+    L.byl = ss_grid_xy(P, T.gbase[1] + W.j0, 1); L.byh = ss_grid_xy(P, T.gbase[1] + j1, 1);
+    L.bzl = ss_grid_z(P, T.gbase[2] + W.k0, sparse); L.bzh = ss_grid_z(P, T.gbase[2] + k1, sparse);
     L.out_idx = (size_t)tile_idx * P.np * P.np * P.np + ((size_t)L.i * P.np + L.j) * P.np + L.k;
     return L;
 }

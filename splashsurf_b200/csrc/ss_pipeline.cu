@@ -863,7 +863,11 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
             c->nflag.ensure(8);                                  // work-list counter of the persistent warps (the fix-up sweep re-zeroes it)
             CK(cudaMemsetAsync(c->nflag.p, 0, 4, st));
             W.taken = c->nflag.as<uint32_t>();
-            const double ih2 = 1.0 / ((double)D.h * (double)D.h);
+            // the bound runs in coordinates scaled by cs = 2^-e, h cs in [1, 2): the coefficients are O(1) at every h (G3 / h^6
+            // in absolute units leaves the f32 range outside about 1e-6 < h < 1e6), and the scaling is exact in f32
+            const int e = std::ilogb(D.h);
+            const double hs = std::ldexp((double)D.h, -e), ih2 = 1.0 / (hs * hs);
+            W.cs = std::ldexp(1.0f, -e);
             W.g1 = (float)((double)SS_G1 * ih2); W.g2 = (float)((double)SS_G2 * ih2 * ih2); W.g3 = (float)((double)SS_G3 * ih2 * ih2 * ih2);
             W.r0sq = 0.3025f * D.h2; W.r1sq = 0.58f * D.h2;
             const bool cw_small = certify_runs <= 16;            // at most 4 candidate bins per axis (3 + the extension plane)
@@ -1053,6 +1057,20 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     }
     if ((double)nsd[0] * (double)nsd[1] * (double)nsd[2] >= 2147483647.0) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many subdomain slots");
     if (S > 1024) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "subdomain_num_cubes_per_dim > 1024 is not supported");
+    {
+        // Far from the origin f32 grid coordinates round by a visible fraction of a cell.  The splat bins place a particle by its
+        // cell with no slack for that rounding (DESIGN.md 4.3).  The limit ulp / c <= 1/64 is a tested one, not a derived bound:
+        // up to it the device matches the oracle and the oracle matches the reference's binary; at 1/32 the latter pin fails.
+        double amax = 0.0;
+        for (int d = 0; d < 3; ++d) amax = std::max({ amax, std::fabs((double)gg.mn[d]), std::fabs((double)gg.mx[d]) });
+        const double ulp = std::ldexp(1.0, std::ilogb(std::max(amax, 1e-30)) - 23);
+        if (ulp > (double)cs / 64.0) {
+            char msg[200];
+            snprintf(msg, sizeof msg, "grid coordinates up to %.6g round by %.3g cells (ulp / cube size > 1/64): too far from the origin for the "
+                     "device level set at this cube size; translate the particles towards the origin", amax, ulp / (double)cs);
+            return ss_fail(SS_ERR_REAL_TOO_SMALL, msg);
+        }
+    }
 
     SsDev D{};
     for (int d = 0; d < 3; ++d) { D.gmin[d] = gg.mn[d]; D.nsd[d] = (int)nsd[d]; }

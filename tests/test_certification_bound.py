@@ -1,5 +1,6 @@
 """CPU tests of the invariant behind the level-set certification pass (DESIGN.md 4.3): the cubic g(s) used by
 `ss_certify_box` never exceeds the kernel shape, and partial sums built from it never exceed the reference's exact value."""
+import math
 import os
 import re
 
@@ -32,6 +33,33 @@ def test_cubic_is_a_lower_bound_of_the_kernel_shape():
     q = np.linspace(0, 1.2, 240001)
     cap = 32 * np.sum(np.maximum(0.0, g0 + q * q * (g1 + q * q * (g2 + q * q * g3))) * q * q) * (q[1] - q[0])
     assert 0.93 < cap < 1.0          # captures ~94 % of the kernel's volume integral
+
+
+def _device_coefficients(h):
+    """k_certify_warp's operands as the host computes them (ss_pipeline.cu): coordinates scaled by cs = 2^-e with h cs in [1, 2),
+    coefficients G_k / (h cs)^(2k) in double, rounded to f32."""
+    g0, g1, g2, g3 = _coeffs()
+    h = float(np.float32(h))
+    e = math.frexp(h)[1] - 1                                     # ilogb
+    hs = math.ldexp(h, -e)
+    ih2 = 1.0 / (hs * hs)
+    return np.float32(math.ldexp(1.0, -e)), np.float32(g0), np.float32(g1 * ih2), np.float32(g2 * ih2 ** 2), np.float32(g3 * ih2 ** 3)
+
+
+def test_scaled_bound_is_below_the_kernel_shape_at_every_length_scale():
+    """At every power-of-two h of the reference's f32 window, and at h with mantissas across [1, 2): the f32 Horner bound on
+    scaled squared distances, with the host's coefficients, never exceeds the kernel shape.  Absolute-unit coefficients failed this
+    from h ~ 1e7 (G3 / h^6 denormal, then zero) and certified nothing below h ~ 5e-7 (overflow)."""
+    s = np.concatenate([np.linspace(0, 1.0, 200_001), np.linspace(1.0, 9.0, 20_001)])
+    hs = [0.1 * 2.0 ** k for k in range(-40, 41)] + [2.0 ** k for k in range(-40, 41)] + list(np.linspace(1.0, 1.999, 37))
+    for h in hs:
+        cs, g0, g1, g2, g3 = _device_coefficients(h)
+        assert all(np.isfinite(x) and (x == 0 or abs(x) >= np.finfo(np.float32).tiny) for x in (g1, g2, g3)), h
+        h32 = np.float64(np.float32(h))
+        d2 = (s * (h32 * float(cs)) ** 2).astype(np.float32)       # scaled squared distances, as the kernel forms them
+        g = np.maximum(np.float32(0), g0 + d2 * (g1 + d2 * (g2 + d2 * g3)))
+        q = np.sqrt(d2.astype(np.float64)) / (h32 * float(cs))
+        assert (g.astype(np.float64) <= _f(q) + 2e-6).all(), h
 
 
 def test_partial_sums_never_exceed_the_exact_level_set(oracle_mod):
