@@ -150,9 +150,11 @@ def interpolate_quantity(particles, densities, rest_mass, h, values, points, fir
     corr = np.zeros(len(p), dtype=np.float64)
     np.add.at(corr, i, w.astype(np.float64))
     num = num.astype(F)
-    if first_order_correction:
-        with np.errstate(invalid="ignore", divide="ignore"):
+    with np.errstate(invalid="ignore", divide="ignore"):
+        if first_order_correction:
             num = (num * (F(1.0) / corr.astype(F))[:, None]).astype(F)
+        else:                                      # :252-254: 0 * (1 / 0) + 1 is NaN for an empty sum as well
+            num[corr.astype(F) == 0] = np.nan
     return num if vec else num[:, 0]
 
 
@@ -173,9 +175,10 @@ def weighted_neighbor_counts(particles, h) -> np.ndarray:
 
 
 def smoothing_weights(vertex_weighted_num_neighbors, normalization: float) -> np.ndarray:
-    """reconstruct.rs:1220-1231: x = min(max(n - 0, 0) / normalization, 1); 6 x^5 - 15 x^4 + 10 x^3."""
+    """reconstruct.rs:1220-1231: x = min(max(n - 0, 0) / normalization, 1); 6 x^5 - 15 x^4 + 10 x^3.  Rust's f32::max ignores
+    NaN (NaN.max(0) = 0), so a NaN count (a vertex without particles in range) gets the weight 0: np.fmax, not np.maximum."""
     n = np.asarray(vertex_weighted_num_neighbors, dtype=F)
-    x = np.minimum((np.maximum(n, F(0.0)) / F(normalization)).astype(F), F(1.0)).astype(F)
+    x = np.minimum((np.fmax(n, F(0.0)) / F(normalization)).astype(F), F(1.0)).astype(F)
     x3 = (x * x * x).astype(F); x4 = (x3 * x).astype(F); x5 = (x4 * x).astype(F)
     return ((x5 * F(6.0)).astype(F) - (x4 * F(15.0)).astype(F) + (x3 * F(10.0)).astype(F)).astype(F)
 

@@ -1195,9 +1195,15 @@ k_sph_normals(SsDev P, SsNrmArgs A) {
     float gx = 0.0f, gy = 0.0f, gz = 0.0f;
     if (found >= 0) {
         const float dqdr = __fdiv_rn(2.0f, P.h);
+        // A brick's range covers the reach of its grid points, [8b - R, 8b + 7 + R); the vertex lies anywhere on its edge from lp
+        // to lp + 1, so the upper end is taken from the brick of lp + 1 (which differs from lp's when lp % 8 == 7).
         int2 rng[3];
 #pragma unroll
-        for (int d = 0; d < 3; ++d) { const int lp = g[d] - t[d] * P.S; rng[d] = A.bins.brick_rng[min(lp >> 3, P.nb - 1)]; }
+        for (int d = 0; d < 3; ++d) {
+            const int lp = g[d] - t[d] * P.S;
+            rng[d] = A.bins.brick_rng[min(lp >> 3, P.nb - 1)];
+            rng[d].y = A.bins.brick_rng[min((lp + 1) >> 3, P.nb - 1)].y;
+        }
         for (int X = rng[0].x; X <= rng[0].y; ++X) for (int Y = rng[1].x; Y <= rng[1].y; ++Y) {
             uint32_t a;
             const uint32_t len = ss_bin_column(P, A.bins.bin_start, A.bins.bin_end, (uint32_t)found, X, Y, rng[2].x, rng[2].y, a);
