@@ -226,7 +226,7 @@ int ss_surface_timings(const ss_surface *s, ss_timings *out);
  * the stage received.  Writes min(n, SS_LSP_N) counters to out[SS_LSP_*] and returns SS_LSP_N (negative: NULL surface).
  * Host bookkeeping of values the stage reads back anyway (no device work, no synchronisation).
  * - fallback cascades, bricks each tier received (tier t + 1 receives what tier t could not take; the last tier takes all):
- *   exact pass, fix-up pass (variant 2) and anisotropic level set;
+ *   exact pass, fix-up pass (variant 2), anisotropic level set and averaged-position surface (appended after BIN_CELLS);
  * - certification: work bricks of k_certify_warp with the 384- or 576-candidate slice (variant 2), of k_certify (variant 1), or
  *   of the fused k_levelset (variant 0, exact everywhere, or more than 32 candidate bin runs per brick);
  * - the GLOBAL and COUNT template flags of the launches (0 / 1), R = ceil(h / cube_size) and the bin width in cells. */
@@ -249,7 +249,10 @@ int ss_surface_timings(const ss_surface *s, ss_timings *out);
 #define SS_LSP_COUNT_PAIRS   16
 #define SS_LSP_R             17
 #define SS_LSP_BIN_CELLS     18
-#define SS_LSP_N             19
+#define SS_LSP_AVG_512       19
+#define SS_LSP_AVG_4096      20
+#define SS_LSP_AVG_SELECT    21
+#define SS_LSP_N             22
 int ss_surface_levelset_paths(const ss_surface *s, uint64_t *out, int n);
 
 /* Tuning knobs (do not change results).
@@ -305,6 +308,22 @@ int ss_context_set_anisotropy_f32(ss_context *ctx, const ss_anisotropy_f32 *anis
 int ss_surface_copy_anisotropy(const ss_surface *s, float *xbar, float *g);
 /* Device time of the anisotropy stage (weighted PCA per particle), ms; 0 without anisotropic kernels.  ss_timings.density excludes it. */
 float ss_surface_anisotropy_ms(const ss_surface *s);
+
+/* ---- Averaged-position surface (Y. Zhu and R. Bridson, "Animating Sand as a Fluid", ACM TOG 24(3), 2005; specification in
+ * DESIGN.md section 12).  At every grid point g the particles within h of g are averaged with the weights k(s) = (1 - s^2)^3,
+ * s = |x_j - g| / h, and the level set is
+ *     f(g) = h - |g - x_bar(g)|   (f = 0 where no particle reaches),   surface f = h - R_s,   R_s = radius_factor * particle_radius
+ * so the surface lies at distance R_s from the local weighted average of the particles: a smooth free surface without the blobs
+ * of the density iso-surface.  iso_surface_threshold is not used in this mode.  R_s must lie in (0, compact support radius),
+ * otherwise the reconstruction returns SS_ERR_INVALID_PARAMETER.  Opt-in per context (NULL = off, the default); exclusive with
+ * ss_context_set_anisotropy_f32 (both on: SS_ERR_INVALID_PARAMETER).  Grid, densities (bit for bit), marching cubes and stitching
+ * are unchanged.  Subdomain path only, as for anisotropic kernels: spatial_decomposition = 0 returns SS_ERR_UNSUPPORTED, the
+ * decomposition is always used, and ss_reconstruct_partition_f32 / _cb_f32 return SS_ERR_UNSUPPORTED.  SPH normals and the [bins]
+ * post-processing entries below keep the SPH kernel at the particle positions. */
+typedef struct ss_averaged_surface_f32 {
+    float radius_factor;                 /* R_s / particle_radius, finite and > 0; default 1 */
+} ss_averaged_surface_f32;
+int ss_context_set_averaged_surface_f32(ss_context *ctx, const ss_averaged_surface_f32 *avg /* NULL = off */);
 
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.

@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "Anisotropy", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -76,12 +76,17 @@ class _Timings(C.Structure):
 # ss_surface_levelset_paths: counter names in index order (SS_LSP_* of include/splashsurf_b200.h)
 LEVELSET_PATHS = ("exact_512", "exact_1024", "exact_4096", "exact_select", "fixup_512", "fixup_1024", "fixup_4096", "fixup_select",
                   "aniso_512", "aniso_4096", "aniso_select", "cert_warp_384", "cert_warp_576", "cert_cta", "cert_fused",
-                  "global", "count_pairs", "R", "bin_cells")
+                  "global", "count_pairs", "R", "bin_cells", "avg_512", "avg_4096", "avg_select")
 
 
 class _Anisotropy(C.Structure):
     """ss_anisotropy_f32 (include/splashsurf_b200.h)."""
     _fields_ = [("smoothing", C.c_float), ("max_stretch", C.c_float), ("min_neighbors", C.c_uint32)]
+
+
+class _AveragedSurface(C.Structure):
+    """ss_averaged_surface_f32 (include/splashsurf_b200.h)."""
+    _fields_ = [("radius_factor", C.c_float)]
 
 
 _LIB = None
@@ -191,6 +196,7 @@ def _bind(L):
     L.ss_meshio_set_chunk_items.argtypes = [u64]
     L.ss_context_set_anisotropy_f32.argtypes = [vp, C.POINTER(_Anisotropy)]
     L.ss_surface_copy_anisotropy.argtypes = [vp, vp, vp]
+    L.ss_context_set_averaged_surface_f32.argtypes = [vp, C.POINTER(_AveragedSurface)]
     L.ss_surface_anisotropy_ms.argtypes = [vp]
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
@@ -617,15 +623,38 @@ class Anisotropy:
         return _Anisotropy(float(np.float32(self.smoothing)), float(np.float32(self.max_stretch)), int(self.min_neighbors))
 
 
-def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Optional[Anisotropy]):
-    """ctx.reconstruct_raw with the context's anisotropy set for this one call (and reset whatever happens)."""
+@dataclass(frozen=True)
+class AveragedSurface:
+    """Averaged-position surface after Zhu & Bridson (ACM TOG 24(3), 2005) for the level set; DESIGN.md section 12.
+
+    At every grid point g the particles within the compact support radius h of g are averaged with the weights
+    ``(1 - |x_j - g|^2 / h^2)^3``, and the level set is ``f(g) = h - |g - x_bar(g)|`` (0 where no particle reaches).  The surface
+    is ``f = h - radius_factor * particle_radius``: it lies at distance ``radius_factor * particle_radius`` from the local
+    weighted average of the particles, which gives a smooth free surface without the blobs of the density iso-surface.
+    ``iso_surface_threshold`` is not used in this mode, and ``radius_factor * particle_radius`` must lie between 0 and h.
+
+    Scope: grid, densities (bit for bit), marching cubes and stitching are unchanged; SPH normals and attribute interpolation keep
+    the SPH kernel at the particle positions.  Requires ``subdomain_grid=True`` (always decomposed), one GPU, and cannot be combined
+    with ``anisotropy``."""
+    radius_factor: float = 1.0
+
+    def _abi(self) -> _AveragedSurface:
+        return _AveragedSurface(float(np.float32(self.radius_factor)))
+
+
+def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Optional[Anisotropy],
+                     averaged_surface: Optional[AveragedSurface] = None):
+    """ctx.reconstruct_raw with the context's anisotropy and averaged surface set for this one call (and reset whatever happens)."""
     L = ctx._L
-    _check(L, L.ss_context_set_anisotropy_f32(ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
     try:
+        _check(L, L.ss_context_set_anisotropy_f32(ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
+        _check(L, L.ss_context_set_averaged_surface_f32(ctx._h, C.byref(averaged_surface._abi()) if averaged_surface is not None else None))
         return ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
     finally:
         if anisotropy is not None:
             L.ss_context_set_anisotropy_f32(ctx._h, None)
+        if averaged_surface is not None:
+            L.ss_context_set_averaged_surface_f32(ctx._h, None)
 
 
 def _collect_anisotropy(ctx: "Context", s, res: "SurfaceReconstruction"):
@@ -1008,13 +1037,14 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                         subdomain_grid: bool = True, subdomain_grid_auto_disable: bool = True,
                         subdomain_num_cubes_per_dim: int = 64, context: Optional[Context] = None,
                         keep_levelset_tile_of: Optional[int] = None, with_debug: bool = False, sph_normals: bool = False,
-                        anisotropy: Optional[Anisotropy] = None) -> SurfaceReconstruction:
+                        anisotropy: Optional[Anisotropy] = None, averaged_surface: Optional[AveragedSurface] = None) -> SurfaceReconstruction:
     """Performs a surface reconstruction from the given particles (no post-processing) on the GPU.
 
     Same signature and semantics as ``pysplashsurf.reconstruct_surface``; ``particles`` is an (N, 3) float32
     array (float64 input is not provided by the device path and raises, like an unsupported dtype does in the
     reference, pysplashsurf/src/reconstruction.rs:204-206).  ``anisotropy=Anisotropy(...)`` switches the level set to anisotropic
-    kernels (not part of the reference; see ``Anisotropy``).
+    kernels, ``averaged_surface=AveragedSurface(...)`` to the averaged-position surface (neither is part of the reference; see
+    ``Anisotropy`` and ``AveragedSurface``).
     """
     arr = np.asarray(particles)
     if arr.dtype != np.float32:
@@ -1031,7 +1061,7 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1 if keep_levelset_tile_of is None else int(keep_levelset_tile_of)))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, int(bool(sph_normals))))
-    s = _reconstruct_raw(ctx, arr, p, anisotropy)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface)
     try:
         res = _collect(ctx, s, len(arr), p, with_debug or keep_levelset_tile_of is not None, keep_levelset_tile_of is not None)
         if anisotropy is not None:
@@ -1253,7 +1283,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                             mesh_smoothing_iters: Optional[int] = None, mesh_smoothing_weights: bool = True,
                             mesh_smoothing_weights_normalization: float = 13.0, output_mesh_smoothing_weights: bool = False,
                             output_raw_normals: bool = False, output_raw_mesh: bool = False, context: Optional[Context] = None,
-                            with_debug: bool = False, anisotropy: Optional[Anisotropy] = None, **post):
+                            with_debug: bool = False, anisotropy: Optional[Anisotropy] = None,
+                            averaged_surface: Optional[AveragedSurface] = None, **post):
     """``pysplashsurf.reconstruction_pipeline`` (pysplashsurf/src/pipeline.rs:109-200) on the GPU: surface reconstruction plus
     the post-processing steps of splashsurf/src/reconstruct.rs:1094-1391 that run on the device -- smoothing weights, weighted
     Laplacian smoothing, SPH or area-weighted normals (at the smoothed vertices), normal smoothing and SPH interpolation of
@@ -1265,8 +1296,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     ``quad_max_edge_diag_ratio`` / ``quad_max_normal_angle`` / ``quad_max_interior_angle``) runs last (reconstruct.rs:1410-1441, host):
     the returned mesh is then a MixedTriQuadMesh3d.  ``mesh_aabb_min`` / ``mesh_aabb_max`` (+ ``mesh_aabb_clamp_vertices``) clamp the
     finished mesh (reconstruct.rs:1394-1408) and ``check_mesh_closed`` / ``check_mesh_manifold`` raise SplashsurfError with the
-    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy`` as in
-    ``reconstruct_surface``."""
+    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy`` and
+    ``averaged_surface`` as in ``reconstruct_surface``."""
     passive = ("mesh_cleanup", "decimate_barnacles", "mesh_cleanup_snap_dist", "keep_vertices", "generate_quads", "quad_max_edge_diag_ratio",
                "quad_max_normal_angle", "quad_max_interior_angle", "mesh_aabb_min", "mesh_aabb_max", "mesh_aabb_clamp_vertices",
                "check_mesh_closed", "check_mesh_manifold", "check_mesh_orientation", "check_mesh_debug")
@@ -1295,7 +1326,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, 0))
-    s = _reconstruct_raw(ctx, arr, p, anisotropy)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface)
     try:
         rec = _collect(ctx, s, len(arr), p, with_debug, False)                  # raw mesh, densities, grids
         if anisotropy is not None:

@@ -116,6 +116,9 @@ def main(argv=None):
     r.add_argument("--aniso-smoothing", type=float, default=0.9)                      # kernel-centre smoothing lambda in [0, 1]
     r.add_argument("--aniso-max-stretch", type=float, default=4.0)                    # longest / shortest kernel axis, >= 1
     r.add_argument("--aniso-min-neighbors", type=int, default=10)                     # fewer neighbours: isotropic kernel
+    # averaged-position surface (Zhu & Bridson 2005; splashsurf_b200.AveragedSurface, DESIGN.md section 12) -- not part of the reference CLI
+    r.add_argument("--averaged-surface", choices=["on", "off"], default="off")
+    r.add_argument("--averaged-radius-factor", type=float, default=None)              # surface at radius_factor * particle radius from x_bar (default 1)
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -254,8 +257,15 @@ def reconstruct(a) -> int:
         raise ValueError("--double-precision=on: the device path reconstructs float32 particles only (SURVEY.md 8b)")
     if on(a.partition) and on(a.anisotropic):
         raise ValueError("--anisotropic=on is not available with --partition=on: anisotropic kernels run on one GPU per frame")
-    from . import Anisotropy
+    if on(a.partition) and on(a.averaged_surface):
+        raise ValueError("--averaged-surface=on is not available with --partition=on: the averaged-position surface runs on one GPU per frame")
+    if on(a.anisotropic) and on(a.averaged_surface):
+        raise ValueError("--averaged-surface=on and --anisotropic=on are exclusive: choose one level set")
+    from . import Anisotropy, AveragedSurface
     aniso = Anisotropy(a.aniso_smoothing, a.aniso_max_stretch, a.aniso_min_neighbors) if on(a.anisotropic) else None
+    if a.averaged_radius_factor is not None and not on(a.averaged_surface):
+        raise ValueError("--averaged-radius-factor applies to the averaged-position surface: add --averaged-surface=on")
+    avg = AveragedSurface(1.0 if a.averaged_radius_factor is None else a.averaged_radius_factor) if on(a.averaged_surface) else None
     paths = collect_paths(a)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)
@@ -301,10 +311,11 @@ def reconstruct(a) -> int:
                     keep_vertices=on(a.keep_verts), generate_quads=on(a.generate_quads), quad_max_edge_diag_ratio=a.quad_max_edge_diag_ratio,
                     quad_max_normal_angle=a.quad_max_normal_angle, quad_max_interior_angle=a.quad_max_interior_angle, mesh_aabb_min=mmin,
                     mesh_aabb_max=mmax, mesh_aabb_clamp_vertices=on(a.mesh_aabb_clamp_verts), check_mesh_closed=closed, check_mesh_manifold=manifold,
-                    check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso, **base)
+                    check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso,
+                    averaged_surface=avg, **base)
                 raw = rec.mesh
             else:
-                raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, **base).mesh
+                raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, averaged_surface=avg, **base).mesh
                 out = MeshWithData(raw, {}, {})
             dt = time.perf_counter() - t
             quads = out.mesh.get_quads() if on(a.generate_quads) else None

@@ -6,10 +6,11 @@
 //   k_aniso             per particle in its owning subdomain: weighted mean and covariance of its density neighbourhood (the
 //                       density stage's walk, ss_nbr_walk), cyclic Jacobi, clamped stretch -> x_bar, G (6 entries), det G
 //   k_records_aniso     splat records (x_bar, V det G) + the G entries of every binned membership
-//   k_aniso_levelset    warp per 8^3-point brick over the non-empty-brick work list: candidates of the brick's bins sorted by
+//   k_fold_levelset     warp per 8^3-point brick over the non-empty-brick work list: candidates of the brick's bins sorted by
 //                       particle index, per 4x4x4 sub-box the candidates within h of the sub-box, two grid points per lane;
 //                       bricks with more candidates than the slice go to a 4096-slot instantiation, beyond that to
-//                       k_aniso_select (O(C^2) selection in index order)
+//                       k_fold_select (O(C^2) selection in index order).  Templated on the fold: SsAnisoFold here, SsAvgFold
+//                       (averaged-position surface, ss_averaged.cuh)
 // Every value the level set writes is exact; there is no certification in this mode.
 #pragma once
 
@@ -189,8 +190,31 @@ __device__ __forceinline__ SsAnBrick ss_an_brick(const SsDev &P, const SsAnArgs 
     return N;
 }
 
-template <int CAP>
-__device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A, unsigned long long *s_key, uint16_t *s_list, uint32_t work, int lane) {
+// The level sets of this file and of ss_averaged.cuh fold every candidate within h of a grid point, in ascending particle index,
+// into per-point accumulators.  A fold F supplies
+//   F::Cand  F::load(A, src)                      what the fold reads of record src
+//   F::Acc   F::zero()                            the accumulators of one grid point
+//   void     F::add(P, cand, gx, gy, gz, acc)     one candidate at the grid point (gx, gy, gz); tests its own support
+//   float    F::value(P, acc)                     the tile value
+// and the brick kernels below stage, order and cull the candidates once for every fold.  A fold's support must lie within the
+// isotropic ball of radius h around the record's position (the sub-box cull).
+
+// phi(x) = sum_j V_j det G_j W(|G_j (x - x_bar_j)|) (DESIGN.md §11)
+struct SsAnisoFold {
+    struct Cand { float4 r, g0, g1; };
+    struct Acc { float phi; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) {
+        return Cand{ A.bins.rec[src], A.grec[2 * (size_t)src], A.grec[2 * (size_t)src + 1] };
+    }
+    static __device__ __forceinline__ Acc zero() { return Acc{ 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        a.phi = ss_aniso_term(P, c.r, c.g0, c.g1, gx, gy, gz, a.phi);
+    }
+    static __device__ __forceinline__ float value(const SsDev &, const Acc &a) { return a.phi; }
+};
+
+template <class F, int CAP>
+__device__ __forceinline__ void ss_fold_brick(const SsDev &P, const SsAnArgs &A, unsigned long long *s_key, uint16_t *s_list, uint32_t work, int lane) {
     const uint32_t brick_lin = A.bricks[work];
     const SsAnBrick N = ss_an_brick(P, A, brick_lin);
     if (A.bstate && lane == 0) A.bstate[brick_lin] = 2;
@@ -201,7 +225,7 @@ __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A
         for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
         C += len;
     }
-    if (C == 0) return;                                      // pre-zeroed tile: phi = 0 exactly
+    if (C == 0) return;                                      // pre-zeroed tile: the value of a point without candidates is 0
     if (C > (uint32_t)CAP) {
         if (lane == 0) A.fallback[1 + atomicAdd(&A.fallback[0], 1u)] = brick_lin;
         return;
@@ -225,8 +249,8 @@ __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A
     const SsSubLane L = ss_sub_lane(P, lane);
     const float cull2 = P.h2 * 1.0001f;
     for (int b = 0; b < 8; ++b) {
-        // grid point coordinates: point_coordinates (uniform_grid.rs:418-425), min + index * cell; culling box: |G d| >= |d|
-        // because every eigenvalue of G is >= 1
+        // grid point coordinates: point_coordinates (uniform_grid.rs:418-425), min + index * cell; culling box: every fold's support
+        // lies within distance h of the record's position
         const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
         if (!X.inside) continue;
         int nlist = 0;
@@ -242,41 +266,41 @@ __device__ __forceinline__ void ss_aniso_brick(const SsDev &P, const SsAnArgs &A
             nlist += __popc(mword);
         }
         __syncwarp();
-        float phiA = 0.0f, phiB = 0.0f;
+        typename F::Acc accA = F::zero(), accB = F::zero();
         for (int n = 0; n < nlist; ++n) {
-            const uint32_t src = (uint32_t)s_key[s_list[n]];
-            const float4 r = A.bins.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
-            phiA = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzA, phiA);
-            phiB = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzB, phiB);
+            const typename F::Cand cd = F::load(A, (uint32_t)s_key[s_list[n]]);
+            F::add(P, cd, X.gx, X.gy, X.gzA, accA);
+            F::add(P, cd, X.gx, X.gy, X.gzB, accB);
         }
-        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = phiA;
-        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = phiB;
+        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = F::value(P, accA);
+        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = F::value(P, accB);
         __syncwarp();                                        // the list is rebuilt for the next sub-box
     }
 }
 
-template <int CAP, int WARPS>
+template <class F, int CAP, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
-k_aniso_levelset(SsDev P, SsAnArgs A) {
+k_fold_levelset(SsDev P, SsAnArgs A) {
     __shared__ unsigned long long s_key[WARPS][CAP];
     __shared__ uint16_t s_list[WARPS][CAP];
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t work = blockIdx.x * WARPS + wib;
     if (work >= A.n_bricks) return;
-    ss_aniso_brick<CAP>(P, A, s_key[wib], s_list[wib], work, lane);
+    ss_fold_brick<F, CAP>(P, A, s_key[wib], s_list[wib], work, lane);
 }
 
 // Bricks with more candidates than the largest slice (extreme clustering): one warp per brick walks the candidates in
 // ascending particle index by repeated selection of the next key, O(C^2 / 32), and folds each into its 16 grid points.
+template <class F>
 __global__ void __launch_bounds__(32)
-k_aniso_select(SsDev P, SsAnArgs A) {
+k_fold_select(SsDev P, SsAnArgs A) {
     if (blockIdx.x >= A.n_bricks) return;
     const int lane = threadIdx.x & 31;
     const SsAnBrick N = ss_an_brick(P, A, A.bricks[blockIdx.x]);
     const SsSubLane L = ss_sub_lane(P, lane);
-    float phi[16];
+    typename F::Acc acc[16];
 #pragma unroll
-    for (int q = 0; q < 16; ++q) phi[q] = 0.0f;
+    for (int q = 0; q < 16; ++q) acc[q] = F::zero();
     unsigned long long last = 0;
     bool first = true;
     for (;;) {
@@ -292,20 +316,19 @@ k_aniso_select(SsDev P, SsAnArgs A) {
         for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
         if (best == ~0ull) break;
         last = best; first = false;
-        const uint32_t src = (uint32_t)best;
-        const float4 r = A.bins.rec[src], g0 = A.grec[2 * (size_t)src], g1 = A.grec[2 * (size_t)src + 1];
+        const typename F::Cand cd = F::load(A, (uint32_t)best);
 #pragma unroll
         for (int b = 0; b < 8; ++b) {
             const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
-            phi[2 * b] = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzA, phi[2 * b]);
-            phi[2 * b + 1] = ss_aniso_term(P, r, g0, g1, X.gx, X.gy, X.gzB, phi[2 * b + 1]);
+            F::add(P, cd, X.gx, X.gy, X.gzA, acc[2 * b]);
+            F::add(P, cd, X.gx, X.gy, X.gzB, acc[2 * b + 1]);
         }
     }
     float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
 #pragma unroll
     for (int b = 0; b < 8; ++b) {
         const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
-        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = phi[2 * b];
-        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = phi[2 * b + 1];
+        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = F::value(P, acc[2 * b]);
+        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = F::value(P, acc[2 * b + 1]);
     }
 }

@@ -9,6 +9,7 @@
 #include "ss_certify.cuh"
 #include "ss_exact.cuh"
 #include "ss_aniso.cuh"
+#include "ss_averaged.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
 
@@ -132,6 +133,8 @@ struct ss_context {
     int sph_normals = 0;             // 1: SPH normals at the mesh vertices (sph_interpolation.rs:82-133)
     int an_on = 0;                   // 1: anisotropic kernels (ss_aniso.cuh) with the parameters `an`
     ss_anisotropy_f32 an{};
+    int avg_on = 0;                  // 1: averaged-position surface (ss_averaged.cuh) with the parameters `avg`
+    ss_averaged_surface_f32 avg{};
     cudaEvent_t ev_an[2] = { nullptr, nullptr };
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
@@ -365,6 +368,13 @@ extern "C" int ss_context_set_anisotropy_f32(ss_context *c, const ss_anisotropy_
     if (!(a->smoothing >= 0.0f && a->smoothing <= 1.0f)) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropy smoothing must lie in [0, 1]");
     if (!(a->max_stretch >= 1.0f) || !std::isfinite(a->max_stretch)) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropy max_stretch must be finite and >= 1");
     c->an = *a; c->an_on = 1;
+    return SS_OK;
+}
+extern "C" int ss_context_set_averaged_surface_f32(ss_context *c, const ss_averaged_surface_f32 *a) {
+    if (!c) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL context");
+    if (!a) { c->avg_on = 0; return SS_OK; }
+    if (!(a->radius_factor > 0.0f) || !std::isfinite(a->radius_factor)) return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface radius_factor must be finite and > 0");
+    c->avg = *a; c->avg_on = 1;
     return SS_OK;
 }
 
@@ -804,25 +814,27 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
     }, ls_launches, received);
 }
 
-// Anisotropic level set of one batch (ss_aniso.cuh): work list of non-empty bricks without extension tasks (the single-point
-// planes of the last brick are bricks of their own), warp-per-brick kernel, then the 4096-slot slice, then selection.  Every
-// listed brick gets state 2 (exact values).  Returns the length of the work list.
-static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, uint64_t &ls_launches, uint64_t *received) {
+// Warp-per-brick level set of one batch for the fold F (anisotropic kernels, ss_aniso.cuh, or the averaged-position surface,
+// ss_averaged.cuh): work list of non-empty bricks without extension tasks (the single-point planes of the last brick are bricks of
+// their own), the 512-slot slice, then the 4096-slot slice, then selection.  Every listed brick gets state 2 (exact values).
+// Returns the length of the work list.
+template <class F>
+static uint32_t launch_fold_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, const float4 *grec, uint64_t &ls_launches, uint64_t *received) {
     SsDev Dw = D;
     Dw.ext_bricks = 0;
     const uint32_t n_work = build_worklist(c, Dw, nbatch);
     const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left, uint8_t *bstate) {
         SsAnArgs A{};
-        A.bins = context_bins(c); A.grec = c->an_grec.as<float4>(); A.bricks = list; A.n_bricks = n; A.tiles = c->tiles.as<float>();
+        A.bins = context_bins(c); A.grec = grec; A.bricks = list; A.n_bricks = n; A.tiles = c->tiles.as<float>();
         A.bstate = bstate; A.fallback = left;
         return A;
     };
     run_cascade(c, c->list_ls.as<uint32_t>(), n_work, {
         [&](const uint32_t *list, uint32_t n, uint32_t *left) {
-            LAUNCH(c, (k_aniso_levelset<SS_AN_CAP, SS_AN_WARPS>), (n + SS_AN_WARPS - 1) / SS_AN_WARPS, SS_AN_WARPS * 32, Dw, args(list, n, left, c->bstate.as<uint8_t>()));
+            LAUNCH(c, (k_fold_levelset<F, SS_AN_CAP, SS_AN_WARPS>), (n + SS_AN_WARPS - 1) / SS_AN_WARPS, SS_AN_WARPS * 32, Dw, args(list, n, left, c->bstate.as<uint8_t>()));
         },
-        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_aniso_levelset<SS_AN_BIG_CAP, 1>), n, 32, Dw, args(list, n, left, nullptr)); },
-        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_aniso_select, n, 32, Dw, args(list, n, left, nullptr)); },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_fold_levelset<F, SS_AN_BIG_CAP, 1>), n, 32, Dw, args(list, n, left, nullptr)); },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_fold_select<F>, n, 32, Dw, args(list, n, left, nullptr)); },
     }, ls_launches, received);
     return n_work;
 }
@@ -831,7 +843,7 @@ static uint32_t launch_aniso_levelset(ss_context *c, const SsDev &D, uint32_t nb
 // exact pass), brick classification, fix-up sweep.  Leaves the tiles, the per-brick states and the marching-cubes brick list
 // (c->list_mc, *n_mc_out entries) in the context scratch.
 static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsigned nbricks, bool exact_all, int certify_runs, bool global_mode,
-                          ss_surface *out, uint64_t &ls_launches, uint64_t &fix_points, uint32_t *n_mc_out) {
+                          bool averaged, ss_surface *out, uint64_t &ls_launches, uint64_t &fix_points, uint32_t *n_mc_out) {
     cudaStream_t st = c->stream;
     SsLsArgs A{};
     A.bins = context_bins(c); A.tiles = c->tiles.as<float>();
@@ -839,10 +851,13 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     A.mode = exact_all ? SS_LS_EXACT_ALL : SS_LS_CERTIFY;
     A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = c->bstate.as<uint8_t>();
     uint64_t *const paths = out->ls_paths;
-    const uint32_t n_work = D.aniso ? launch_aniso_levelset(c, D, nbatch, ls_launches, paths + SS_LSP_ANISO_512) : build_worklist(c, D, nbatch);
+    const bool folded = D.aniso || averaged;            // warp-per-brick fold cascade, exact values only
+    const uint32_t n_work = D.aniso ? launch_fold_levelset<SsAnisoFold>(c, D, nbatch, c->an_grec.as<float4>(), ls_launches, paths + SS_LSP_ANISO_512)
+                          : averaged ? launch_fold_levelset<SsAvgFold>(c, D, nbatch, nullptr, ls_launches, paths + SS_LSP_AVG_512)
+                          : build_worklist(c, D, nbatch);
     A.work_list = c->list_ls.as<uint32_t>();
-    const bool split_certify = !D.aniso && c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
-    if (n_work && !split_certify && !D.aniso) {
+    const bool split_certify = !folded && c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
+    if (n_work && !split_certify && !folded) {
         launch_levelset(c, dim3(n_work), D, A, c->count_pairs != 0, global_mode); ++ls_launches;
         paths[SS_LSP_CERT_FUSED] += n_work;
     }
@@ -1041,6 +1056,8 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     // anisotropic kernels (ss_aniso.cuh): a kernel centre moves up to smoothing * h < h from its particle, so memberships need a
     // margin of 2h; the neighbourhood-search grids and cell lists stay on the standard margin (bit-identical densities)
     const bool aniso = c->an_on && !global_mode && !part.enabled && !part.given_rho;
+    // averaged-position surface (ss_averaged.cuh): kernel centres at the particles, standard margins and bins; surface f = h - R_s
+    const bool averaged = c->avg_on && !global_mode && !part.enabled && !part.given_rho;
     const float margin = aniso ? member_margin(fmulr(2.0f, h), cs) : ns_margin;
     int64_t nsd[3], ncg[3];
     for (int d = 0; d < 3; ++d) { nsd[d] = (PP.grid.nc[d] + S - 1) / S; ncg[d] = nsd[d] * S; }
@@ -1078,6 +1095,13 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     rc = set_member_margin(D, margin);
     if (rc) return rc;
     D.thr = p->iso_surface_threshold; D.grow = fmulr(ns_margin, 1.5f);
+    if (averaged) {
+        // DESIGN.md §12: 0 < R_s < h, so that t = h - R_s > 0 and a point no particle reaches (f = 0) lies outside
+        const float rs = fmulr(c->avg.radius_factor, p->particle_radius);
+        if (!(rs > 0.0f && rs < h) || !std::isfinite(rs))
+            return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface: radius_factor * particle_radius must lie in (0, compact support radius)");
+        D.thr = fsubr(h, rs);
+    }
     D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)ns_margin) / (double)h) + 3;
     D.ns_stride = D.nsD * D.nsD * D.nsD;
     D.simd = p->enable_simd ? 1 : 0;
@@ -1263,7 +1287,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     float ls_ms = 0.f, mc_ms = 0.f, setup_ms = 0.f;
     uint64_t ls_launches = 0, fix_points = 0;
     out->tile.clear();
-    const bool exact_all = c->ls_exact_all || c->keep_tile_flat >= 0 || aniso;
+    const bool exact_all = c->ls_exact_all || c->keep_tile_flat >= 0 || aniso || averaged;
     for (uint32_t s0 = 0; s0 < nown; s0 += (uint32_t)max_tiles) {
         const uint32_t nbatch = std::min<uint32_t>((uint32_t)max_tiles, nown - s0);
         for (uint32_t q = 0; q < nbatch; ++q) {
@@ -1289,7 +1313,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
             setup_ms += su;
         }
         uint32_t n_mc = 0;
-        rc = levelset_batch(c, D, nbatch, nbricks, exact_all, certify_runs, global_mode, out, ls_launches, fix_points, &n_mc);
+        rc = levelset_batch(c, D, nbatch, nbricks, exact_all, certify_runs, global_mode, averaged, out, ls_launches, fix_points, &n_mc);
         if (rc) return rc;
         CK(cudaEventRecord(c->ev[11], st));
         // optional parity tap
@@ -1643,6 +1667,7 @@ static int reconstruct_partition_impl(ss_context *c, const float *xyz, uint64_t 
     if (rc) return rc;
     if (p->has_particle_aabb) return ss_fail(SS_ERR_UNSUPPORTED, "filter particles before partitioning (particle_aabb is applied by the caller)");
     if (c->an_on) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels are not available on partitioned (multi-GPU) reconstructions");
+    if (c->avg_on) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface is not available on partitioned (multi-GPU) reconstructions");
     if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "partitioned reconstruction requires the subdomain grid");
     if (axis < 0 || axis > 2 || own_lo < 0 || own_hi < own_lo || halo < 0) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad partition");
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
@@ -1712,7 +1737,12 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
         s->n = P.n; s->grid = P.grid;
         // decomposition decision, lib.rs:421-464
         int use_dec = 0;
-        if (c->an_on) {
+        if (c->an_on && c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropic kernels and the averaged-position surface are exclusive");
+        if (c->avg_on) {
+            // averaged-position surface: subdomain path only, always decomposed (no auto-disable)
+            if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface requires the subdomain grid (spatial_decomposition = UniformGrid)");
+            use_dec = 1;
+        } else if (c->an_on) {
             // anisotropic kernels: subdomain path only, always decomposed (no auto-disable)
             if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels require the subdomain grid (spatial_decomposition = UniformGrid)");
             use_dec = 1;

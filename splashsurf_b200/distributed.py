@@ -216,12 +216,16 @@ def _pinned(t: torch.Tensor, device) -> torch.Tensor:
 class Runner:
     """Drives one reconstruct step on this rank's GPU (world == 1: plain C-ABI call)."""
 
-    def __init__(self, ctx, params, world: int, rank: int, local_rank: int, group=None, device=None, protocol: str = "stats", anisotropy=None):
+    def __init__(self, ctx, params, world: int, rank: int, local_rank: int, group=None, device=None, protocol: str = "stats", anisotropy=None,
+                 averaged_surface=None):
         self.ctx, self.params, self.world, self.rank, self.local_rank, self.group = ctx, params, world, rank, local_rank, group
-        # anisotropic kernels (splashsurf_b200.Anisotropy): single GPU only -- the slab partition does not provide them
+        # anisotropic kernels (splashsurf_b200.Anisotropy) and the averaged-position surface (splashsurf_b200.AveragedSurface):
+        # single GPU only -- the slab partition does not provide them
         if anisotropy is not None and world > 1:
             raise ValueError("anisotropic kernels are not available on multi-GPU (partitioned) reconstructions; run them on one GPU")
-        self.anisotropy = anisotropy
+        if averaged_surface is not None and world > 1:
+            raise ValueError("the averaged-position surface is not available on multi-GPU (partitioned) reconstructions; run it on one GPU")
+        self.anisotropy, self.averaged_surface = anisotropy, averaged_surface
         # how the global maximum subdomain population (sparse rule) reaches the library: "stats" (default) = the plan statistics
         # count the members of every subdomain with the exact classifier (ss_partition_members_f32), their all-reduced maximum
         # is passed to ONE library call; "two_call" = decomposition pre-pass, all-reduce, full call (one more library call per step);
@@ -278,14 +282,18 @@ class Runner:
     # -- single GPU
     def _step_single(self, xyz_ptr: int, n: int, copy_out: bool, params=None, force_copy: bool = False) -> dict:
         L = self.ctx._L
-        if self.anisotropy is not None:
-            from . import _check
-            _check(L, L.ss_context_set_anisotropy_f32(self.ctx._h, C.byref(self.anisotropy._abi())))
+        from . import _check
         try:
+            if self.anisotropy is not None:
+                _check(L, L.ss_context_set_anisotropy_f32(self.ctx._h, C.byref(self.anisotropy._abi())))
+            if self.averaged_surface is not None:
+                _check(L, L.ss_context_set_averaged_surface_f32(self.ctx._h, C.byref(self.averaged_surface._abi())))
             s = self.ctx.reconstruct_raw(xyz_ptr, n, self.params if params is None else params)
         finally:
             if self.anisotropy is not None:
                 L.ss_context_set_anisotropy_f32(self.ctx._h, None)
+            if self.averaged_surface is not None:
+                L.ss_context_set_averaged_surface_f32(self.ctx._h, None)
         keep = self.keep_surface and self.world == 1
         try:
             out = self._collect(s, copy_out, n_local=n, force_copy=force_copy)
@@ -750,7 +758,7 @@ class DistributedReconstructor:
     `reconstruction_pipeline` is a single-GPU step."""
 
     def __init__(self, *, sph_normals: bool = False, group=None, device=None, protocol: str = "stats", local_rank: Optional[int] = None,
-                 anisotropy=None, **params):
+                 anisotropy=None, averaged_surface=None, **params):
         import os
         import splashsurf_b200 as ss
         if not dist.is_initialized():
@@ -762,7 +770,9 @@ class DistributedReconstructor:
         self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
         if anisotropy is not None and self.world > 1:
             raise ValueError("anisotropic kernels are not available on multi-GPU (partitioned) reconstructions; run them on one GPU")
-        self.anisotropy = anisotropy
+        if averaged_surface is not None and self.world > 1:
+            raise ValueError("the averaged-position surface is not available on multi-GPU (partitioned) reconstructions; run it on one GPU")
+        self.anisotropy, self.averaged_surface = anisotropy, averaged_surface
         lr = int(os.environ.get("LOCAL_RANK", "0")) if local_rank is None else int(local_rank)
         self.ctx = ss.Context(lr if device is None else 0)
         self.sph_normals = bool(sph_normals)
@@ -778,7 +788,8 @@ class DistributedReconstructor:
         ss = self._ss
         p = np.ascontiguousarray(particles_local, dtype=np.float32).reshape(-1, 3)
         if self.world == 1:
-            r = ss.reconstruct_surface(p, context=self.ctx, sph_normals=self.sph_normals, anisotropy=self.anisotropy, **self._kw)
+            r = ss.reconstruct_surface(p, context=self.ctx, sph_normals=self.sph_normals, anisotropy=self.anisotropy,
+                                       averaged_surface=self.averaged_surface, **self._kw)
             return ss.MeshWithData(r.mesh, {"normals": r.normals} if self.sph_normals and r.normals is not None else {}, {})
         if self._aabb is not None:                    # lib.rs:369-406: particles outside the half-open box take no part
             p = np.ascontiguousarray(p[np.all(p >= self._aabb[0], axis=1) & np.all(p < self._aabb[1], axis=1)])
