@@ -101,17 +101,17 @@ __device__ __forceinline__ void ss_aniso_matrix(const SsDev &P, float (&a)[3][3]
 __global__ void __launch_bounds__(128)
 k_aniso(SsDev P, uint32_t m, const uint32_t *__restrict__ list, const uint32_t *__restrict__ list_off, const uint32_t *__restrict__ list_flag,
         const uint32_t *__restrict__ key, const float4 *__restrict__ spos, const uint32_t *__restrict__ sub_flat,
-        const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend, float *__restrict__ xbar, float *__restrict__ gmat,
+        const uint32_t *__restrict__ off, float *__restrict__ xbar, float *__restrict__ gmat,
         float *__restrict__ gdet) {
     const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= list_off[m - 1] + list_flag[m - 1]) return;
-    const uint32_t e = list[tid];
-    const float4 pi = spos[e];
+    const SsWalk W = ss_walk_sub(P, list[tid], key, sub_flat, off);
+    const float4 pi = spos[W.e];
     const uint32_t p = __float_as_uint(pi.w);
     // weighted mean of the offsets x_j - x_i (self: w = 1, offset 0)
     float sw = 1.0f, mx = 0.0f, my = 0.0f, mz = 0.0f;
     uint32_t nn = 0;
-    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &, float dx, float dy, float dz, float d2) {
+    ss_nbr_walk(P, W, pi, spos, [&](const float4 &, float dx, float dy, float dz, float d2) {
         const float q = __fdiv_rn(__fsqrt_rn(d2), P.h);
         const float w = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(q, q), q));
         sw = __fadd_rn(sw, w);
@@ -126,7 +126,7 @@ k_aniso(SsDev P, uint32_t m, const uint32_t *__restrict__ list, const uint32_t *
         c00 = __fmul_rn(ex, ex); c01 = __fmul_rn(ex, ey); c02 = __fmul_rn(ex, ez);
         c11 = __fmul_rn(ey, ey); c12 = __fmul_rn(ey, ez); c22 = __fmul_rn(ez, ez);
     }
-    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &, float dx, float dy, float dz, float d2) {
+    ss_nbr_walk(P, W, pi, spos, [&](const float4 &, float dx, float dy, float dz, float d2) {
         const float q = __fdiv_rn(__fsqrt_rn(d2), P.h);
         const float w = __fsub_rn(1.0f, __fmul_rn(__fmul_rn(q, q), q));
         const float ex = __fsub_rn(dx, ux), ey = __fsub_rn(dy, uy), ez = __fsub_rn(dz, uz);

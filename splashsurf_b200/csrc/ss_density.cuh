@@ -1,4 +1,4 @@
-// ss_density.cuh -- SPH particle densities, cell-cooperative kernel (sm_90a).  NOT the default; its speed on the H100 has not been measured.
+// ss_density.cuh -- SPH particle densities, cell-cooperative kernel (sm_90a).  NOT the default; slower than k_density on the H100 (DESIGN.md section 6).
 //
 // An attempt to replace the thread-per-particle k_density (ss_kernels.cuh), whose warps leave many lanes idle
 // (every lane walks its own 27 cell runs and its own hit list).  The pair test is only ~10 instructions, so the per-chunk bookkeeping
@@ -54,7 +54,7 @@ struct SsDcArgs {
     const uint32_t *list, *list_off, *list_flag;       // compacted first entries of the listed cells; length = list_off[m-1] + list_flag[m-1]
     const uint32_t *key;                               // NS key of every entry (subdomain * ns_stride + cell)
     const float4 *spos;                                // NS-sorted positions
-    const uint32_t *sub_flat, *cstart, *cend;
+    const uint32_t *sub_flat, *off;                    // cell offsets (k_cell_offsets)
     float *rho;
     unsigned long long *nbr_count;                     // optional
 };
@@ -62,14 +62,14 @@ struct SsDcArgs {
 // flag = 1 on the first entry of every h-cell run that holds at least one particle inside its subdomain's half-open AABB
 // (aabb.rs:220-222): those are the cells with densities to compute
 __global__ void k_density_cell_flags(SsDev P, uint32_t m, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-                                     const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cend, uint32_t *__restrict__ flag) {
+                                     const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ off, uint32_t *__restrict__ flag) {
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= m) return;
     const uint32_t k = key[e];
     uint32_t f = 0;
     if (e == 0 || key[e - 1] != k) {
         const SsSubGeom g = ss_sub_geom(P, sub_flat[k / (uint32_t)P.ns_stride]);
-        const uint32_t b = cend[k];
+        const uint32_t b = off[k + 1];
         for (uint32_t t = e; t < b && !f; ++t) {
             const float4 pi = spos[t];
             if ((pi.x >= g.smin[0] && pi.y >= g.smin[1] && pi.z >= g.smin[2]) && (pi.x < g.smax[0] && pi.y < g.smax[1] && pi.z < g.smax[2])) f = 1u;
@@ -94,7 +94,7 @@ __device__ __forceinline__ void ss_dc_flush(const SsDev &P, const SsDcArgs &A, S
             if (A.nbr_count) A.nbr_count[idx] = (unsigned long long)cnt;
             A.rho[idx] = __fmul_rn(acc, P.rest_mass);
         } else {
-            ss_density_entry<false>(P, e, A.key, A.spos, A.sub_flat, A.cstart, A.cend, A.rho, A.nbr_count, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
+            ss_density_entry<false>(P, ss_walk_sub(P, e, A.key, A.sub_flat, A.off), A.spos, A.rho, A.nbr_count, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
         }
     }
     __syncwarp();
@@ -127,7 +127,7 @@ k_density_cells(SsDev P, SsDcArgs A) {
         const uint32_t a0 = A.list[w];
         const uint32_t k = A.key[a0];
         const uint32_t s = k / (uint32_t)P.ns_stride, cell = k - s * (uint32_t)P.ns_stride;
-        const int nown = (int)(A.cend[k] - a0);
+        const int nown = (int)(A.off[k + 1] - a0);
         if (s != s_cached) { g = ss_sub_geom(P, A.sub_flat[s]); ns = ss_ns_grid(P, g); s_cached = s; }
         const int c0 = (int)cell / (P.nsD * P.nsD), c1 = ((int)cell / P.nsD) % P.nsD, c2 = (int)cell % P.nsD;
 
@@ -140,16 +140,9 @@ k_density_cells(SsDev P, SsDcArgs A) {
             const int q0 = c0 + lane / 3 - 1, q1 = c1 + lane % 3 - 1;
             if (q0 >= 0 && q1 >= 0 && q0 < ns.nc[0] && q1 < ns.nc[1]) {
                 const uint32_t kb = s * (uint32_t)P.ns_stride + (uint32_t)((q0 * P.nsD + q1) * P.nsD);
-                uint32_t a = 0xffffffffu, b = 0;
-#pragma unroll
-                for (int dz = -1; dz <= 1; ++dz) {
-                    const int q2 = c2 + dz;
-                    if (q2 < 0 || q2 >= ns.nc[2]) continue;
-                    const uint32_t st = A.cstart[kb + q2];
-                    if (st != 0xffffffffu) { if (a == 0xffffffffu) a = st; b = A.cend[kb + q2]; }
-                }
-                if (a != 0xffffffffu) { run_a = a; run_len = b - a; }
-                if (lane == 4) own_before = a0 - a;             // entries of the cell (0, 0, -1): they precede the own cell in its run
+                run_a = A.off[kb + (uint32_t)max(c2 - 1, 0)];
+                run_len = A.off[kb + (uint32_t)min(c2 + 1, ns.nc[2] - 1) + 1u] - run_a;
+                if (lane == 4) own_before = a0 - run_a;         // entries of the cell (0, 0, -1): they precede the own cell in its run
             }
         }
         uint32_t incl = run_len;
@@ -166,8 +159,8 @@ k_density_cells(SsDev P, SsDcArgs A) {
             for (int t = lane; t < nown; t += 32) {
                 const float4 pi = A.spos[a0 + t];
                 if ((pi.x >= g.smin[0] && pi.y >= g.smin[1] && pi.z >= g.smin[2]) && (pi.x < g.smax[0] && pi.y < g.smax[1] && pi.z < g.smax[2]))
-                    ss_density_entry<false>(P, a0 + t, A.key, A.spos, A.sub_flat, A.cstart, A.cend, A.rho, A.nbr_count, (const unsigned long long *)nullptr,
-                                            (uint32_t *)nullptr);
+                    ss_density_entry<false>(P, ss_walk_sub(P, a0 + t, A.key, A.sub_flat, A.off), A.spos, A.rho, A.nbr_count,
+                                            (const unsigned long long *)nullptr, (uint32_t *)nullptr);
             }
             continue;
         }

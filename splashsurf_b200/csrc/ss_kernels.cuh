@@ -205,6 +205,19 @@ __global__ void k_run_counts(const uint32_t *__restrict__ key, uint32_t m, uint3
     if (e == m - 1 || k != key[e + 1]) end[k] = e + 1;
 }
 
+// Cell offsets over a sorted key array, for k = 0 .. nkeys: off[k] = the first entry whose key is >= k (m if there is none).
+// Cell k holds the entries [off[k], off[k+1]), and a run of consecutive cells [klo, khi] the entries [off[klo], off[khi+1]).
+// Launched over m + 1 threads: entry e writes the keys in (key[e-1], key[e]], clipped to nkeys, and thread m fills up to nkeys,
+// so every slot is written once and the table needs no fill.  Keys >= nkeys (members k_ns_keys dropped) sort behind every cell
+// and lie in none.
+__global__ void k_cell_offsets(const uint32_t *__restrict__ key, uint32_t m, uint32_t *__restrict__ off, uint32_t nkeys) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e > m) return;
+    const uint32_t hi = e < m ? min(key[e], nkeys) : nkeys;
+    const uint32_t lo = e > 0 ? min(key[e - 1], nkeys) + 1u : 0u;
+    for (uint32_t k = lo; k <= hi; ++k) off[k] = e;
+}
+
 __global__ void k_gather_pos(const float *__restrict__ xyz, const uint32_t *__restrict__ pidx, uint32_t m,
                              float4 *__restrict__ out) {
     uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -213,14 +226,6 @@ __global__ void k_gather_pos(const float *__restrict__ xyz, const uint32_t *__re
     out[e] = make_float4(xyz[3 * (uint64_t)p], xyz[3 * (uint64_t)p + 1], xyz[3 * (uint64_t)p + 2], __uint_as_float(p));
 }
 
-#define SS_NS_LIST 96
-// One thread per (subdomain, particle) membership in NS-sorted order.  Particles contained in the
-// subdomain's AABB get rho = m * (W(0) + sum_j W(|xj - xi|)) with neighbours visited in the reference's
-// order: 26 adjacent cells in x-major (-1,0,1)^3 order, then the own cell; ascending particle index
-// inside a cell (neighborhood_search.rs:396-433, density_map.rs:169-185).
-// FILL = false: densities (+ optional neighbour counts); FILL = true: writes the neighbour indices (global particle ids, in
-// the reference's order) into the CSR array prepared from those counts (Parameters::global_neighborhood_list,
-// dense_subdomains.rs:617-639).
 // Membership entries whose particle lies inside its subdomain's half-open AABB (aabb.rs:220-222): only those get a density.
 // Roughly half of the entries are ghosts, so k_density runs over the compacted list of the others (full warps).
 __global__ void k_density_flags(SsDev P, uint32_t m, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
@@ -236,85 +241,179 @@ __global__ void k_density_flags(SsDev P, uint32_t m, const uint32_t *__restrict_
     flag[e] = inside ? 1u : 0u;
 }
 
-// Neighbour walk of ONE membership entry `e` (thread-serial): visit(pj, dx, dy, dz, d2) for every other particle with
-// d^2 < h^2, in the reference's order (26 adjacent cells x-major, then the own cell; ascending index inside a cell), with
-// dx = xj - xi.  Shared by the densities, the neighbour lists and the anisotropy of a particle (ss_aniso.cuh).
+// The neighbour cells of one entry as 12 runs of consecutive entries of the cell-sorted array, in the reference's visiting
+// order (26 adjacent cells x-major, then the own cell; ascending index inside a cell).  The three z-cells of an (x, y) column
+// have consecutive keys, so a column is one run:
+//   runs 0-3: columns (-1,-1), (-1,0), (-1,1), (0,-1);   run 4: cell (0,0,-1);   run 5: cell (0,0,+1);
+//   runs 6-9: columns (0,1), (1,-1), (1,0), (1,1);       runs 10, 11: the own cell before and after the entry itself.
+// Cells outside [0, nc) per dimension are clipped, as the reference skips them.
+#define SS_WALK_RUNS 12
+struct SsWalk {
+    const uint32_t *off;         // cell offsets (k_cell_offsets)
+    uint32_t base;               // key of the grid's cell (0, 0, 0)
+    uint32_t e;                  // the entry itself
+    int sx, sy;                  // key strides of x and y (z: 1)
+    int c[3], nc[3];             // own cell, cells per dimension
+};
+
+// per-subdomain grids: key = subdomain * ns_stride + x-major cell, padded to nsD per dimension
+__device__ __forceinline__ SsWalk ss_walk_sub(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key,
+                                              const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ off) {
+    const uint32_t k = key[e];
+    const uint32_t s = k / (uint32_t)P.ns_stride, cell = k - s * (uint32_t)P.ns_stride;
+    const SsNsGrid ns = ss_ns_grid(P, ss_sub_geom(P, sub_flat[s]));
+    SsWalk W;
+    W.off = off; W.base = s * (uint32_t)P.ns_stride; W.e = e; W.sx = P.nsD * P.nsD; W.sy = P.nsD;
+    W.c[0] = (int)cell / W.sx; W.c[1] = ((int)cell / P.nsD) % P.nsD; W.c[2] = (int)cell % P.nsD;
+    for (int d = 0; d < 3; ++d) W.nc[d] = ns.nc[d];
+    return W;
+}
+
+// the global path's grid over the whole domain: key = x-major cell
+__device__ __forceinline__ SsWalk ss_walk_global(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const uint32_t *__restrict__ off) {
+    const int cell = (int)key[e];
+    SsWalk W;
+    W.off = off; W.base = 0; W.e = e; W.sx = P.g_ns_nc[1] * P.g_ns_nc[2]; W.sy = P.g_ns_nc[2];
+    W.c[0] = cell / W.sx; W.c[1] = (cell / W.sy) % P.g_ns_nc[1]; W.c[2] = cell % W.sy;
+    for (int d = 0; d < 3; ++d) W.nc[d] = P.g_ns_nc[d];
+    return W;
+}
+
+// entries [t, b) of run r (empty: t == b)
+__device__ __forceinline__ void ss_walk_run(const SsWalk &W, const int r, uint32_t &t, uint32_t &b) {
+    if (r >= 10) {
+        const uint32_t own = W.base + (uint32_t)(W.c[0] * W.sx + W.c[1] * W.sy + W.c[2]);
+        if (r == 10) { t = W.off[own]; b = W.e; } else { t = W.e + 1u; b = W.off[own + 1]; }
+        return;
+    }
+    const int j = r < 4 ? r : (r < 6 ? 4 : r - 1);                       // column, (-1,0,1)^2 x-major
+    const int q0 = W.c[0] + j / 3 - 1, q1 = W.c[1] + j % 3 - 1;
+    const int zlo = max(r == 5 ? W.c[2] + 1 : W.c[2] - 1, 0), zhi = min(r == 4 ? W.c[2] - 1 : W.c[2] + 1, W.nc[2] - 1);
+    t = b = 0u;
+    if (q0 < 0 || q1 < 0 || q0 >= W.nc[0] || q1 >= W.nc[1] || zlo > zhi) return;
+    const uint32_t kb = W.base + (uint32_t)(q0 * W.sx + q1 * W.sy);
+    t = W.off[kb + zlo]; b = W.off[kb + zhi + 1];
+}
+
+// d^2 = |xj - xi|^2 with the reference's operation order; visit(pj, dx, dy, dz, d2) if d^2 < h^2
 template <typename F>
-__device__ __forceinline__ void ss_nbr_walk(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-                                            const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
-                                            F &&visit) {
-    uint32_t k = key[e];
-    uint32_t s = k / (uint32_t)P.ns_stride, cell = k - s * (uint32_t)P.ns_stride;
-    float4 pi = spos[e];
-    SsSubGeom g = ss_sub_geom(P, sub_flat[s]);
-    SsNsGrid ns = ss_ns_grid(P, g);
-    int c0 = (int)cell / (P.nsD * P.nsD), c1 = ((int)cell / P.nsD) % P.nsD, c2 = (int)cell % P.nsD;
-    const uint32_t base = s * (uint32_t)P.ns_stride;
-    for (int pass = 0; pass < 2; ++pass) {
-        for (int sx = -1; sx <= 1; ++sx) for (int sy = -1; sy <= 1; ++sy) for (int sz = -1; sz <= 1; ++sz) {
-            bool self = (sx == 0 && sy == 0 && sz == 0);
-            if ((pass == 0) == self) continue;
-            int q0 = c0 + sx, q1 = c1 + sy, q2 = c2 + sz;
-            if (q0 < 0 || q1 < 0 || q2 < 0 || q0 >= ns.nc[0] || q1 >= ns.nc[1] || q2 >= ns.nc[2]) continue;
-            uint32_t kk = base + (uint32_t)((q0 * P.nsD + q1) * P.nsD + q2);
-            uint32_t a = cstart[kk];
-            if (a == 0xffffffffu) continue;
-            uint32_t b = cend[kk];
-            for (uint32_t t = a; t < b; ++t) {
-                if (t == e) continue;
-                float4 pj = spos[t];
-                float dx = __fsub_rn(pj.x, pi.x), dy = __fsub_rn(pj.y, pi.y), dz = __fsub_rn(pj.z, pi.z);
-                float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-                if (d2 < P.h2) visit(pj, dx, dy, dz, d2);
-            }
+__device__ __forceinline__ void ss_nbr_pair(const SsDev &P, const float4 &pi, const float4 &pj, F &visit) {
+    const float dx = __fsub_rn(pj.x, pi.x), dy = __fsub_rn(pj.y, pi.y), dz = __fsub_rn(pj.z, pi.z);
+    const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    if (d2 < P.h2) visit(pj, dx, dy, dz, d2);
+}
+
+// Neighbour walk of ONE entry (thread-serial): visit(pj, dx, dy, dz, d2) for every other particle with d^2 < h^2, in the
+// reference's order, with dx = xj - xi.  Shared by the neighbour lists, the global path's densities, the fallback of the
+// cell-cooperative density kernel (ss_density.cuh) and the anisotropy of a particle (ss_aniso.cuh).
+template <typename F>
+__device__ __forceinline__ void ss_nbr_walk(const SsDev &P, const SsWalk &W, const float4 &pi, const float4 *__restrict__ spos, F &&visit) {
+    for (int r = 0; r < SS_WALK_RUNS; ++r) {
+        uint32_t t, b;
+        ss_walk_run(W, r, t, b);
+        for (; t + 1u < b; t += 2u) {                                     // two independent loads in flight
+            const float4 p0 = spos[t], p1 = spos[t + 1u];
+            ss_nbr_pair(P, pi, p0, visit);
+            ss_nbr_pair(P, pi, p1, visit);
         }
+        if (t < b) ss_nbr_pair(P, pi, spos[t], visit);
     }
 }
 
-// The ordered neighbour sum of ONE membership entry `e` (thread-serial): the per-particle routine of k_density and the
-// fallback of the cell-cooperative kernel (ss_density.cuh) for oversized cells.
+// The ordered neighbour sum of ONE entry (thread-serial), or with FILL its neighbour indices (global particle ids, in the
+// reference's order) written into the CSR array prepared from the counts (Parameters::global_neighborhood_list,
+// dense_subdomains.rs:617-639).
 template <bool FILL>
-__device__ __forceinline__ void ss_density_entry(const SsDev &P, const uint32_t e, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-                                                 const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
-                                                 float *__restrict__ rho, unsigned long long *__restrict__ nbr_count,
-                                                 const unsigned long long *__restrict__ nbr_off, uint32_t *__restrict__ nbr_idx) {
-    const float4 pi = spos[e];
-    // Phase 1 collects the squared distances of the neighbours (d^2 < h^2) in visiting order, phase 2 evaluates the kernel
-    // over that list: the expensive evaluation is then not executed for every candidate of the warp (only ~15 % of the
-    // candidates of the 27 cells are neighbours), and the summation order is unchanged.
-    float d2list[FILL ? 1 : SS_NS_LIST];
-    int nl = 0;
+__device__ __forceinline__ void ss_density_entry(const SsDev &P, const SsWalk &W, const float4 *__restrict__ spos, float *__restrict__ rho,
+                                                 unsigned long long *__restrict__ nbr_count, const unsigned long long *__restrict__ nbr_off,
+                                                 uint32_t *__restrict__ nbr_idx) {
+    const float4 pi = spos[W.e];
     unsigned long long ncount = 0;
     const unsigned long long fill_base = FILL ? nbr_off[__float_as_uint(pi.w)] : 0ull;
     float acc = ss_kernel_scalar(P, 0.0f);
-    ss_nbr_walk(P, e, key, spos, sub_flat, cstart, cend, [&](const float4 &pj, float, float, float, float d2) {
-        if constexpr (FILL) { nbr_idx[fill_base + ncount] = __float_as_uint(pj.w); ++ncount; }
-        else {
-            ++ncount;
-            if (nl == SS_NS_LIST) {      // list full (very dense cluster): drain it, order is preserved
-                for (int n = 0; n < SS_NS_LIST; ++n) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2list[n])));
-                nl = 0;
-            }
-            d2list[nl++] = d2;
-        }
+    ss_nbr_walk(P, W, pi, spos, [&](const float4 &pj, float, float, float, float d2) {
+        if constexpr (FILL) nbr_idx[fill_base + ncount] = __float_as_uint(pj.w);
+        else acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2)));
+        ++ncount;
     });
     if (FILL) return;
-    for (int n = 0; n < nl; ++n) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2list[n])));
     if (nbr_count) nbr_count[__float_as_uint(pi.w)] = ncount;
     rho[__float_as_uint(pi.w)] = __fmul_rn(acc, P.rest_mass);
 }
 
+// d^2 slots per thread of k_density's hit list (shared memory: SS_DENSITY_K * 4 B per thread)
+#define SS_DENSITY_K 16
+#define SS_DENSITY_BLOCK 128
+
+// One thread per membership entry of the compacted list (entries with the particle inside its subdomain, ascending):
+// rho = m * (W(0) + sum_j W(|xj - xi|)) with neighbours visited in the reference's order (neighborhood_search.rs:396-433,
+// density_map.rs:169-185), plus the optional neighbour counts.  FILL = true writes the neighbour lists instead (thread-serial).
+// The walk tests ~216 candidates for ~33 hits, so the kernel W(sqrt(d^2)) is not evaluated per candidate: every lane appends the
+// d^2 of its hits to its list in shared memory (slot s of lane l at [32 s + l] of the warp's region: no bank conflicts), and when
+// a lane's list may overflow in the next step the whole warp drains -- each lane folds its list into its sum in order, with all
+// lanes converged.  The summation order is the visiting order, as in the reference.  The warp walks the 12 runs together,
+// each run as long as its longest lane's, four candidates per step, and loads the next run's bounds while it walks the current one.
 template <bool FILL>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(SS_DENSITY_BLOCK)
 k_density(SsDev P, uint32_t m, const uint32_t *__restrict__ list, const uint32_t *__restrict__ list_off, const uint32_t *__restrict__ list_flag,
-          const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-          const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend,
+          const uint32_t *__restrict__ key, const float4 *__restrict__ spos, const uint32_t *__restrict__ sub_flat, const uint32_t *__restrict__ off,
           float *__restrict__ rho, unsigned long long *__restrict__ nbr_count, const unsigned long long *__restrict__ nbr_off,
           uint32_t *__restrict__ nbr_idx) {
-    // `list` holds the entries with a particle inside its subdomain (ascending); its length is list_off[m-1] + list_flag[m-1]
+    const uint32_t n_list = list_off[m - 1] + list_flag[m - 1];
     const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= list_off[m - 1] + list_flag[m - 1]) return;
-    ss_density_entry<FILL>(P, list[tid], key, spos, sub_flat, cstart, cend, rho, nbr_count, nbr_off, nbr_idx);
+    if constexpr (FILL) {
+        if (tid < n_list) ss_density_entry<true>(P, ss_walk_sub(P, list[tid], key, sub_flat, off), spos, rho, nbr_count, nbr_off, nbr_idx);
+    } else {
+        __shared__ float s_d2[SS_DENSITY_BLOCK * SS_DENSITY_K];
+        if ((tid & ~31u) >= n_list) return;                               // whole warps only: the drains are warp-wide
+        const bool live = tid < n_list;
+        float *const slot = s_d2 + (threadIdx.x & ~31u) * SS_DENSITY_K + (threadIdx.x & 31u);
+        SsWalk W{};
+        float4 pi = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        uint32_t t = 0u, b = 0u;
+        if (live) {
+            W = ss_walk_sub(P, list[tid], key, sub_flat, off);
+            pi = spos[W.e];
+            ss_walk_run(W, 0, t, b);
+        }
+        float acc = ss_kernel_scalar(P, 0.0f);
+        int nl = 0;
+        uint32_t ncount = 0;
+        auto drain = [&]() {
+            for (int s = 0; s < nl; ++s) acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(slot[32 * s])));
+            ncount += (uint32_t)nl;
+            nl = 0;
+        };
+        for (int r = 0; r < SS_WALK_RUNS; ++r) {
+            uint32_t tn = 0u, bn = 0u;
+            if (live && r + 1 < SS_WALK_RUNS) ss_walk_run(W, r + 1, tn, bn);
+            while (__any_sync(0xffffffffu, t < b)) {
+                if (t < b) {
+                    // four candidates per step with their loads issued together; a hit's d^2 is stored unconditionally at
+                    // the list's end and kept by advancing nl, so the step has no branches (nl <= K - 4 on entry)
+                    const uint32_t last = b - t - 1u;
+                    float4 q[4];
+#pragma unroll
+                    for (uint32_t i = 0; i < 4u; ++i) q[i] = spos[t + min(i, last)];
+#pragma unroll
+                    for (uint32_t i = 0; i < 4u; ++i) {
+                        const float dx = __fsub_rn(q[i].x, pi.x), dy = __fsub_rn(q[i].y, pi.y), dz = __fsub_rn(q[i].z, pi.z);
+                        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+                        slot[32 * nl] = d2;
+                        nl += (i <= last && d2 < P.h2) ? 1 : 0;
+                    }
+                    t += 4u;
+                }
+                if (__any_sync(0xffffffffu, nl > SS_DENSITY_K - 4)) drain();
+            }
+            t = tn; b = bn;
+        }
+        drain();
+        if (!live) return;
+        const uint32_t p = __float_as_uint(pi.w);
+        if (nbr_count) nbr_count[p] = ncount;
+        rho[p] = __fmul_rn(acc, P.rest_mass);
+    }
 }
 
 
@@ -336,44 +435,12 @@ __global__ void k_ns_keys_global(SsDev P, const float *__restrict__ xyz, uint32_
 }
 template <bool FILL>
 __global__ void __launch_bounds__(128)
-k_density_global(SsDev P, uint32_t n, const uint32_t *__restrict__ key, const float4 *__restrict__ spos,
-                 const uint32_t *__restrict__ cstart, const uint32_t *__restrict__ cend, float *__restrict__ rho,
-                 unsigned long long *__restrict__ nbr_count, const unsigned long long *__restrict__ nbr_off, uint32_t *__restrict__ nbr_idx) {
-    uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+k_density_global(SsDev P, uint32_t n, const uint32_t *__restrict__ key, const float4 *__restrict__ spos, const uint32_t *__restrict__ off,
+                 float *__restrict__ rho, unsigned long long *__restrict__ nbr_count, const unsigned long long *__restrict__ nbr_off,
+                 uint32_t *__restrict__ nbr_idx) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
-    const int cell = (int)key[e];
-    const int n1 = P.g_ns_nc[1], n2 = P.g_ns_nc[2];
-    const int c0 = cell / (n1 * n2), c1 = (cell / n2) % n1, c2 = cell % n2;
-    const float4 pi = spos[e];
-    float acc = ss_kernel_scalar(P, 0.0f);
-    unsigned long long ncount = 0;
-    const unsigned long long fill_base = FILL ? nbr_off[__float_as_uint(pi.w)] : 0ull;
-    for (int pass = 0; pass < 2; ++pass) {
-        for (int sx = -1; sx <= 1; ++sx) for (int sy = -1; sy <= 1; ++sy) for (int sz = -1; sz <= 1; ++sz) {
-            bool self = (sx == 0 && sy == 0 && sz == 0);
-            if ((pass == 0) == self) continue;
-            int q0 = c0 + sx, q1 = c1 + sy, q2 = c2 + sz;
-            if (q0 < 0 || q1 < 0 || q2 < 0 || q0 >= P.g_ns_nc[0] || q1 >= n1 || q2 >= n2) continue;
-            uint32_t kk = (uint32_t)((q0 * n1 + q1) * n2 + q2);
-            uint32_t a = cstart[kk];
-            if (a == 0xffffffffu) continue;
-            uint32_t b = cend[kk];
-            for (uint32_t t = a; t < b; ++t) {
-                if (t == e) continue;
-                float4 pj = spos[t];
-                float dx = __fsub_rn(pj.x, pi.x), dy = __fsub_rn(pj.y, pi.y), dz = __fsub_rn(pj.z, pi.z);
-                float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-                if (d2 < P.h2) {
-                    if (FILL) nbr_idx[fill_base + ncount] = __float_as_uint(pj.w);
-                    else acc = __fadd_rn(acc, ss_kernel_scalar(P, __fsqrt_rn(d2)));
-                    ++ncount;
-                }
-            }
-        }
-    }
-    if (FILL) return;
-    rho[__float_as_uint(pi.w)] = __fmul_rn(acc, P.rest_mass);
-    if (nbr_count) nbr_count[__float_as_uint(pi.w)] = ncount;
+    ss_density_entry<FILL>(P, ss_walk_global(P, e, key, off), spos, rho, nbr_count, nbr_off, nbr_idx);
 }
 
 // ------------------------------------------------------------------ splat binning ----

@@ -678,10 +678,8 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
     const uint64_t ns_keys = (uint64_t)nsub * D.ns_stride;
     // anisotropic mode: members outside the neighbourhood-search grid carry key 0xffffffff and sort behind every cell
     cub_sort(c, c->key_a.as<uint32_t>(), c->key_b.as<uint32_t>(), M, D.aniso ? 32 : bits_for(ns_keys), c->val_b.as<uint32_t>(), c->val_a.as<uint32_t>());
-    c->tab_a.ensure(ns_keys * 4); c->tab_b.ensure(ns_keys * 4);
-    CK(cudaMemsetAsync(c->tab_a.p, 0xff, ns_keys * 4, st));
-    LAUNCH(c, k_mark_starts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_a.as<uint32_t>(), (uint32_t)ns_keys);
-    LAUNCH(c, k_run_counts, nblk(M, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_b.as<uint32_t>(), (uint32_t)ns_keys);
+    c->tab_a.ensure((ns_keys + 1) * 4);                  // cell offsets
+    LAUNCH(c, k_cell_offsets, nblk((uint64_t)M + 1, 256), 256, c->key_b.as<uint32_t>(), M, c->tab_a.as<uint32_t>(), (uint32_t)ns_keys);
     c->spos.ensure((size_t)M * 16);
     LAUNCH(c, k_gather_pos, nblk(M, 256), 256, d_xyz, c->val_a.as<uint32_t>(), M, c->spos.as<float4>());
     unsigned long long *d_ncnt = nullptr;
@@ -691,28 +689,28 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
     if (c->density_variant >= 1 && !want_nbrs && !D.aniso) {
         // cell-cooperative kernel (ss_density.cuh): one warp per h-cell that holds a particle inside its subdomain (<= n cells), persistent grid
         LAUNCH(c, k_density_cell_flags, nblk(M, 256), 256, D, M, c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
-               c->tab_b.as<uint32_t>(), c->dflag.as<uint32_t>());
+               c->tab_a.as<uint32_t>(), c->dflag.as<uint32_t>());
         scan_compact(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
         SsDcArgs DA{};
         DA.m = M; DA.list = c->dlist.as<uint32_t>(); DA.list_off = c->doff.as<uint32_t>(); DA.list_flag = c->dflag.as<uint32_t>();
         DA.key = c->key_b.as<uint32_t>(); DA.spos = c->spos.as<float4>(); DA.sub_flat = c->sub_flat.as<uint32_t>();
-        DA.cstart = c->tab_a.as<uint32_t>(); DA.cend = c->tab_b.as<uint32_t>(); DA.rho = d_rho; DA.nbr_count = nullptr;
+        DA.off = c->tab_a.as<uint32_t>(); DA.rho = d_rho; DA.nbr_count = nullptr;
         const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * 7u, ((uint64_t)n + SS_DC_WARPS - 1) / SS_DC_WARPS);
         if (c->density_variant == 1) LAUNCH(c, k_density_cells<true>, std::max(grid, 1u), SS_DC_WARPS * 32, D, DA);
         else LAUNCH(c, k_density_cells<false>, std::max(grid, 1u), SS_DC_WARPS * 32, D, DA);
     } else {
     LAUNCH(c, k_density_flags, nblk(M, 256), 256, D, M, c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(), c->dflag.as<uint32_t>());
     scan_compact(c, c->dflag.as<uint32_t>(), c->doff.as<uint32_t>(), M, c->dlist.as<uint32_t>());
-    LAUNCH(c, k_density<false>, nblk(n, 128), 128, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
+    LAUNCH(c, k_density<false>, nblk(n, SS_DENSITY_BLOCK), SS_DENSITY_BLOCK, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
            c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
-           c->tab_a.as<uint32_t>(), c->tab_b.as<uint32_t>(), d_rho, d_ncnt, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
+           c->tab_a.as<uint32_t>(), d_rho, d_ncnt, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
     }
     if (want_nbrs) {
         const uint64_t total = scan_neighbor_counts(c, d_ncnt, n);
         out->nbr_idx.ensure(std::max<uint64_t>(total, 1) * 4);
-        LAUNCH(c, k_density<true>, nblk(n, 128), 128, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
+        LAUNCH(c, k_density<true>, nblk(n, SS_DENSITY_BLOCK), SS_DENSITY_BLOCK, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
                c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(),
-               c->tab_a.as<uint32_t>(), c->tab_b.as<uint32_t>(), d_rho, (unsigned long long *)nullptr, (const unsigned long long *)d_ncnt, out->nbr_idx.as<uint32_t>());
+               c->tab_a.as<uint32_t>(), d_rho, (unsigned long long *)nullptr, (const unsigned long long *)d_ncnt, out->nbr_idx.as<uint32_t>());
         out->has_neighbors = 1; out->n_neighbors = total;
     }
     } else {
@@ -721,21 +719,19 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
         c->gkey_a.ensure((size_t)n32 * 4); c->gkey_b.ensure((size_t)n32 * 4); c->gval_a.ensure((size_t)n32 * 4); c->gval_b.ensure((size_t)n32 * 4);
         LAUNCH(c, k_ns_keys_global, nblk(n32, 256), 256, D, d_xyz, n32, c->gkey_a.as<uint32_t>(), c->gval_a.as<uint32_t>(), c->err.as<int>());
         cub_sort(c, c->gkey_a.as<uint32_t>(), c->gkey_b.as<uint32_t>(), n32, bits_for(g_ns_cells), c->gval_a.as<uint32_t>(), c->gval_b.as<uint32_t>());
-        c->tab_a.ensure(g_ns_cells * 4); c->tab_b.ensure(g_ns_cells * 4);
-        CK(cudaMemsetAsync(c->tab_a.p, 0xff, g_ns_cells * 4, st));
-        LAUNCH(c, k_mark_starts, nblk(n32, 256), 256, c->gkey_b.as<uint32_t>(), n32, c->tab_a.as<uint32_t>(), (uint32_t)g_ns_cells);
-        LAUNCH(c, k_run_counts, nblk(n32, 256), 256, c->gkey_b.as<uint32_t>(), n32, c->tab_b.as<uint32_t>(), (uint32_t)g_ns_cells);
+        c->tab_a.ensure((g_ns_cells + 1) * 4);            // cell offsets
+        LAUNCH(c, k_cell_offsets, nblk((uint64_t)n32 + 1, 256), 256, c->gkey_b.as<uint32_t>(), n32, c->tab_a.as<uint32_t>(), (uint32_t)g_ns_cells);
         c->spos.ensure((size_t)n32 * 16);
         LAUNCH(c, k_gather_pos, nblk(n32, 256), 256, d_xyz, c->gval_b.as<uint32_t>(), n32, c->spos.as<float4>());
         unsigned long long *d_ncnt = nullptr;
         if (want_nbrs) { out->nbr_off.ensure((n + 1) * 8); d_ncnt = out->nbr_off.as<unsigned long long>(); CK(cudaMemsetAsync(d_ncnt, 0, (n + 1) * 8, st)); }
         LAUNCH(c, k_density_global<false>, nblk(n32, 128), 128, D, n32, c->gkey_b.as<uint32_t>(), c->spos.as<float4>(), c->tab_a.as<uint32_t>(),
-               c->tab_b.as<uint32_t>(), d_rho, d_ncnt, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
+               d_rho, d_ncnt, (const unsigned long long *)nullptr, (uint32_t *)nullptr);
         if (want_nbrs) {
             const uint64_t total = scan_neighbor_counts(c, d_ncnt, n);
             out->nbr_idx.ensure(std::max<uint64_t>(total, 1) * 4);
             LAUNCH(c, k_density_global<true>, nblk(n32, 128), 128, D, n32, c->gkey_b.as<uint32_t>(), c->spos.as<float4>(), c->tab_a.as<uint32_t>(),
-                   c->tab_b.as<uint32_t>(), d_rho, (unsigned long long *)nullptr, (const unsigned long long *)d_ncnt, out->nbr_idx.as<uint32_t>());
+                   d_rho, (unsigned long long *)nullptr, (const unsigned long long *)d_ncnt, out->nbr_idx.as<uint32_t>());
             out->has_neighbors = 1; out->n_neighbors = total;
         }
     }
@@ -1236,7 +1232,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         // x_bar, G, det G of every particle in its owning subdomain, over the density stage's list and cell tables
         CK(cudaEventRecord(c->ev_an[0], st));
         LAUNCH(c, k_aniso, nblk(n, 128), 128, D, M, c->dlist.as<uint32_t>(), c->doff.as<uint32_t>(), c->dflag.as<uint32_t>(),
-               c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(), c->tab_a.as<uint32_t>(), c->tab_b.as<uint32_t>(),
+               c->key_b.as<uint32_t>(), c->spos.as<float4>(), c->sub_flat.as<uint32_t>(), c->tab_a.as<uint32_t>(),
                out->an_xbar.as<float>(), out->an_g.as<float>(), c->an_det.as<float>());
         CK(cudaEventRecord(c->ev_an[1], st));
     }
