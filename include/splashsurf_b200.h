@@ -226,7 +226,8 @@ int ss_surface_timings(const ss_surface *s, ss_timings *out);
  * the stage received.  Writes min(n, SS_LSP_N) counters to out[SS_LSP_*] and returns SS_LSP_N (negative: NULL surface).
  * Host bookkeeping of values the stage reads back anyway (no device work, no synchronisation).
  * - fallback cascades, bricks each tier received (tier t + 1 receives what tier t could not take; the last tier takes all):
- *   exact pass, fix-up pass (variant 2), anisotropic level set and averaged-position surface (appended after BIN_CELLS);
+ *   exact pass, fix-up pass (variant 2), anisotropic level set and averaged-position surface (appended after BIN_CELLS; with or
+ *   without its Jacobian correction);
  * - certification: work bricks of k_certify_warp with the 384- or 576-candidate slice (variant 2), of k_certify (variant 1), or
  *   of the fused k_levelset (variant 0, exact everywhere, or more than 32 candidate bin runs per brick);
  * - the GLOBAL and COUNT template flags of the launches (0 / 1), R = ceil(h / cube_size) and the bin width in cells. */
@@ -324,6 +325,21 @@ typedef struct ss_averaged_surface_f32 {
     float radius_factor;                 /* R_s / particle_radius, finite and > 0; default 1 */
 } ss_averaged_surface_f32;
 int ss_context_set_averaged_surface_f32(ss_context *ctx, const ss_averaged_surface_f32 *avg /* NULL = off */);
+
+/* Jacobian correction of the averaged-position surface (B. Solenthaler, J. Schläfli and R. Pajarola, "A unified particle model for
+ * fluid-solid interactions", Computer Animation and Virtual Worlds 18(1), 2007; specification in DESIGN.md section 12.1).  Where
+ * particle groups come close or the fluid is concave, x_bar(g) is pulled between groups and the plain surface bulges or bridges.
+ * The correction shrinks the radius there: with EV the largest eigenvalue of the symmetric part of the Jacobian of x_bar(g),
+ *     gamma = clamp((t_high - EV) / (t_high - t_low), 0, 1),   f = gamma^3 - 3 gamma^2 + 3 gamma,
+ *     value(g) = (h - |g - x_bar(g)|) - R_s (1 - f)
+ * so a point is inside where |g - x_bar(g)| < f R_s; f = 1 (the plain surface) for EV <= t_low, f = 0 for EV >= t_high.  Opt-in per
+ * context (NULL = off, the default); the setter refuses non-finite values, t_low < 0 and t_low >= t_high.  A reconstruction with the
+ * correction on and the averaged-position surface off returns SS_ERR_INVALID_PARAMETER; otherwise the scope is that of
+ * ss_context_set_averaged_surface_f32. */
+typedef struct ss_averaged_correction_f32 {
+    float t_low, t_high;                 /* default 0.4, 3.5 */
+} ss_averaged_correction_f32;
+int ss_context_set_averaged_correction_f32(ss_context *ctx, const ss_averaged_correction_f32 *corr /* NULL = off */);
 
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.

@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -87,6 +87,11 @@ class _Anisotropy(C.Structure):
 class _AveragedSurface(C.Structure):
     """ss_averaged_surface_f32 (include/splashsurf_b200.h)."""
     _fields_ = [("radius_factor", C.c_float)]
+
+
+class _AveragedCorrection(C.Structure):
+    """ss_averaged_correction_f32 (include/splashsurf_b200.h)."""
+    _fields_ = [("t_low", C.c_float), ("t_high", C.c_float)]
 
 
 _LIB = None
@@ -197,6 +202,7 @@ def _bind(L):
     L.ss_context_set_anisotropy_f32.argtypes = [vp, C.POINTER(_Anisotropy)]
     L.ss_surface_copy_anisotropy.argtypes = [vp, vp, vp]
     L.ss_context_set_averaged_surface_f32.argtypes = [vp, C.POINTER(_AveragedSurface)]
+    L.ss_context_set_averaged_correction_f32.argtypes = [vp, C.POINTER(_AveragedCorrection)]
     L.ss_surface_anisotropy_ms.argtypes = [vp]
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
@@ -624,6 +630,23 @@ class Anisotropy:
 
 
 @dataclass(frozen=True)
+class JacobianCorrection:
+    """Jacobian correction of the averaged-position surface after Solenthaler, Schläfli & Pajarola (Computer Animation and Virtual
+    Worlds 18(1), 2007); DESIGN.md section 12.1.  Use it as ``AveragedSurface(correction=JacobianCorrection())``.
+
+    Where the fluid is concave or particle groups come close, the weighted average ``x_bar(g)`` is pulled between the groups and
+    the plain averaged surface bulges or bridges.  With ``EV`` the largest eigenvalue of the symmetric part of the Jacobian of
+    ``x_bar``, ``gamma = clamp((t_high - EV) / (t_high - t_low), 0, 1)`` and ``f = gamma^3 - 3 gamma^2 + 3 gamma``, a grid point is
+    inside where ``|g - x_bar(g)| < f * radius_factor * particle_radius``: the plain surface where ``EV <= t_low``, no surface
+    where ``EV >= t_high``.  The defaults are the paper's; ``0 <= t_low < t_high``, both finite."""
+    t_low: float = 0.4
+    t_high: float = 3.5
+
+    def _abi(self) -> _AveragedCorrection:
+        return _AveragedCorrection(float(np.float32(self.t_low)), float(np.float32(self.t_high)))
+
+
+@dataclass(frozen=True)
 class AveragedSurface:
     """Averaged-position surface after Zhu & Bridson (ACM TOG 24(3), 2005) for the level set; DESIGN.md section 12.
 
@@ -635,11 +658,17 @@ class AveragedSurface:
 
     Scope: grid, densities (bit for bit), marching cubes and stitching are unchanged; SPH normals and attribute interpolation keep
     the SPH kernel at the particle positions.  Requires ``subdomain_grid=True`` (always decomposed), one GPU, and cannot be combined
-    with ``anisotropy``."""
+    with ``anisotropy``.  ``correction=JacobianCorrection(...)`` shrinks the radius in concave regions and between particle groups
+    (Solenthaler et al. 2007; off by default)."""
     radius_factor: float = 1.0
+    correction: Optional[JacobianCorrection] = None
 
     def _abi(self) -> _AveragedSurface:
         return _AveragedSurface(float(np.float32(self.radius_factor)))
+
+    def _correction_abi(self):
+        """The argument of ss_context_set_averaged_correction_f32 (None: off)."""
+        return C.byref(self.correction._abi()) if self.correction is not None else None
 
 
 def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Optional[Anisotropy],
@@ -649,12 +678,14 @@ def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Op
     try:
         _check(L, L.ss_context_set_anisotropy_f32(ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
         _check(L, L.ss_context_set_averaged_surface_f32(ctx._h, C.byref(averaged_surface._abi()) if averaged_surface is not None else None))
+        _check(L, L.ss_context_set_averaged_correction_f32(ctx._h, averaged_surface._correction_abi() if averaged_surface is not None else None))
         return ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
     finally:
         if anisotropy is not None:
             L.ss_context_set_anisotropy_f32(ctx._h, None)
         if averaged_surface is not None:
             L.ss_context_set_averaged_surface_f32(ctx._h, None)
+            L.ss_context_set_averaged_correction_f32(ctx._h, None)
 
 
 def _collect_anisotropy(ctx: "Context", s, res: "SurfaceReconstruction"):

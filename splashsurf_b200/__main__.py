@@ -119,6 +119,10 @@ def main(argv=None):
     # averaged-position surface (Zhu & Bridson 2005; splashsurf_b200.AveragedSurface, DESIGN.md section 12) -- not part of the reference CLI
     r.add_argument("--averaged-surface", choices=["on", "off"], default="off")
     r.add_argument("--averaged-radius-factor", type=float, default=None)              # surface at radius_factor * particle radius from x_bar (default 1)
+    # its Jacobian correction (Solenthaler et al. 2007; splashsurf_b200.JacobianCorrection, DESIGN.md section 12.1)
+    r.add_argument("--averaged-correction", choices=["on", "off"], default="off")
+    r.add_argument("--averaged-correction-low", type=float, default=None)            # t_low: largest Jacobian eigenvalue still at full radius (default 0.4)
+    r.add_argument("--averaged-correction-high", type=float, default=None)           # t_high: from this eigenvalue on the radius is 0 (default 3.5)
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -261,11 +265,20 @@ def reconstruct(a) -> int:
         raise ValueError("--averaged-surface=on is not available with --partition=on: the averaged-position surface runs on one GPU per frame")
     if on(a.anisotropic) and on(a.averaged_surface):
         raise ValueError("--averaged-surface=on and --anisotropic=on are exclusive: choose one level set")
-    from . import Anisotropy, AveragedSurface
+    from . import Anisotropy, AveragedSurface, JacobianCorrection
     aniso = Anisotropy(a.aniso_smoothing, a.aniso_max_stretch, a.aniso_min_neighbors) if on(a.anisotropic) else None
     if a.averaged_radius_factor is not None and not on(a.averaged_surface):
         raise ValueError("--averaged-radius-factor applies to the averaged-position surface: add --averaged-surface=on")
-    avg = AveragedSurface(1.0 if a.averaged_radius_factor is None else a.averaged_radius_factor) if on(a.averaged_surface) else None
+    if on(a.averaged_correction) and not on(a.averaged_surface):
+        raise ValueError("--averaged-correction=on applies to the averaged-position surface: add --averaged-surface=on")
+    if (a.averaged_correction_low is not None or a.averaged_correction_high is not None) and not on(a.averaged_correction):
+        raise ValueError("--averaged-correction-low / --averaged-correction-high apply to the Jacobian correction: add --averaged-correction=on")
+    corr = None
+    if on(a.averaged_correction):
+        d = JacobianCorrection()
+        corr = JacobianCorrection(d.t_low if a.averaged_correction_low is None else a.averaged_correction_low,
+                                  d.t_high if a.averaged_correction_high is None else a.averaged_correction_high)
+    avg = AveragedSurface(1.0 if a.averaged_radius_factor is None else a.averaged_radius_factor, corr) if on(a.averaged_surface) else None
     paths = collect_paths(a)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)

@@ -10,7 +10,7 @@
 //                       particle index, per 4x4x4 sub-box the candidates within h of the sub-box, two grid points per lane;
 //                       bricks with more candidates than the slice go to a 4096-slot instantiation, beyond that to
 //                       k_fold_select (O(C^2) selection in index order).  Templated on the fold: SsAnisoFold here, SsAvgFold
-//                       (averaged-position surface, ss_averaged.cuh)
+//                       and SsAvgCorrFold (averaged-position surface, plain and Jacobian-corrected, ss_averaged.cuh)
 // Every value the level set writes is exact; there is no certification in this mode.
 #pragma once
 
@@ -196,6 +196,7 @@ __device__ __forceinline__ SsAnBrick ss_an_brick(const SsDev &P, const SsAnArgs 
 //   F::Acc   F::zero()                            the accumulators of one grid point
 //   void     F::add(P, cand, gx, gy, gz, acc)     one candidate at the grid point (gx, gy, gz); tests its own support
 //   float    F::value(P, acc)                     the tile value
+//   int      F::SELECT_BOXES                      sub-boxes whose accumulators k_fold_select holds per walk (1, 2, 4 or 8)
 // and the brick kernels below stage, order and cull the candidates once for every fold.  A fold's support must lie within the
 // isotropic ball of radius h around the record's position (the sub-box cull).
 
@@ -203,6 +204,7 @@ __device__ __forceinline__ SsAnBrick ss_an_brick(const SsDev &P, const SsAnArgs 
 struct SsAnisoFold {
     struct Cand { float4 r, g0, g1; };
     struct Acc { float phi; };
+    static constexpr int SELECT_BOXES = 8;
     static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) {
         return Cand{ A.bins.rec[src], A.grec[2 * (size_t)src], A.grec[2 * (size_t)src + 1] };
     }
@@ -290,45 +292,52 @@ k_fold_levelset(SsDev P, SsAnArgs A) {
 }
 
 // Bricks with more candidates than the largest slice (extreme clustering): one warp per brick walks the candidates in
-// ascending particle index by repeated selection of the next key, O(C^2 / 32), and folds each into its 16 grid points.
+// ascending particle index by repeated selection of the next key, O(C^2 / 32), and folds each into its grid points.  A lane holds
+// the accumulators of two points per sub-box for F::SELECT_BOXES sub-boxes at a time; with fewer than 8 the walk is repeated per
+// group of sub-boxes.
 template <class F>
 __global__ void __launch_bounds__(32)
 k_fold_select(SsDev P, SsAnArgs A) {
+    constexpr int NB = F::SELECT_BOXES;
+    static_assert(8 % NB == 0, "the sub-boxes of a brick split into equal groups");
     if (blockIdx.x >= A.n_bricks) return;
     const int lane = threadIdx.x & 31;
     const SsAnBrick N = ss_an_brick(P, A, A.bricks[blockIdx.x]);
     const SsSubLane L = ss_sub_lane(P, lane);
-    typename F::Acc acc[16];
+#pragma unroll 1
+    for (int b0 = 0; b0 < 8; b0 += NB) {
+        typename F::Acc acc[2 * NB];
 #pragma unroll
-    for (int q = 0; q < 16; ++q) acc[q] = F::zero();
-    unsigned long long last = 0;
-    bool first = true;
-    for (;;) {
-        unsigned long long best = ~0ull;
-        for (int r = 0; r < N.K.nruns; ++r) {
-            uint32_t a;
-            const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r, a);
-            for (uint32_t t = a + lane; t < a + len; t += 32) {
-                const unsigned long long kk = ((unsigned long long)A.bins.pidx[t] << 32) | (unsigned long long)t;
-                if ((first || kk > last) && kk < best) best = kk;
+        for (int q = 0; q < 2 * NB; ++q) acc[q] = F::zero();
+        unsigned long long last = 0;
+        bool first = true;
+        for (;;) {
+            unsigned long long best = ~0ull;
+            for (int r = 0; r < N.K.nruns; ++r) {
+                uint32_t a;
+                const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r, a);
+                for (uint32_t t = a + lane; t < a + len; t += 32) {
+                    const unsigned long long kk = ((unsigned long long)A.bins.pidx[t] << 32) | (unsigned long long)t;
+                    if ((first || kk > last) && kk < best) best = kk;
+                }
+            }
+            for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
+            if (best == ~0ull) break;
+            last = best; first = false;
+            const typename F::Cand cd = F::load(A, (uint32_t)best);
+#pragma unroll
+            for (int b = 0; b < NB; ++b) {
+                const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b0 + b, L, true);
+                F::add(P, cd, X.gx, X.gy, X.gzA, acc[2 * b]);
+                F::add(P, cd, X.gx, X.gy, X.gzB, acc[2 * b + 1]);
             }
         }
-        for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
-        if (best == ~0ull) break;
-        last = best; first = false;
-        const typename F::Cand cd = F::load(A, (uint32_t)best);
+        float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
 #pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
-            F::add(P, cd, X.gx, X.gy, X.gzA, acc[2 * b]);
-            F::add(P, cd, X.gx, X.gy, X.gzB, acc[2 * b + 1]);
+        for (int b = 0; b < NB; ++b) {
+            const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b0 + b, L, true);
+            if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = F::value(P, acc[2 * b]);
+            if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = F::value(P, acc[2 * b + 1]);
         }
-    }
-    float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
-#pragma unroll
-    for (int b = 0; b < 8; ++b) {
-        const SsSubBox X = ss_sub_box(P, N.T, N.B.bx, N.B.by, N.B.bz, b, L, true);
-        if (X.vA) tile[((size_t)X.i * P.np + X.j) * P.np + X.k] = F::value(P, acc[2 * b]);
-        if (X.vB) tile[((size_t)X.i * P.np + X.j) * P.np + X.k + 1] = F::value(P, acc[2 * b + 1]);
     }
 }

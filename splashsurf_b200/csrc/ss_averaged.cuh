@@ -12,6 +12,7 @@
 #pragma once
 
 struct SsAvgFold {
+    static constexpr int SELECT_BOXES = 8;
     struct Cand { float4 r; };
     struct Acc { float s, x, y, z; };
     static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return Cand{ A.bins.rec[src] }; }
@@ -30,5 +31,69 @@ struct SsAvgFold {
         const float mx = __fdiv_rn(a.x, a.s), my = __fdiv_rn(a.y, a.s), mz = __fdiv_rn(a.z, a.s);
         const float m2 = __fadd_rn(__fadd_rn(__fmul_rn(mx, mx), __fmul_rn(my, my)), __fmul_rn(mz, mz));
         return __fsub_rn(P.h, __fsqrt_rn(m2));
+    }
+};
+
+// Jacobian correction of the averaged-position surface (B. Solenthaler, J. Schläfli and R. Pajarola, "A unified particle model for
+// fluid-solid interactions", Computer Animation and Virtual Worlds 18(1), 2007), the opt-in of ss_context_set_averaged_correction_f32;
+// DESIGN.md §12.1.  With u_j = 1 - d2_j / h2, besides SsAvgFold's sums S, X, Y, Z (same order, so x_bar is bit-identical):
+//     T_b = sum_j u_j^2 d_jb,   M_ab = sum_j u_j^2 d_ja d_jb   (a <= b)
+// J = grad_g x_bar = (6 / h^2) (M / S - m (T / S)^T) with m = (X, Y, Z) / S.  EV, the largest eigenvalue of the symmetric part of J
+// (cyclic Jacobi, add / sub / mul / div / sqrt only), sets f in [0, 1] (1 for EV <= t_low, 0 for EV >= t_high), and the tile value
+//     v = (h - |m|) - R_s (1 - f)
+// puts the surface (v = h - R_s) where |m| = f R_s: the radius shrinks where the average is pulled between particle groups.
+struct SsAvgCorrFold {
+    static constexpr int SELECT_BOXES = 2;          // 13 accumulators per point: k_fold_select holds 4 points per lane, not 16
+    using Cand = SsAvgFold::Cand;
+    struct Acc { SsAvgFold::Acc a; float tx, ty, tz, mxx, mxy, mxz, myy, myz, mzz; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgFold::zero(), 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        const float dx = __fsub_rn(c.r.x, gx), dy = __fsub_rn(c.r.y, gy), dz = __fsub_rn(c.r.z, gz);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+        if (!(d2 < P.h2)) return;
+        SsAvgFold::add(P, c, gx, gy, gz, a.a);
+        const float u = __fsub_rn(1.0f, __fdiv_rn(d2, P.h2));
+        const float uu = __fmul_rn(u, u);
+        const float ex = __fmul_rn(uu, dx), ey = __fmul_rn(uu, dy), ez = __fmul_rn(uu, dz);
+        a.tx = __fadd_rn(a.tx, ex); a.ty = __fadd_rn(a.ty, ey); a.tz = __fadd_rn(a.tz, ez);
+        a.mxx = __fadd_rn(a.mxx, __fmul_rn(ex, dx)); a.mxy = __fadd_rn(a.mxy, __fmul_rn(ex, dy)); a.mxz = __fadd_rn(a.mxz, __fmul_rn(ex, dz));
+        a.myy = __fadd_rn(a.myy, __fmul_rn(ey, dy)); a.myz = __fadd_rn(a.myz, __fmul_rn(ey, dz)); a.mzz = __fadd_rn(a.mzz, __fmul_rn(ez, dz));
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) {
+        const float s = a.a.s;
+        if (!(s > 0.0f)) return 0.0f;
+        const float m[3] = { __fdiv_rn(a.a.x, s), __fdiv_rn(a.a.y, s), __fdiv_rn(a.a.z, s) };
+        const float m2 = __fadd_rn(__fadd_rn(__fmul_rn(m[0], m[0]), __fmul_rn(m[1], m[1])), __fmul_rn(m[2], m[2]));
+        const float plain = __fsub_rn(P.h, __fsqrt_rn(m2));           // SsAvgFold::value
+        const float t[3] = { __fdiv_rn(a.tx, s), __fdiv_rn(a.ty, s), __fdiv_rn(a.tz, s) };
+        const float q[3][3] = { { __fdiv_rn(a.mxx, s), __fdiv_rn(a.mxy, s), __fdiv_rn(a.mxz, s) },
+                                { 0.0f, __fdiv_rn(a.myy, s), __fdiv_rn(a.myz, s) },
+                                { 0.0f, 0.0f, __fdiv_rn(a.mzz, s) } };
+        // symmetric part of J' = M / S - m t^T (J = (6 / h^2) J'): A_ab = 0.5 ((q_ab - m_a t_b) + (q_ab - m_b t_a))
+        float A[3][3], v[3][3] = {};
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+#pragma unroll
+            for (int j = i; j < 3; ++j) {
+                A[i][j] = __fmul_rn(0.5f, __fadd_rn(__fsub_rn(q[i][j], __fmul_rn(m[i], t[j])), __fsub_rn(q[i][j], __fmul_rn(m[j], t[i]))));
+                A[j][i] = A[i][j];
+            }
+        }
+#pragma unroll
+        for (int sweep = 0; sweep < SS_AN_SWEEPS; ++sweep) {           // eigenvalues only: v is never read
+            ss_jacobi_rot<0, 1>(A, v);
+            ss_jacobi_rot<0, 2>(A, v);
+            ss_jacobi_rot<1, 2>(A, v);
+        }
+        float e = A[0][0];
+        if (A[1][1] > e) e = A[1][1];
+        if (A[2][2] > e) e = A[2][2];
+        const float ev = __fmul_rn(__fdiv_rn(6.0f, P.h2), e);
+        float g = __fdiv_rn(__fsub_rn(P.av_high, ev), __fsub_rn(P.av_high, P.av_low));
+        g = g > 0.0f ? (g < 1.0f ? g : 1.0f) : 0.0f;                  // a NaN EV gives f = 0
+        float f = __fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(g, 3.0f), g), 3.0f), g);
+        f = f < 1.0f ? f : 1.0f;                                       // rounding gives 1 + 2^-23 for some gamma < 1
+        return __fsub_rn(plain, __fmul_rn(P.av_rs, __fsub_rn(1.0f, f)));
     }
 };

@@ -54,6 +54,8 @@ struct SsDev {
     int aniso;                                 // 1: memberships outside the neighbourhood-search grid are dropped, not an error
     float an_lambda, an_kr;                    // smoothing of the kernel centres, maximum stretch k_r
     uint32_t an_min_nb;                        // fewer neighbours than this: isotropic kernel
+    // Jacobian correction of the averaged-position surface (ss_averaged.cuh, SsAvgCorrFold)
+    float av_rs, av_low, av_high;              // R_s, t_low, t_high
 };
 
 // ------------------------------------------------------------------ exact helpers ----

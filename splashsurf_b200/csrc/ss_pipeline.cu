@@ -135,6 +135,8 @@ struct ss_context {
     ss_anisotropy_f32 an{};
     int avg_on = 0;                  // 1: averaged-position surface (ss_averaged.cuh) with the parameters `avg`
     ss_averaged_surface_f32 avg{};
+    int ac_on = 0;                   // 1: Jacobian correction of the averaged-position surface (SsAvgCorrFold) with `ac`
+    ss_averaged_correction_f32 ac{};
     cudaEvent_t ev_an[2] = { nullptr, nullptr };
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
@@ -375,6 +377,14 @@ extern "C" int ss_context_set_averaged_surface_f32(ss_context *c, const ss_avera
     if (!a) { c->avg_on = 0; return SS_OK; }
     if (!(a->radius_factor > 0.0f) || !std::isfinite(a->radius_factor)) return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface radius_factor must be finite and > 0");
     c->avg = *a; c->avg_on = 1;
+    return SS_OK;
+}
+extern "C" int ss_context_set_averaged_correction_f32(ss_context *c, const ss_averaged_correction_f32 *a) {
+    if (!c) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL context");
+    if (!a) { c->ac_on = 0; return SS_OK; }
+    if (!std::isfinite(a->t_low) || !std::isfinite(a->t_high) || !(a->t_low >= 0.0f) || !(a->t_low < a->t_high))
+        return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface correction: t_low and t_high must be finite with 0 <= t_low < t_high");
+    c->ac = *a; c->ac_on = 1;
     return SS_OK;
 }
 
@@ -810,9 +820,9 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
     }, ls_launches, received);
 }
 
-// Warp-per-brick level set of one batch for the fold F (anisotropic kernels, ss_aniso.cuh, or the averaged-position surface,
-// ss_averaged.cuh): work list of non-empty bricks without extension tasks (the single-point planes of the last brick are bricks of
-// their own), the 512-slot slice, then the 4096-slot slice, then selection.  Every listed brick gets state 2 (exact values).
+// Warp-per-brick level set of one batch for the fold F (anisotropic kernels, ss_aniso.cuh, or the averaged-position surface with
+// or without its Jacobian correction, ss_averaged.cuh): work list of non-empty bricks without extension tasks (the single-point
+// planes of the last brick are bricks of their own), the 512-slot slice, then the 4096-slot slice, then selection.  Every listed brick gets state 2 (exact values).
 // Returns the length of the work list.
 template <class F>
 static uint32_t launch_fold_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, const float4 *grec, uint64_t &ls_launches, uint64_t *received) {
@@ -849,6 +859,7 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     uint64_t *const paths = out->ls_paths;
     const bool folded = D.aniso || averaged;            // warp-per-brick fold cascade, exact values only
     const uint32_t n_work = D.aniso ? launch_fold_levelset<SsAnisoFold>(c, D, nbatch, c->an_grec.as<float4>(), ls_launches, paths + SS_LSP_ANISO_512)
+                          : averaged && c->ac_on ? launch_fold_levelset<SsAvgCorrFold>(c, D, nbatch, nullptr, ls_launches, paths + SS_LSP_AVG_512)
                           : averaged ? launch_fold_levelset<SsAvgFold>(c, D, nbatch, nullptr, ls_launches, paths + SS_LSP_AVG_512)
                           : build_worklist(c, D, nbatch);
     A.work_list = c->list_ls.as<uint32_t>();
@@ -1097,6 +1108,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         if (!(rs > 0.0f && rs < h) || !std::isfinite(rs))
             return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface: radius_factor * particle_radius must lie in (0, compact support radius)");
         D.thr = fsubr(h, rs);
+        D.av_rs = rs; D.av_low = c->ac.t_low; D.av_high = c->ac.t_high;     // read by SsAvgCorrFold only (DESIGN.md §12.1)
     }
     D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)ns_margin) / (double)h) + 3;
     D.ns_stride = D.nsD * D.nsD * D.nsD;
@@ -1664,6 +1676,7 @@ static int reconstruct_partition_impl(ss_context *c, const float *xyz, uint64_t 
     if (p->has_particle_aabb) return ss_fail(SS_ERR_UNSUPPORTED, "filter particles before partitioning (particle_aabb is applied by the caller)");
     if (c->an_on) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels are not available on partitioned (multi-GPU) reconstructions");
     if (c->avg_on) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface is not available on partitioned (multi-GPU) reconstructions");
+    if (c->ac_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "the Jacobian correction applies to the averaged-position surface, which is off");
     if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "partitioned reconstruction requires the subdomain grid");
     if (axis < 0 || axis > 2 || own_lo < 0 || own_hi < own_lo || halo < 0) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad partition");
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
@@ -1734,6 +1747,7 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
         // decomposition decision, lib.rs:421-464
         int use_dec = 0;
         if (c->an_on && c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropic kernels and the averaged-position surface are exclusive");
+        if (c->ac_on && !c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "the Jacobian correction applies to the averaged-position surface, which is off");
         if (c->avg_on) {
             // averaged-position surface: subdomain path only, always decomposed (no auto-disable)
             if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface requires the subdomain grid (spatial_decomposition = UniformGrid)");

@@ -288,12 +288,14 @@ class Runner:
                 _check(L, L.ss_context_set_anisotropy_f32(self.ctx._h, C.byref(self.anisotropy._abi())))
             if self.averaged_surface is not None:
                 _check(L, L.ss_context_set_averaged_surface_f32(self.ctx._h, C.byref(self.averaged_surface._abi())))
+                _check(L, L.ss_context_set_averaged_correction_f32(self.ctx._h, self.averaged_surface._correction_abi()))
             s = self.ctx.reconstruct_raw(xyz_ptr, n, self.params if params is None else params)
         finally:
             if self.anisotropy is not None:
                 L.ss_context_set_anisotropy_f32(self.ctx._h, None)
             if self.averaged_surface is not None:
                 L.ss_context_set_averaged_surface_f32(self.ctx._h, None)
+                L.ss_context_set_averaged_correction_f32(self.ctx._h, None)
         keep = self.keep_surface and self.world == 1
         try:
             out = self._collect(s, copy_out, n_local=n, force_copy=force_copy)

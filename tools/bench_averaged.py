@@ -1,6 +1,7 @@
 #!/usr/bin/env python3
-"""Times the averaged-position surface (DESIGN.md §12) beside the plain reconstruction on the same cloud and the same context, one GPU:
-device-resident steps through splashsurf_b200.distributed.Runner (what bench.py times), the two modes alternated `--rounds` times.
+"""Times the averaged-position surface (DESIGN.md §12), plain and with the Jacobian correction (§12.1), beside the standard
+reconstruction on the same cloud and the same context, one GPU: device-resident steps through splashsurf_b200.distributed.Runner (what
+bench.py times), the three modes alternated `--rounds` times.
 Per mode and round: mean device ms per step over `--steps` timed steps after `--warmup` untimed ones, the stage times of the last step
 (CUDA events) and the mesh size.  The card name and its power limit are read at the start and at the end.  Prints one JSON line;
 writes nothing.
@@ -41,7 +42,9 @@ def main():
     x = syn.dam_break_50m() if a.particles == 50_000_400 else syn.dam_break_scaled(a.particles, 0.01, 3)
     ctx = ss.Context(0)
     params = ss.make_params(particle_radius=0.01, smoothing_length=2.0, cube_size=0.5)
-    runners = {"plain": ssd.Runner(ctx, params, 1, 0, 0), "averaged": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=ss.AveragedSurface())}
+    runners = {"plain": ssd.Runner(ctx, params, 1, 0, 0), "averaged": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=ss.AveragedSurface()),
+               "averaged_corrected": ssd.Runner(ctx, params, 1, 0, 0,
+                                                averaged_surface=ss.AveragedSurface(correction=ss.JacobianCorrection()))}
     dev = torch.from_numpy(x).cuda()
     torch.cuda.synchronize()
     out = {"tool": "bench_averaged", "particles": len(x), "workload": "dam break, r = 0.01, -l 2, -c 0.5", "card_before": card_before,
