@@ -341,6 +341,20 @@ typedef struct ss_averaged_correction_f32 {
 } ss_averaged_correction_f32;
 int ss_context_set_averaged_correction_f32(ss_context *ctx, const ss_averaged_correction_f32 *corr /* NULL = off */);
 
+/* Per-particle radii of the averaged-position surface (Zhu & Bridson's r_bar; specification in DESIGN.md section 12.2), for
+ * polydisperse clouds (adaptive-resolution SPH, grain-size distributions, a per-particle `pscale`).  With R_j = radius_factor * r_j,
+ * delta_j = R_j - R_s and b(g) = sum_j w_j delta_j / sum_j w_j (the weights of x_bar(g)), the radius becomes r_bar(g) = R_s + b(g):
+ *     value(g) = (h - |g - x_bar(g)|) + b(g)                                  (plain),
+ *     value(g) = ((h - |g - x_bar(g)|) + b(g)) - (R_s + b(g)) (1 - f)        (with the Jacobian correction),
+ * against the unchanged threshold h - R_s.  Radii all equal to particle_radius give the results of the single radius bit for bit.
+ * `radii` holds n floats in host or device memory (detected like xyz); they are copied, so the caller may free its array when the
+ * setter returns, and they stay set until the next call (NULL = off, the default).  A reconstruction returns SS_ERR_INVALID_PARAMETER
+ * when the averaged-position surface is off, when n differs from its particle count, or when a radius (of all n, before the
+ * particle-AABB filter) does not give a finite R_j in (0, compact support radius); the message names the first such index.
+ * Otherwise the scope is that of ss_context_set_averaged_surface_f32 (partitioned entries: SS_ERR_UNSUPPORTED with the averaged
+ * surface on, SS_ERR_INVALID_PARAMETER with it off).  Cost: 4 bytes per subdomain membership and 8 bytes per particle. */
+int ss_context_set_averaged_radii_f32(ss_context *ctx, const float *radii /* NULL = off */, uint64_t n);
+
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.
  * The entries marked [bins] query the particles through the splat bins of the reconstruction that produced the surface and

@@ -203,6 +203,7 @@ def _bind(L):
     L.ss_surface_copy_anisotropy.argtypes = [vp, vp, vp]
     L.ss_context_set_averaged_surface_f32.argtypes = [vp, C.POINTER(_AveragedSurface)]
     L.ss_context_set_averaged_correction_f32.argtypes = [vp, C.POINTER(_AveragedCorrection)]
+    L.ss_context_set_averaged_radii_f32.argtypes = [vp, vp, C.c_uint64]
     L.ss_surface_anisotropy_ms.argtypes = [vp]
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
@@ -659,7 +660,11 @@ class AveragedSurface:
     Scope: grid, densities (bit for bit), marching cubes and stitching are unchanged; SPH normals and attribute interpolation keep
     the SPH kernel at the particle positions.  Requires ``subdomain_grid=True`` (always decomposed), one GPU, and cannot be combined
     with ``anisotropy``.  ``correction=JacobianCorrection(...)`` shrinks the radius in concave regions and between particle groups
-    (Solenthaler et al. 2007; off by default)."""
+    (Solenthaler et al. 2007; off by default).
+
+    Per-particle radii (``particle_radii=`` of ``reconstruct_surface``; DESIGN.md section 12.2): ``radius_factor`` scales every
+    particle's radius, ``R_j = radius_factor * r_j``, and the surface radius at g becomes the average of the ``R_j`` with the
+    weights of ``x_bar(g)``.  Every ``R_j`` must lie between 0 and h."""
     radius_factor: float = 1.0
     correction: Optional[JacobianCorrection] = None
 
@@ -671,14 +676,31 @@ class AveragedSurface:
         return C.byref(self.correction._abi()) if self.correction is not None else None
 
 
+def _particle_radii(particle_radii, n: int, averaged_surface: Optional[AveragedSurface]) -> Optional[np.ndarray]:
+    """The per-particle radii of the averaged surface as a contiguous float32 array of n entries (None: not given)."""
+    if particle_radii is None:
+        return None
+    if averaged_surface is None:
+        raise ValueError("particle_radii apply to the averaged-position surface: pass averaged_surface=AveragedSurface(...)")
+    r = np.asarray(particle_radii)
+    if not np.issubdtype(r.dtype, np.floating):
+        raise TypeError(f"particle_radii must be a float array, not {r.dtype}")
+    if r.shape != (n,):
+        raise ValueError(f"particle_radii must have shape ({n},), one radius per particle, not {r.shape}")
+    return np.ascontiguousarray(r, dtype=np.float32)
+
+
 def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Optional[Anisotropy],
-                     averaged_surface: Optional[AveragedSurface] = None):
-    """ctx.reconstruct_raw with the context's anisotropy and averaged surface set for this one call (and reset whatever happens)."""
+                     averaged_surface: Optional[AveragedSurface] = None, radii: Optional[np.ndarray] = None):
+    """ctx.reconstruct_raw with the context's anisotropy, averaged surface and per-particle radii set for this one call (and reset
+    whatever happens)."""
     L = ctx._L
     try:
         _check(L, L.ss_context_set_anisotropy_f32(ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
         _check(L, L.ss_context_set_averaged_surface_f32(ctx._h, C.byref(averaged_surface._abi()) if averaged_surface is not None else None))
         _check(L, L.ss_context_set_averaged_correction_f32(ctx._h, averaged_surface._correction_abi() if averaged_surface is not None else None))
+        if radii is not None:
+            _check(L, L.ss_context_set_averaged_radii_f32(ctx._h, radii.ctypes.data, len(radii)))
         return ctx.reconstruct_raw(arr.ctypes.data, len(arr), p)
     finally:
         if anisotropy is not None:
@@ -686,6 +708,8 @@ def _reconstruct_raw(ctx: "Context", arr: np.ndarray, p: _Params, anisotropy: Op
         if averaged_surface is not None:
             L.ss_context_set_averaged_surface_f32(ctx._h, None)
             L.ss_context_set_averaged_correction_f32(ctx._h, None)
+        if radii is not None:
+            L.ss_context_set_averaged_radii_f32(ctx._h, None, 0)
 
 
 def _collect_anisotropy(ctx: "Context", s, res: "SurfaceReconstruction"):
@@ -1068,14 +1092,16 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                         subdomain_grid: bool = True, subdomain_grid_auto_disable: bool = True,
                         subdomain_num_cubes_per_dim: int = 64, context: Optional[Context] = None,
                         keep_levelset_tile_of: Optional[int] = None, with_debug: bool = False, sph_normals: bool = False,
-                        anisotropy: Optional[Anisotropy] = None, averaged_surface: Optional[AveragedSurface] = None) -> SurfaceReconstruction:
+                        anisotropy: Optional[Anisotropy] = None, averaged_surface: Optional[AveragedSurface] = None,
+                        particle_radii=None) -> SurfaceReconstruction:
     """Performs a surface reconstruction from the given particles (no post-processing) on the GPU.
 
     Same signature and semantics as ``pysplashsurf.reconstruct_surface``; ``particles`` is an (N, 3) float32
     array (float64 input is not provided by the device path and raises, like an unsupported dtype does in the
     reference, pysplashsurf/src/reconstruction.rs:204-206).  ``anisotropy=Anisotropy(...)`` switches the level set to anisotropic
     kernels, ``averaged_surface=AveragedSurface(...)`` to the averaged-position surface (neither is part of the reference; see
-    ``Anisotropy`` and ``AveragedSurface``).
+    ``Anisotropy`` and ``AveragedSurface``).  ``particle_radii``, a float array of one radius per particle (converted to float32),
+    gives the averaged-position surface a radius per particle (DESIGN.md section 12.2); it requires ``averaged_surface``.
     """
     arr = np.asarray(particles)
     if arr.dtype != np.float32:
@@ -1083,6 +1109,7 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
     if arr.ndim != 2 or arr.shape[1] != 3:
         raise ValueError("particles must have shape (N, 3)")
     arr = np.ascontiguousarray(arr)
+    radii = _particle_radii(particle_radii, len(arr), averaged_surface)
     ctx = context or default_context()
     L = ctx._L
     p = make_params(particle_radius=particle_radius, rest_density=rest_density, smoothing_length=smoothing_length,
@@ -1092,7 +1119,7 @@ def reconstruct_surface(particles, *, particle_radius: float, rest_density: floa
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1 if keep_levelset_tile_of is None else int(keep_levelset_tile_of)))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, int(bool(sph_normals))))
-    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface, radii)
     try:
         res = _collect(ctx, s, len(arr), p, with_debug or keep_levelset_tile_of is not None, keep_levelset_tile_of is not None)
         if anisotropy is not None:
@@ -1315,7 +1342,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                             mesh_smoothing_weights_normalization: float = 13.0, output_mesh_smoothing_weights: bool = False,
                             output_raw_normals: bool = False, output_raw_mesh: bool = False, context: Optional[Context] = None,
                             with_debug: bool = False, anisotropy: Optional[Anisotropy] = None,
-                            averaged_surface: Optional[AveragedSurface] = None, **post):
+                            averaged_surface: Optional[AveragedSurface] = None, particle_radii=None, **post):
     """``pysplashsurf.reconstruction_pipeline`` (pysplashsurf/src/pipeline.rs:109-200) on the GPU: surface reconstruction plus
     the post-processing steps of splashsurf/src/reconstruct.rs:1094-1391 that run on the device -- smoothing weights, weighted
     Laplacian smoothing, SPH or area-weighted normals (at the smoothed vertices), normal smoothing and SPH interpolation of
@@ -1327,8 +1354,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     ``quad_max_edge_diag_ratio`` / ``quad_max_normal_angle`` / ``quad_max_interior_angle``) runs last (reconstruct.rs:1410-1441, host):
     the returned mesh is then a MixedTriQuadMesh3d.  ``mesh_aabb_min`` / ``mesh_aabb_max`` (+ ``mesh_aabb_clamp_vertices``) clamp the
     finished mesh (reconstruct.rs:1394-1408) and ``check_mesh_closed`` / ``check_mesh_manifold`` raise SplashsurfError with the
-    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy`` and
-    ``averaged_surface`` as in ``reconstruct_surface``."""
+    reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy``,
+    ``averaged_surface`` and ``particle_radii`` as in ``reconstruct_surface``."""
     passive = ("mesh_cleanup", "decimate_barnacles", "mesh_cleanup_snap_dist", "keep_vertices", "generate_quads", "quad_max_edge_diag_ratio",
                "quad_max_normal_angle", "quad_max_interior_angle", "mesh_aabb_min", "mesh_aabb_max", "mesh_aabb_clamp_vertices",
                "check_mesh_closed", "check_mesh_manifold", "check_mesh_orientation", "check_mesh_debug")
@@ -1349,6 +1376,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
         if a.dtype != np.float32 or not (a.ndim == 1 or (a.ndim == 2 and a.shape[1] == 3)) or len(a) != len(arr):
             raise NotImplementedError(f"attribute {name!r}: only float32 arrays of shape (N,) or (N, 3) are interpolated")
         attributes[name] = np.ascontiguousarray(a)
+    radii = _particle_radii(particle_radii, len(arr), averaged_surface)
     ctx = context or default_context()
     L = ctx._L
     p = make_params(particle_radius=particle_radius, rest_density=rest_density, smoothing_length=smoothing_length, cube_size=cube_size,
@@ -1357,7 +1385,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                     subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
     _check(L, L.ss_context_keep_levelset_tile(ctx._h, -1))
     _check(L, L.ss_context_set_compute_sph_normals(ctx._h, 0))
-    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface)
+    s = _reconstruct_raw(ctx, arr, p, anisotropy, averaged_surface, radii)
     try:
         rec = _collect(ctx, s, len(arr), p, with_debug, False)                  # raw mesh, densities, grids
         if anisotropy is not None:

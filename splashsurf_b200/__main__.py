@@ -123,6 +123,8 @@ def main(argv=None):
     r.add_argument("--averaged-correction", choices=["on", "off"], default="off")
     r.add_argument("--averaged-correction-low", type=float, default=None)            # t_low: largest Jacobian eigenvalue still at full radius (default 0.4)
     r.add_argument("--averaged-correction-high", type=float, default=None)           # t_high: from this eigenvalue on the radius is 0 (default 3.5)
+    # per-particle radii of the averaged-position surface (DESIGN.md section 12.2): the scalar point attribute NAME of each input frame
+    r.add_argument("--averaged-radius-attribute", default=None, metavar="NAME")
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -279,6 +281,8 @@ def reconstruct(a) -> int:
         corr = JacobianCorrection(d.t_low if a.averaged_correction_low is None else a.averaged_correction_low,
                                   d.t_high if a.averaged_correction_high is None else a.averaged_correction_high)
     avg = AveragedSurface(1.0 if a.averaged_radius_factor is None else a.averaged_radius_factor, corr) if on(a.averaged_surface) else None
+    if a.averaged_radius_attribute is not None and not on(a.averaged_surface):
+        raise ValueError("--averaged-radius-attribute applies to the averaged-position surface: add --averaged-surface=on")
     paths = collect_paths(a)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)
@@ -312,6 +316,12 @@ def reconstruct(a) -> int:
             for name, arr in attrs.items():
                 if arr.dtype.kind != "f":              # BGEO Int attributes load as u64; the reference cannot interpolate them either (reconstruct.rs:1387)
                     raise ValueError(f'Interpolation of this attribute type not implemented (attribute "{name}")')
+            radii = None
+            if a.averaged_radius_attribute is not None:
+                name = a.averaged_radius_attribute
+                radii = io.read_particle_attributes(src, [name])[name]     # a file without it: ValueError 'Missing attribute(s) ...'
+                if radii.dtype.kind != "f" or radii.shape != (len(p),):
+                    raise ValueError(f'--averaged-radius-attribute: attribute "{name}" of {src} is not a float scalar per particle')
             t = time.perf_counter()
             if post:
                 # --sph-normals only selects how --normals are computed (reconstruct.rs:1094-1149)
@@ -325,10 +335,10 @@ def reconstruct(a) -> int:
                     quad_max_normal_angle=a.quad_max_normal_angle, quad_max_interior_angle=a.quad_max_interior_angle, mesh_aabb_min=mmin,
                     mesh_aabb_max=mmax, mesh_aabb_clamp_vertices=on(a.mesh_aabb_clamp_verts), check_mesh_closed=closed, check_mesh_manifold=manifold,
                     check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso,
-                    averaged_surface=avg, **base)
+                    averaged_surface=avg, particle_radii=radii, **base)
                 raw = rec.mesh
             else:
-                raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, averaged_surface=avg, **base).mesh
+                raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, averaged_surface=avg, particle_radii=radii, **base).mesh
                 out = MeshWithData(raw, {}, {})
             dt = time.perf_counter() - t
             quads = out.mesh.get_quads() if on(a.generate_quads) else None

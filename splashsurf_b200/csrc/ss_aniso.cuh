@@ -10,7 +10,8 @@
 //                       particle index, per 4x4x4 sub-box the candidates within h of the sub-box, two grid points per lane;
 //                       bricks with more candidates than the slice go to a 4096-slot instantiation, beyond that to
 //                       k_fold_select (O(C^2) selection in index order).  Templated on the fold: SsAnisoFold here, SsAvgFold
-//                       and SsAvgCorrFold (averaged-position surface, plain and Jacobian-corrected, ss_averaged.cuh)
+//                       and SsAvgCorrFold (averaged-position surface, plain and Jacobian-corrected, ss_averaged.cuh), and
+//                       SsAvgRadFold / SsAvgCorrRadFold (the same with per-particle radii)
 // Every value the level set writes is exact; there is no certification in this mode.
 #pragma once
 
@@ -163,6 +164,7 @@ __global__ void k_records_aniso(uint32_t m, const uint32_t *__restrict__ key, co
 struct SsAnArgs {
     SsBins bins;                       // records: (x_bar, V det G), bin-sorted
     const float4 *grec;                // two per record: (g00, g01, g02, g11), (g12, g22, -, -)
+    const float *rrec;                 // one per record: delta_j of the averaged surface's per-particle radii (ss_averaged.cuh)
     const uint32_t *bricks;            // listed bricks (linear index)
     uint32_t n_bricks;
     float *tiles;

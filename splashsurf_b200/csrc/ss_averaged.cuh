@@ -66,6 +66,11 @@ struct SsAvgCorrFold {
         const float m[3] = { __fdiv_rn(a.a.x, s), __fdiv_rn(a.a.y, s), __fdiv_rn(a.a.z, s) };
         const float m2 = __fadd_rn(__fadd_rn(__fmul_rn(m[0], m[0]), __fmul_rn(m[1], m[1])), __fmul_rn(m[2], m[2]));
         const float plain = __fsub_rn(P.h, __fsqrt_rn(m2));           // SsAvgFold::value
+        return __fsub_rn(plain, __fmul_rn(P.av_rs, __fsub_rn(1.0f, factor(P, a, m))));
+    }
+    // f of a point with S > 0 and averaged offset m = (X, Y, Z) / S (shared with SsAvgCorrRadFold)
+    static __device__ __forceinline__ float factor(const SsDev &P, const Acc &a, const float (&m)[3]) {
+        const float s = a.a.s;
         const float t[3] = { __fdiv_rn(a.tx, s), __fdiv_rn(a.ty, s), __fdiv_rn(a.tz, s) };
         const float q[3][3] = { { __fdiv_rn(a.mxx, s), __fdiv_rn(a.mxy, s), __fdiv_rn(a.mxz, s) },
                                 { 0.0f, __fdiv_rn(a.myy, s), __fdiv_rn(a.myz, s) },
@@ -92,8 +97,88 @@ struct SsAvgCorrFold {
         const float ev = __fmul_rn(__fdiv_rn(6.0f, P.h2), e);
         float g = __fdiv_rn(__fsub_rn(P.av_high, ev), __fsub_rn(P.av_high, P.av_low));
         g = g > 0.0f ? (g < 1.0f ? g : 1.0f) : 0.0f;                  // a NaN EV gives f = 0
-        float f = __fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(g, 3.0f), g), 3.0f), g);
-        f = f < 1.0f ? f : 1.0f;                                       // rounding gives 1 + 2^-23 for some gamma < 1
-        return __fsub_rn(plain, __fmul_rn(P.av_rs, __fsub_rn(1.0f, f)));
+        const float f = __fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(g, 3.0f), g), 3.0f), g);
+        return f < 1.0f ? f : 1.0f;                                    // rounding gives 1 + 2^-23 for some gamma < 1
     }
 };
+
+// Per-particle radii of the averaged-position surface (Zhu & Bridson's r_bar), the opt-in of ss_context_set_averaged_radii_f32;
+// DESIGN.md §12.2.  Each record carries delta_j = R_j - R_s (R_j = radius_factor * r_j) in the side array SsAnArgs::rrec, at the
+// record's index; with the same weight w_j as S, X, Y, Z one more sum Q = sum_j w_j delta_j gives b = Q / S, r_bar = R_s + b and
+//     plain:      v = (h - |m|) + b                      (inside where |m| < r_bar)
+//     corrected:  v = ((h - |m|) + b) - (R_s + b) (1 - f)   (inside where |m| < f r_bar)
+// against the unchanged threshold h - R_s.  Every delta_j = +0 gives Q = b = +0, and the values of SsAvgFold / SsAvgCorrFold bit
+// for bit.  The folds compose those two: the candidates, their order and the other sums are theirs.
+struct SsAvgRadFold {
+    static constexpr int SELECT_BOXES = 4;          // 5 accumulators per point: k_fold_select holds 8 points per lane
+    struct Cand { SsAvgFold::Cand c; float delta; };
+    struct Acc { SsAvgFold::Acc a; float q; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return Cand{ SsAvgFold::load(A, src), A.rrec[src] }; }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgFold::zero(), 0.0f }; }
+    // w_j delta_j added to q when the candidate is within the support (the weight of SsAvgFold::add)
+    static __device__ __forceinline__ void add_q(const SsDev &P, const Cand &c, float gx, float gy, float gz, float &q) {
+        const float dx = __fsub_rn(c.c.r.x, gx), dy = __fsub_rn(c.c.r.y, gy), dz = __fsub_rn(c.c.r.z, gz);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+        if (!(d2 < P.h2)) return;
+        const float u = __fsub_rn(1.0f, __fdiv_rn(d2, P.h2));
+        const float w = __fmul_rn(__fmul_rn(u, u), u);
+        q = __fadd_rn(q, __fmul_rn(w, c.delta));
+    }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgFold::add(P, c.c, gx, gy, gz, a.a);
+        add_q(P, c, gx, gy, gz, a.q);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) {
+        if (!(a.a.s > 0.0f)) return 0.0f;
+        return __fadd_rn(SsAvgFold::value(P, a.a), __fdiv_rn(a.q, a.a.s));
+    }
+};
+
+struct SsAvgCorrRadFold {
+    static constexpr int SELECT_BOXES = 2;          // 14 accumulators per point: k_fold_select holds 4 points per lane
+    using Cand = SsAvgRadFold::Cand;
+    struct Acc { SsAvgCorrFold::Acc a; float q; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgRadFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgCorrFold::zero(), 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgCorrFold::add(P, c.c, gx, gy, gz, a.a);
+        SsAvgRadFold::add_q(P, c, gx, gy, gz, a.q);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) {
+        const float s = a.a.a.s;
+        if (!(s > 0.0f)) return 0.0f;
+        const float m[3] = { __fdiv_rn(a.a.a.x, s), __fdiv_rn(a.a.a.y, s), __fdiv_rn(a.a.a.z, s) };
+        const float b = __fdiv_rn(a.q, s);
+        const float f = SsAvgCorrFold::factor(P, a.a, m);
+        return __fsub_rn(__fadd_rn(SsAvgFold::value(P, a.a.a), b), __fmul_rn(__fadd_rn(P.av_rs, b), __fsub_rn(1.0f, f)));
+    }
+};
+
+// ------------------------------------------------------------------ per-particle radii (DESIGN.md §12.2) ----
+// Validation of the n input radii (all of them, before the particle-AABB filter): R_j = radius_factor * r_j must be finite with
+// 0 < R_j < h.  chk[0] counts the invalid radii, chk[1] receives the lowest invalid index (preset to 0 and 0xffffffff).
+__global__ void k_radii_check(const float *__restrict__ radii, uint64_t n, float factor, float h, uint32_t *__restrict__ chk) {
+    const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float R = __fmul_rn(factor, radii[i]);
+    if (R > 0.0f && R < h) return;                      // NaN and +-inf fail both comparisons or the second
+    atomicAdd(&chk[0], 1u);
+    atomicMin(&chk[1], (uint32_t)i);
+}
+
+// delta_j = R_j - R_s of the particles the particle-AABB filter keeps, compacted with the filter's flags and offsets (those of
+// k_filter_scatter, so that delta is indexed like the filtered positions); flag == NULL: no filter, delta_j for every particle.
+__global__ void k_radii_delta(const float *__restrict__ radii, uint64_t n, const uint8_t *__restrict__ flag, const uint32_t *__restrict__ off,
+                              float factor, float rs, float *__restrict__ delta) {
+    const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= n || (flag && !flag[i])) return;
+    delta[flag ? off[i] : i] = __fsub_rn(__fmul_rn(factor, radii[i]), rs);
+}
+
+// After k_records: the side array of SsAvgRadFold / SsAvgCorrRadFold, delta of every binned membership in bin order.
+__global__ void k_records_radius(uint32_t m, const uint32_t *__restrict__ key, const uint32_t *__restrict__ pidx, const float *__restrict__ delta,
+                                 float *__restrict__ out) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m || key[e] == 0xffffffffu) return;
+    out[e] = delta[pidx[e]];
+}

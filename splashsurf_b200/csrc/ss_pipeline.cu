@@ -137,11 +137,14 @@ struct ss_context {
     ss_averaged_surface_f32 avg{};
     int ac_on = 0;                   // 1: Jacobian correction of the averaged-position surface (SsAvgCorrFold) with `ac`
     ss_averaged_correction_f32 ac{};
+    int rad_on = 0;                  // 1: per-particle radii of the averaged-position surface (SsAvgRadFold, SsAvgCorrRadFold),
+    uint64_t rad_n = 0;              //    rad_n of them in av_radii
     cudaEvent_t ev_an[2] = { nullptr, nullptr };
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
         sub_flat, sub_off, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, tiles, vcnt,
         tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
+    DevBuf av_radii, av_delta, av_rrec, av_chk;      // per-particle radii: the caller's copy, delta_j (filtered), per membership, check
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
@@ -386,6 +389,26 @@ extern "C" int ss_context_set_averaged_correction_f32(ss_context *c, const ss_av
         return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface correction: t_low and t_high must be finite with 0 <= t_low < t_high");
     c->ac = *a; c->ac_on = 1;
     return SS_OK;
+}
+extern "C" int ss_context_set_averaged_radii_f32(ss_context *c, const float *radii, uint64_t n) {
+    if (!c) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL context");
+    if (!radii) { c->rad_on = 0; c->rad_n = 0; return SS_OK; }
+    if (n > 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "more than 2^32 particle radii are not supported by one device");
+    return ss_guard([&]() -> int {
+        CK(cudaSetDevice(c->device));
+        if (n) {
+            // host or device memory, like the positions; copied, so the caller may free its array when this returns
+            cudaPointerAttributes attr{};
+            const cudaError_t e = cudaPointerGetAttributes(&attr, radii);
+            const bool on_device = e == cudaSuccess && (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+            if (e != cudaSuccess) cudaGetLastError();
+            c->av_radii.ensure(n * 4);
+            CK(cudaMemcpyAsync(c->av_radii.p, radii, n * 4, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
+            CK(cudaStreamSynchronize(c->stream));
+        }
+        c->rad_on = 1; c->rad_n = n;
+        return SS_OK;
+    });
 }
 
 // ------------------------------------------------------------------ stage: input, filter, AABB, grid ----
@@ -752,8 +775,9 @@ static int stage_densities(ss_context *c, const SsDev &D, const float *d_xyz, ui
 // val_b still holds the membership particle indices in subdomain order (stable input for the bin sort).
 // Anisotropic mode: d_xyz are the smoothed centres and `an_g` / `an_det` the per-particle G entries and determinants; the records
 // then carry V det G and the G entries go to c->an_grec.  `record_event` = false: a re-binning that is not part of the stage time.
+// Per-particle radii of the averaged surface: `av_delta` (delta_j per filtered particle) goes to c->av_rrec per membership.
 static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, const float *d_rho, uint32_t M, uint32_t nsub, bool partitioned,
-                         const float *an_g = nullptr, const float *an_det = nullptr, bool record_event = true) {
+                         const float *an_g = nullptr, const float *an_det = nullptr, bool record_event = true, const float *av_delta = nullptr) {
     cudaStream_t st = c->stream;
     LAUNCH(c, k_bin_keys, nblk(M, 256), 256, D, d_xyz, M, c->cid.as<uint32_t>(), c->sub_flat.as<uint32_t>(), c->val_b.as<uint32_t>(),
            partitioned ? c->sub_owned.as<uint8_t>() : nullptr, c->key_a.as<uint32_t>());
@@ -770,6 +794,10 @@ static int stage_binning(ss_context *c, const SsDev &D, const float *d_xyz, cons
         c->an_grec.ensure((size_t)M * 32);
         LAUNCH(c, k_records_aniso, nblk(M, 256), 256, M, c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(), an_g, an_det, c->rec.as<float4>(),
                c->an_grec.as<float4>());
+    }
+    if (av_delta) {
+        c->av_rrec.ensure((size_t)M * 4);
+        LAUNCH(c, k_records_radius, nblk(M, 256), 256, M, c->key_b.as<uint32_t>(), c->val_a.as<uint32_t>(), av_delta, c->av_rrec.as<float>());
     }
     int h_err = 0;
     CK(cudaMemcpyAsync(&h_err, c->err.p, 4, cudaMemcpyDeviceToHost, st));
@@ -821,17 +849,18 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
 }
 
 // Warp-per-brick level set of one batch for the fold F (anisotropic kernels, ss_aniso.cuh, or the averaged-position surface with
-// or without its Jacobian correction, ss_averaged.cuh): work list of non-empty bricks without extension tasks (the single-point
+// or without its Jacobian correction and per-particle radii, ss_averaged.cuh): work list of non-empty bricks without extension tasks (the single-point
 // planes of the last brick are bricks of their own), the 512-slot slice, then the 4096-slot slice, then selection.  Every listed brick gets state 2 (exact values).
 // Returns the length of the work list.
 template <class F>
-static uint32_t launch_fold_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, const float4 *grec, uint64_t &ls_launches, uint64_t *received) {
+static uint32_t launch_fold_levelset(ss_context *c, const SsDev &D, uint32_t nbatch, const float4 *grec, const float *rrec, uint64_t &ls_launches,
+                                     uint64_t *received) {
     SsDev Dw = D;
     Dw.ext_bricks = 0;
     const uint32_t n_work = build_worklist(c, Dw, nbatch);
     const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left, uint8_t *bstate) {
         SsAnArgs A{};
-        A.bins = context_bins(c); A.grec = grec; A.bricks = list; A.n_bricks = n; A.tiles = c->tiles.as<float>();
+        A.bins = context_bins(c); A.grec = grec; A.rrec = rrec; A.bricks = list; A.n_bricks = n; A.tiles = c->tiles.as<float>();
         A.bstate = bstate; A.fallback = left;
         return A;
     };
@@ -858,9 +887,12 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
     A.wflag = nullptr; A.fix_bricks = nullptr; A.bstate = c->bstate.as<uint8_t>();
     uint64_t *const paths = out->ls_paths;
     const bool folded = D.aniso || averaged;            // warp-per-brick fold cascade, exact values only
-    const uint32_t n_work = D.aniso ? launch_fold_levelset<SsAnisoFold>(c, D, nbatch, c->an_grec.as<float4>(), ls_launches, paths + SS_LSP_ANISO_512)
-                          : averaged && c->ac_on ? launch_fold_levelset<SsAvgCorrFold>(c, D, nbatch, nullptr, ls_launches, paths + SS_LSP_AVG_512)
-                          : averaged ? launch_fold_levelset<SsAvgFold>(c, D, nbatch, nullptr, ls_launches, paths + SS_LSP_AVG_512)
+    const float *const rrec = c->av_rrec.as<float>();    // per-particle radii (c->rad_on): delta_j per membership
+    const uint32_t n_work = D.aniso ? launch_fold_levelset<SsAnisoFold>(c, D, nbatch, c->an_grec.as<float4>(), nullptr, ls_launches, paths + SS_LSP_ANISO_512)
+                          : averaged && c->rad_on && c->ac_on ? launch_fold_levelset<SsAvgCorrRadFold>(c, D, nbatch, nullptr, rrec, ls_launches, paths + SS_LSP_AVG_512)
+                          : averaged && c->rad_on ? launch_fold_levelset<SsAvgRadFold>(c, D, nbatch, nullptr, rrec, ls_launches, paths + SS_LSP_AVG_512)
+                          : averaged && c->ac_on ? launch_fold_levelset<SsAvgCorrFold>(c, D, nbatch, nullptr, nullptr, ls_launches, paths + SS_LSP_AVG_512)
+                          : averaged ? launch_fold_levelset<SsAvgFold>(c, D, nbatch, nullptr, nullptr, ls_launches, paths + SS_LSP_AVG_512)
                           : build_worklist(c, D, nbatch);
     A.work_list = c->list_ls.as<uint32_t>();
     const bool split_certify = !folded && c->ls_variant >= 1 && !exact_all && certify_runs <= 32;
@@ -1046,6 +1078,33 @@ static int weld_boundary_vertices(ss_context *c, ss_surface *out, uint64_t vtota
     return SS_OK;
 }
 
+// Per-particle radii of the averaged surface (DESIGN.md §12.2): checks all n_in radii of the context (0 < radius_factor * r_j < h,
+// one read-back of the count and the first offending index), then delta_j = radius_factor * r_j - R_s of the particles the
+// particle-AABB filter kept (prepare_particles left its flags and offsets in the context scratch) into c->av_delta.
+static int prepare_radii(ss_context *c, const ss_params_f32 *p, uint64_t n_in, float factor, float h, float rs) {
+    if (!n_in) return SS_OK;
+    cudaStream_t st = c->stream;
+    const float *radii = c->av_radii.as<float>();
+    c->av_chk.ensure(8);
+    const uint32_t init[2] = { 0u, 0xffffffffu };
+    uint32_t chk[2];
+    CK(cudaMemcpyAsync(c->av_chk.p, init, 8, cudaMemcpyHostToDevice, st));
+    LAUNCH(c, k_radii_check, nblk(n_in, 256), 256, radii, n_in, factor, h, c->av_chk.as<uint32_t>());
+    CK(cudaMemcpyAsync(chk, c->av_chk.p, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (chk[0]) {
+        char msg[240];
+        snprintf(msg, sizeof msg, "averaged surface radii: radius_factor * radius must be finite and lie in (0, compact support radius); "
+                 "%u of %llu radii are not, the first at index %u", chk[0], (unsigned long long)n_in, chk[1]);
+        return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+    }
+    const bool filtered = p->has_particle_aabb != 0;
+    c->av_delta.ensure(n_in * 4);
+    LAUNCH(c, k_radii_delta, nblk(n_in, 256), 256, radii, n_in, filtered ? c->filt_flag.as<uint8_t>() : nullptr,
+           filtered ? c->filt_off.as<uint32_t>() : nullptr, factor, rs, c->av_delta.as<float>());
+    return SS_OK;
+}
+
 static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params_f32 *p, ss_surface *out, const Partition &part = Partition(),
                               bool global_mode = false) {
     const uint64_t n = PP.n;
@@ -1109,6 +1168,10 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
             return ss_fail(SS_ERR_INVALID_PARAMETER, "averaged surface: radius_factor * particle_radius must lie in (0, compact support radius)");
         D.thr = fsubr(h, rs);
         D.av_rs = rs; D.av_low = c->ac.t_low; D.av_high = c->ac.t_high;     // read by SsAvgCorrFold only (DESIGN.md §12.1)
+        if (c->rad_on) {
+            rc = prepare_radii(c, p, out->n_in, c->avg.radius_factor, h, rs);
+            if (rc) return rc;
+        }
     }
     D.nsD = (int)ceil(((double)S * cs + 3.0 * (double)ns_margin) / (double)h) + 3;
     D.ns_stride = D.nsD * D.nsD * D.nsD;
@@ -1250,7 +1313,8 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     }
     CK(cudaEventRecord(c->ev[4], st));
     if (aniso) rc = stage_binning(c, D, out->an_xbar.as<float>(), d_rho, M, nsub, false, out->an_g.as<float>(), c->an_det.as<float>());
-    else rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, part.enabled != 0);
+    else rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, part.enabled != 0, nullptr, nullptr, true,
+                            averaged && c->rad_on ? c->av_delta.as<float>() : nullptr);
     if (rc) return rc;
 
     // ---- level set + marching cubes over batches of subdomain tiles
@@ -1677,6 +1741,7 @@ static int reconstruct_partition_impl(ss_context *c, const float *xyz, uint64_t 
     if (c->an_on) return ss_fail(SS_ERR_UNSUPPORTED, "anisotropic kernels are not available on partitioned (multi-GPU) reconstructions");
     if (c->avg_on) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface is not available on partitioned (multi-GPU) reconstructions");
     if (c->ac_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "the Jacobian correction applies to the averaged-position surface, which is off");
+    if (c->rad_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "per-particle radii apply to the averaged-position surface, which is off");
     if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "partitioned reconstruction requires the subdomain grid");
     if (axis < 0 || axis > 2 || own_lo < 0 || own_hi < own_lo || halo < 0) return ss_fail(SS_ERR_INVALID_PARAMETER, "bad partition");
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
@@ -1738,6 +1803,12 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
     int rc = validate_params(p);
     if (rc) return rc;
     if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
+    if (c->rad_on && !c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "per-particle radii apply to the averaged-position surface, which is off");
+    if (c->rad_on && c->rad_n != n_in) {
+        char msg[160];
+        snprintf(msg, sizeof msg, "averaged surface radii: %llu radii for %llu particles", (unsigned long long)c->rad_n, (unsigned long long)n_in);
+        return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+    }
     return with_new_surface(c, out, [&](ss_surface *s) -> int {
         s->n_in = n_in;
         Prepared P;

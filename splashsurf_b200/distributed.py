@@ -226,6 +226,9 @@ class Runner:
         if averaged_surface is not None and world > 1:
             raise ValueError("the averaged-position surface is not available on multi-GPU (partitioned) reconstructions; run it on one GPU")
         self.anisotropy, self.averaged_surface = anisotropy, averaged_surface
+        # per-particle radii of the averaged-position surface (DESIGN.md section 12.2): None, or one float32 radius per particle of
+        # the next steps' clouds, a torch tensor on this rank's device or a numpy array; one GPU only
+        self.particle_radii = None
         # how the global maximum subdomain population (sparse rule) reaches the library: "stats" (default) = the plan statistics
         # count the members of every subdomain with the exact classifier (ss_partition_members_f32), their all-reduced maximum
         # is passed to ONE library call; "two_call" = decomposition pre-pass, all-reduce, full call (one more library call per step);
@@ -280,15 +283,32 @@ class Runner:
         return np.ascontiguousarray(particles[lo:hi])
 
     # -- single GPU
+    def _radii_arg(self):
+        """(pointer, count, keep-alive) of `particle_radii` for ss_context_set_averaged_radii_f32."""
+        r = self.particle_radii
+        if isinstance(r, torch.Tensor):
+            if r.dtype != torch.float32 or r.dim() != 1 or not r.is_contiguous():
+                raise ValueError("particle_radii must be a contiguous 1-D float32 tensor")
+            return r.data_ptr(), r.shape[0], r
+        a = np.asarray(r)
+        if not np.issubdtype(a.dtype, np.floating) or a.ndim != 1:
+            raise ValueError("particle_radii must be a 1-D float array")
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        return a.ctypes.data, len(a), a
+
     def _step_single(self, xyz_ptr: int, n: int, copy_out: bool, params=None, force_copy: bool = False) -> dict:
         L = self.ctx._L
         from . import _check
+        radii = self.particle_radii is not None
         try:
             if self.anisotropy is not None:
                 _check(L, L.ss_context_set_anisotropy_f32(self.ctx._h, C.byref(self.anisotropy._abi())))
             if self.averaged_surface is not None:
                 _check(L, L.ss_context_set_averaged_surface_f32(self.ctx._h, C.byref(self.averaged_surface._abi())))
                 _check(L, L.ss_context_set_averaged_correction_f32(self.ctx._h, self.averaged_surface._correction_abi()))
+            if radii:
+                ptr, nr, _keep = self._radii_arg()
+                _check(L, L.ss_context_set_averaged_radii_f32(self.ctx._h, ptr, nr))
             s = self.ctx.reconstruct_raw(xyz_ptr, n, self.params if params is None else params)
         finally:
             if self.anisotropy is not None:
@@ -296,6 +316,8 @@ class Runner:
             if self.averaged_surface is not None:
                 L.ss_context_set_averaged_surface_f32(self.ctx._h, None)
                 L.ss_context_set_averaged_correction_f32(self.ctx._h, None)
+            if radii:
+                L.ss_context_set_averaged_radii_f32(self.ctx._h, None, 0)
         keep = self.keep_surface and self.world == 1
         try:
             out = self._collect(s, copy_out, n_local=n, force_copy=force_copy)
@@ -358,6 +380,8 @@ class Runner:
 
     # -- public step: `x` is this rank's (n, 3) float32 tensor (cuda, or pinned host for the end-to-end path)
     def step(self, x, n: Optional[int] = None, copy_out: bool = False) -> dict:
+        if self.particle_radii is not None and self.world > 1:
+            raise ValueError("per-particle radii (averaged-position surface) are not available on multi-GPU (partitioned) reconstructions")
         if self.world == 1:
             if isinstance(x, int):
                 return self._step_single(x, int(n), copy_out)
@@ -786,12 +810,15 @@ class DistributedReconstructor:
         if self._aabb is not None:
             self.runner.grid_params = ss.make_params(**params)
 
-    def __call__(self, particles_local: np.ndarray):
+    def __call__(self, particles_local: np.ndarray, particle_radii=None):
+        """`particle_radii`: per-particle radii of the averaged-position surface (`reconstruct_surface`), one GPU only."""
         ss = self._ss
         p = np.ascontiguousarray(particles_local, dtype=np.float32).reshape(-1, 3)
+        if particle_radii is not None and self.world > 1:
+            raise ValueError("per-particle radii (averaged-position surface) are not available on multi-GPU (partitioned) reconstructions")
         if self.world == 1:
             r = ss.reconstruct_surface(p, context=self.ctx, sph_normals=self.sph_normals, anisotropy=self.anisotropy,
-                                       averaged_surface=self.averaged_surface, **self._kw)
+                                       averaged_surface=self.averaged_surface, particle_radii=particle_radii, **self._kw)
             return ss.MeshWithData(r.mesh, {"normals": r.normals} if self.sph_normals and r.normals is not None else {}, {})
         if self._aabb is not None:                    # lib.rs:369-406: particles outside the half-open box take no part
             p = np.ascontiguousarray(p[np.all(p >= self._aabb[0], axis=1) & np.all(p < self._aabb[1], axis=1)])

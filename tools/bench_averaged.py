@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Times the averaged-position surface (DESIGN.md §12), plain and with the Jacobian correction (§12.1), beside the standard
-reconstruction on the same cloud and the same context, one GPU: device-resident steps through splashsurf_b200.distributed.Runner (what
-bench.py times), the three modes alternated `--rounds` times.
+"""Times the averaged-position surface (DESIGN.md §12), plain and with the Jacobian correction (§12.1), each also with per-particle radii
+uniform in [0.8, 1.2] r (§12.2), beside the standard reconstruction on the same cloud and the same context, one GPU: device-resident
+steps through splashsurf_b200.distributed.Runner (what bench.py times), the modes alternated `--rounds` times (`--modes` picks some).
 Per mode and round: mean device ms per step over `--steps` timed steps after `--warmup` untimed ones, the stage times of the last step
 (CUDA events) and the mesh size.  The card name and its power limit are read at the start and at the end.  Prints one JSON line;
 writes nothing.
@@ -33,7 +33,9 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=2)
+    ap.add_argument("--modes", default="plain,averaged,averaged_corrected,averaged_radii,averaged_corrected_radii")
     a = ap.parse_args()
+    import numpy as np
     import torch
     import splashsurf_b200 as ss
     from splashsurf_b200 import distributed as ssd
@@ -42,10 +44,17 @@ def main():
     x = syn.dam_break_50m() if a.particles == 50_000_400 else syn.dam_break_scaled(a.particles, 0.01, 3)
     ctx = ss.Context(0)
     params = ss.make_params(particle_radius=0.01, smoothing_length=2.0, cube_size=0.5)
+    corr = ss.AveragedSurface(correction=ss.JacobianCorrection())
     runners = {"plain": ssd.Runner(ctx, params, 1, 0, 0), "averaged": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=ss.AveragedSurface()),
-               "averaged_corrected": ssd.Runner(ctx, params, 1, 0, 0,
-                                                averaged_surface=ss.AveragedSurface(correction=ss.JacobianCorrection()))}
+               "averaged_corrected": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=corr),
+               "averaged_radii": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=ss.AveragedSurface()),
+               "averaged_corrected_radii": ssd.Runner(ctx, params, 1, 0, 0, averaged_surface=corr)}
+    runners = {m: runners[m] for m in a.modes.split(",")}
     dev = torch.from_numpy(x).cuda()
+    radii = torch.from_numpy((np.random.default_rng(4).uniform(0.8, 1.2, len(x)) * 0.01).astype(np.float32)).cuda()
+    for m in ("averaged_radii", "averaged_corrected_radii"):
+        if m in runners:
+            runners[m].particle_radii = radii
     torch.cuda.synchronize()
     out = {"tool": "bench_averaged", "particles": len(x), "workload": "dam break, r = 0.01, -l 2, -c 0.5", "card_before": card_before,
            "steps": a.steps, "warmup": a.warmup, "runs": []}
