@@ -355,6 +355,31 @@ int ss_context_set_averaged_correction_f32(ss_context *ctx, const ss_averaged_co
  * surface on, SS_ERR_INVALID_PARAMETER with it off).  Cost: 4 bytes per subdomain membership and 8 bytes per particle. */
 int ss_context_set_averaged_radii_f32(ss_context *ctx, const float *radii /* NULL = off */, uint64_t n);
 
+/* ---- The level set at arbitrary points (specification in DESIGN.md section 13): what the field is at a point, and whether the point
+ * lies inside the liquid, for every level set of the reconstruction.  The value at p (f32, the caller's coordinates) is the tile
+ * formula of the level set with p in place of the grid point: the same candidates, the same operations, ascending particle index.
+ *   - standard level set: phi = phi + V_j W(sqrt(d2)) over d2 < 1.01 h^2, from 0 -- the scalar formula of sparse subdomains and
+ *     simd = off, so at grid points it equals the tiles of an enable_simd = 0 reconstruction bit for bit (with SIMD on, the tiles'
+ *     remainder lanes use fma and differ by a few ulp);
+ *   - anisotropic, averaged, corrected, radii: the brick folds of those modes unchanged.
+ * Points no candidate reaches are 0, among them points outside the grid and points in subdomains without members.  A point is
+ * inside iff value > threshold, the threshold of marching cubes (iso_surface_threshold, or h - R_s for the averaged surface).
+ *
+ * ss_levelset_field_create_f32 uses the context's anisotropy / averaged surface / correction / radii settings and runs the
+ * reconstruction's decomposition (always: spatial_decomposition is not read), densities, anisotropy and binning, then stops.  Grid,
+ * densities, particle-AABB filter and refusals are those of ss_reconstruct_surface_f32 with the subdomain grid.  The result is a
+ * surface without a mesh (accessors: ss_surface_grid, ss_surface_copy_particle_densities, ss_surface_num_particles; free with
+ * ss_surface_free).  Its records live in the context's scratch: query it before the next reconstruction, interpolator or field on
+ * the same context (SS_ERR_INVALID_PARAMETER afterwards).
+ * ss_levelset_field_at_f32: m points (m x 3 floats) -> m values; both arrays in host or device memory.  A non-finite coordinate is
+ * SS_ERR_INVALID_PARAMETER naming the first such point.
+ * ss_levelset_field_paths: the point groups of the last query per tier of the cascade: out[0] 512-slot slice, out[1] 4096-slot
+ * slice, out[2] selection walk. */
+int ss_levelset_field_create_f32(ss_context *ctx, const float *xyz, uint64_t n, const ss_params_f32 *params, ss_surface **out);
+int ss_levelset_field_at_f32(ss_surface *field, const float *points, uint64_t m, float *out);
+int ss_levelset_field_threshold_f32(const ss_surface *field, float *threshold);
+int ss_levelset_field_paths(const ss_surface *field, uint64_t out[3]);
+
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.
  * The entries marked [bins] query the particles through the splat bins of the reconstruction that produced the surface and

@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "LevelSetField", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -205,6 +205,10 @@ def _bind(L):
     L.ss_context_set_averaged_correction_f32.argtypes = [vp, C.POINTER(_AveragedCorrection)]
     L.ss_context_set_averaged_radii_f32.argtypes = [vp, vp, C.c_uint64]
     L.ss_surface_anisotropy_ms.argtypes = [vp]
+    L.ss_levelset_field_create_f32.argtypes = [vp, vp, C.c_uint64, C.POINTER(_Params), C.POINTER(vp)]
+    L.ss_levelset_field_at_f32.argtypes = [vp, vp, C.c_uint64, vp]
+    L.ss_levelset_field_threshold_f32.argtypes = [vp, C.POINTER(C.c_float)]
+    L.ss_levelset_field_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
         raise ImportError("libsplashsurf_b200.so ABI version mismatch")
@@ -1036,6 +1040,118 @@ class SphInterpolator:
         L = self._ctx._L
         _check(L, L.ss_sph_interpolate_normals_at_f32(self._s, x.ctypes.data if len(x) else None, len(x), out.ctypes.data if len(x) else None))
         return out
+
+    def close(self):
+        if getattr(self, "_s", None):
+            self._ctx._L.ss_surface_free(self._s)
+            self._s = None
+            if self._own:
+                self._ctx.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class LevelSetField:
+    """The level set of ``reconstruct_surface`` at arbitrary points, on the GPU (DESIGN.md section 13): the field value and whether a
+    point lies inside the liquid, for the standard, anisotropic and averaged-position level sets -- whitewater classification,
+    collision, sphere tracing, or the averaged field ``h - |g - x_bar(g)|`` as an approximate distance field.
+
+    The keywords mean what they mean in ``reconstruct_surface``; ``particles`` is an (N, 3) float32 array (float64 raises
+    ``TypeError``).  The value at a point is the level set's tile formula with the point in place of the grid point; points no
+    particle reaches are 0.  ``value > threshold`` is inside (the threshold of marching cubes: ``iso_surface_threshold``, or
+    ``h - R_s`` for the averaged surface).  The standard level set uses its scalar formula, so at grid points it equals the tiles
+    of ``reconstruct_surface(..., simd=False)`` bit for bit.  The particles are always decomposed into subdomains; grid and
+    densities are those of the reconstruction with ``subdomain_grid_auto_disable=False``.
+
+    The records stay on the device inside a context of their own for the lifetime of the object (pass ``context=`` to share one:
+    the field is then only valid until the next reconstruction, interpolator or field on that context)."""
+
+    def __init__(self, particles, *, particle_radius: float, rest_density: float = 1000.0, smoothing_length: float, cube_size: float,
+                 iso_surface_threshold: float = 0.6, aabb_min: Optional[Sequence[float]] = None, aabb_max: Optional[Sequence[float]] = None,
+                 subdomain_num_cubes_per_dim: int = 64, anisotropy: Optional[Anisotropy] = None,
+                 averaged_surface: Optional[AveragedSurface] = None, particle_radii=None, context: Optional[Context] = None):
+        arr = np.asarray(particles)
+        if arr.dtype != np.float32:
+            raise TypeError("unsupported scalar type: the device path reconstructs float32 particles only")
+        if arr.ndim != 2 or arr.shape[1] != 3:
+            raise ValueError("particles must have shape (N, 3)")
+        arr = np.ascontiguousarray(arr)
+        radii = _particle_radii(particle_radii, len(arr), averaged_surface)
+        p = make_params(particle_radius=particle_radius, rest_density=rest_density, smoothing_length=smoothing_length, cube_size=cube_size,
+                        iso_surface_threshold=iso_surface_threshold, aabb_min=aabb_min, aabb_max=aabb_max,
+                        subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim)
+        self._own = context is None
+        self._ctx = Context() if context is None else context
+        self._n_in = len(arr)
+        self._s = C.c_void_p()
+        L = self._ctx._L
+        try:
+            try:
+                _check(L, L.ss_context_set_anisotropy_f32(self._ctx._h, C.byref(anisotropy._abi()) if anisotropy is not None else None))
+                _check(L, L.ss_context_set_averaged_surface_f32(self._ctx._h, C.byref(averaged_surface._abi()) if averaged_surface is not None else None))
+                _check(L, L.ss_context_set_averaged_correction_f32(self._ctx._h, averaged_surface._correction_abi() if averaged_surface is not None else None))
+                if radii is not None:
+                    _check(L, L.ss_context_set_averaged_radii_f32(self._ctx._h, radii.ctypes.data, len(radii)))
+                _check(L, L.ss_levelset_field_create_f32(self._ctx._h, arr.ctypes.data if len(arr) else None, len(arr), C.byref(p), C.byref(self._s)))
+            finally:
+                L.ss_context_set_anisotropy_f32(self._ctx._h, None)
+                L.ss_context_set_averaged_surface_f32(self._ctx._h, None)
+                L.ss_context_set_averaged_correction_f32(self._ctx._h, None)
+                L.ss_context_set_averaged_radii_f32(self._ctx._h, None, 0)
+        except Exception:
+            if self._own:
+                self._ctx.close()
+            raise
+        t = C.c_float()
+        _check(L, L.ss_levelset_field_threshold_f32(self._s, C.byref(t)))
+        self.threshold = float(t.value)
+        n = L.ss_surface_num_particles(self._s)
+        self.particle_densities = np.empty(n, dtype=np.float32)
+        if n:
+            _check(L, L.ss_surface_copy_particle_densities(self._s, self.particle_densities.ctypes.data))
+        g = _Grid()
+        _check(L, L.ss_surface_grid(self._s, C.byref(g)))
+        self.grid = UniformGrid._from(g)
+
+    def evaluate(self, points):
+        """The field at the points: an (M, 3) float32 numpy array gives an (M,) float32 numpy array; a CUDA float32 torch tensor of
+        shape (M, 3) is read on the device and gives an (M,) CUDA tensor."""
+        L = self._ctx._L
+        if hasattr(points, "data_ptr") and getattr(points, "is_cuda", False):
+            import torch
+            if points.dtype != torch.float32:
+                raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
+            if points.ndim != 2 or points.shape[1] != 3:
+                raise ValueError("points must have shape (M, 3)")
+            x = points.contiguous()
+            out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+            torch.cuda.current_stream(x.device).synchronize()
+            _check(L, L.ss_levelset_field_at_f32(self._s, x.data_ptr() if len(x) else None, len(x), out.data_ptr() if len(x) else None))
+            return out
+        x = np.asarray(points)
+        if x.dtype != np.float32:
+            raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
+        if x.ndim != 2 or x.shape[1] != 3:
+            raise ValueError("points must have shape (M, 3)")
+        x = np.ascontiguousarray(x)
+        out = np.empty(len(x), dtype=np.float32)
+        _check(L, L.ss_levelset_field_at_f32(self._s, x.ctypes.data if len(x) else None, len(x), out.ctypes.data if len(x) else None))
+        return out
+
+    def inside(self, points):
+        """``evaluate(points) > threshold``."""
+        return self.evaluate(points) > self.threshold
+
+    @property
+    def paths(self) -> dict:
+        """The point groups of the last ``evaluate`` per tier of the cascade: 512-slot slice, 4096-slot slice, selection walk."""
+        out = (C.c_uint64 * 3)()
+        _check(self._ctx._L, self._ctx._L.ss_levelset_field_paths(self._s, out))
+        return {"512": int(out[0]), "4096": int(out[1]), "select": int(out[2])}
 
     def close(self):
         if getattr(self, "_s", None):

@@ -217,37 +217,64 @@ struct SsAnisoFold {
     static __device__ __forceinline__ float value(const SsDev &, const Acc &a) { return a.phi; }
 };
 
+// The candidates of bins K of subdomain s, one warp: counts them, and when there are 1 to CAP of them stages their sort keys
+// (particle index << 32 | record index) in s_key, run by run, and sorts them ascending.  Returns the count C (nothing is staged
+// for C = 0 or C > CAP).  Shared by the brick kernels below and the point queries of ss_field.cuh.
+template <int CAP>
+__device__ __forceinline__ uint32_t ss_stage_candidates(const SsDev &P, const SsBins &B, uint32_t s, const SsBrickBins &K, unsigned long long *s_key,
+                                                        int lane) {
+    uint32_t C = 0;
+    for (int r0 = 0; r0 < K.nruns; r0 += 32) {
+        uint32_t a;
+        uint32_t len = ss_brick_run(P, B, s, K, r0 + lane, a);
+        for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
+        C += len;
+    }
+    if (C == 0 || C > (uint32_t)CAP) return C;
+    uint32_t dst0 = 0;
+    for (int r0 = 0; r0 < K.nruns; r0 += 32) {
+        uint32_t a, tot;
+        const uint32_t len = ss_brick_run(P, B, s, K, r0 + lane, a);
+        const uint32_t dst = dst0 + ss_warp_excl_scan(len, lane, tot);
+        const int nr = min(32, K.nruns - r0);
+        for (int rr = 0; rr < nr; ++rr) {
+            const uint32_t ra = __shfl_sync(0xffffffffu, a, rr), rl = __shfl_sync(0xffffffffu, len, rr), rd = __shfl_sync(0xffffffffu, dst, rr);
+            for (uint32_t t = lane; t < rl; t += 32) s_key[rd + t] = ((unsigned long long)B.pidx[ra + t] << 32) | (unsigned long long)(ra + t);
+        }
+        dst0 += tot;
+    }
+    ss_sort_keys<true>(s_key, (int)C);
+    return C;
+}
+
+// The selection walk over bins K of subdomain s, one warp: the smallest candidate key above `last` (any key when `first`), ~0 when
+// none is left.  O(C / 32) per step; for bricks and point groups above the largest slice.
+__device__ __forceinline__ unsigned long long ss_select_next(const SsDev &P, const SsBins &B, uint32_t s, const SsBrickBins &K, unsigned long long last,
+                                                             bool first, int lane) {
+    unsigned long long best = ~0ull;
+    for (int r = 0; r < K.nruns; ++r) {
+        uint32_t a;
+        const uint32_t len = ss_brick_run(P, B, s, K, r, a);
+        for (uint32_t t = a + lane; t < a + len; t += 32) {
+            const unsigned long long kk = ((unsigned long long)B.pidx[t] << 32) | (unsigned long long)t;
+            if ((first || kk > last) && kk < best) best = kk;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
+    return best;
+}
+
 template <class F, int CAP>
 __device__ __forceinline__ void ss_fold_brick(const SsDev &P, const SsAnArgs &A, unsigned long long *s_key, uint16_t *s_list, uint32_t work, int lane) {
     const uint32_t brick_lin = A.bricks[work];
     const SsAnBrick N = ss_an_brick(P, A, brick_lin);
     if (A.bstate && lane == 0) A.bstate[brick_lin] = 2;
-    uint32_t C = 0;
-    for (int r0 = 0; r0 < N.K.nruns; r0 += 32) {
-        uint32_t a;
-        uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r0 + lane, a);
-        for (int o = 16; o > 0; o >>= 1) len += __shfl_xor_sync(0xffffffffu, len, o);
-        C += len;
-    }
+    const uint32_t C = ss_stage_candidates<CAP>(P, A.bins, N.T.s, N.K, s_key, lane);
     if (C == 0) return;                                      // pre-zeroed tile: the value of a point without candidates is 0
     if (C > (uint32_t)CAP) {
         if (lane == 0) A.fallback[1 + atomicAdd(&A.fallback[0], 1u)] = brick_lin;
         return;
     }
-    // ---- stage the sort keys (particle index << 32 | record index), run by run
-    uint32_t dst0 = 0;
-    for (int r0 = 0; r0 < N.K.nruns; r0 += 32) {
-        uint32_t a, tot;
-        const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r0 + lane, a);
-        const uint32_t dst = dst0 + ss_warp_excl_scan(len, lane, tot);
-        const int nr = min(32, N.K.nruns - r0);
-        for (int rr = 0; rr < nr; ++rr) {
-            const uint32_t ra = __shfl_sync(0xffffffffu, a, rr), rl = __shfl_sync(0xffffffffu, len, rr), rd = __shfl_sync(0xffffffffu, dst, rr);
-            for (uint32_t t = lane; t < rl; t += 32) s_key[rd + t] = ((unsigned long long)A.bins.pidx[ra + t] << 32) | (unsigned long long)(ra + t);
-        }
-        dst0 += tot;
-    }
-    ss_sort_keys<true>(s_key, (int)C);
 
     float *const tile = A.tiles + (size_t)N.B.tile * P.np * P.np * P.np;
     const SsSubLane L = ss_sub_lane(P, lane);
@@ -314,16 +341,7 @@ k_fold_select(SsDev P, SsAnArgs A) {
         unsigned long long last = 0;
         bool first = true;
         for (;;) {
-            unsigned long long best = ~0ull;
-            for (int r = 0; r < N.K.nruns; ++r) {
-                uint32_t a;
-                const uint32_t len = ss_brick_run(P, A.bins, N.T.s, N.K, r, a);
-                for (uint32_t t = a + lane; t < a + len; t += 32) {
-                    const unsigned long long kk = ((unsigned long long)A.bins.pidx[t] << 32) | (unsigned long long)t;
-                    if ((first || kk > last) && kk < best) best = kk;
-                }
-            }
-            for (int o = 16; o > 0; o >>= 1) { const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o); if (other < best) best = other; }
+            const unsigned long long best = ss_select_next(P, A.bins, N.T.s, N.K, last, first, lane);
             if (best == ~0ull) break;
             last = best; first = false;
             const typename F::Cand cd = F::load(A, (uint32_t)best);

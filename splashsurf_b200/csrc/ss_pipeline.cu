@@ -10,6 +10,7 @@
 #include "ss_exact.cuh"
 #include "ss_aniso.cuh"
 #include "ss_averaged.cuh"
+#include "ss_field.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
 
@@ -145,6 +146,9 @@ struct ss_context {
         sub_flat, sub_off, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, tiles, vcnt,
         tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
     DevBuf av_radii, av_delta, av_rrec, av_chk;      // per-particle radii: the caller's copy, delta_j (filtered), per membership, check
+    // level-set field queries (ss_field.cuh): points, group keys and caller indices (sorted and not), group starts, values, checks,
+    // and the candidate bin ranges of a group
+    DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng;
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
@@ -181,6 +185,11 @@ struct ss_surface {
     std::vector<float> tile;
     ss_timings tm{};
     uint64_t ls_paths[SS_LSP_N] = {};                        // ss_surface_levelset_paths
+    // level-set field (ss_levelset_field_create_f32): the level set's device constants, its fold, whether records were binned
+    int fld = 0, fld_mode = 0, fld_ready = 0;
+    SsDev fld_D{};
+    uint32_t fld_nsub = 0;
+    uint64_t fld_paths[3] = {};                              // groups of the last query per tier: 512, 4096, select
 };
 
 // ------------------------------------------------------------------ host grid math (exact f32) ----
@@ -626,6 +635,19 @@ static void upload_brick_ranges(ss_context *c, const SsDev &D) {
     CK(cudaStreamSynchronize(c->stream));
 }
 
+// Candidate bin range of a level-set field's point group along one axis (ss_field.cuh): the bins overlapping [8b - R, 8b + 8 + R),
+// because a point of brick b lies anywhere in the cells 8b .. 8b + 7 -> c->fld_rng.
+static void upload_field_brick_ranges(ss_context *c, const SsDev &D) {
+    std::vector<int2> h_rng(D.nb);
+    for (int bb = 0; bb < D.nb; ++bb) {
+        h_rng[bb].x = std::max(ss_floor_div(8 * bb - D.R, D.be) + D.nlo, 0);
+        h_rng[bb].y = std::min(ss_floor_div(8 * bb + 7 + D.R, D.be) + D.nlo, D.nbin - 1);
+    }
+    c->fld_rng.ensure((size_t)D.nb * sizeof(int2));
+    CK(cudaMemcpyAsync(c->fld_rng.p, h_rng.data(), (size_t)D.nb * sizeof(int2), cudaMemcpyHostToDevice, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+}
+
 // (i, j, k) of the flat index f of a subdomain in a grid of nsd subdomains (k fastest).
 static void subdomain_ijk(int64_t f, const int64_t nsd[3], int64_t ijk[3]) {
     ijk[0] = f / (nsd[1] * nsd[2]); ijk[1] = (f - ijk[0] * nsd[1] * nsd[2]) / nsd[2]; ijk[2] = f - ijk[0] * nsd[1] * nsd[2] - ijk[1] * nsd[2];
@@ -692,6 +714,8 @@ struct Partition {
     // SphInterpolator entry (ss_sph_interpolator_create_f32): densities supplied by the caller; stop after the particle bins are built
     const float *given_rho = nullptr;
     float given_mass = 0.0f;
+    // level-set field (ss_levelset_field_create_f32): the context's level set up to its records in the splat bins; no level set, no mesh
+    int field = 0;
 };
 
 // SPH densities (and optional CSR neighbour lists) of the filtered particles: per-subdomain cell lists on the h-lattice with
@@ -1231,6 +1255,11 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
         if (reduce && part.enabled && part.max_reduce) part.max_reduce(0, part.max_reduce_user);
         return SS_OK;
     };
+    if (part.field) {
+        out->fld = 1; out->fld_D = D;
+        out->fld_mode = aniso ? SS_FLD_ANISO : !averaged ? SS_FLD_SPH
+                      : c->ac_on ? (c->rad_on ? SS_FLD_AVG_CORR_RAD : SS_FLD_AVG_CORR) : (c->rad_on ? SS_FLD_AVG_RAD : SS_FLD_AVG);
+    }
     if (n == 0) return finish_early(true);
 
     // ---- decomposition: memberships (owner + ghosts), stable sort by subdomain
@@ -1316,6 +1345,16 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     else rc = stage_binning(c, D, d_xyz, d_rho, M, nsub, part.enabled != 0, nullptr, nullptr, true,
                             averaged && c->rad_on ? c->av_delta.as<float>() : nullptr);
     if (rc) return rc;
+    if (part.field) {
+        // the records of the level set stay in the scratch for ss_levelset_field_at_f32 (DESIGN.md §13)
+        if ((uint64_t)nsub * (uint64_t)(D.nb * D.nb * D.nb) >= 0xffffffffull)
+            return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many non-empty subdomains for 32-bit point group keys");
+        upload_field_brick_ranges(c, D);
+        out->fld_nsub = nsub; out->fld_ready = 1;
+        for (int e = 6; e <= 9; ++e) CK(cudaEventRecord(c->ev[e], st));
+        CK(cudaStreamSynchronize(st));
+        return SS_OK;
+    }
 
     // ---- level set + marching cubes over batches of subdomain tiles
     const size_t np3 = (size_t)D.np * D.np * D.np;
@@ -1797,18 +1836,31 @@ extern "C" int ss_surface_copy_subdomain_owned(const ss_surface *s, uint8_t *dst
 }
 
 // ------------------------------------------------------------------ public entry ----
-extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint64_t n_in, const ss_params_f32 *p, ss_surface **out) {
-    if (!c || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
-    *out = nullptr;
-    int rc = validate_params(p);
-    if (rc) return rc;
-    if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
+// The context's per-particle radii against the call's particle count (before the level set is built)
+static int check_radii_setting(const ss_context *c, uint64_t n_in) {
     if (c->rad_on && !c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "per-particle radii apply to the averaged-position surface, which is off");
     if (c->rad_on && c->rad_n != n_in) {
         char msg[160];
         snprintf(msg, sizeof msg, "averaged surface radii: %llu radii for %llu particles", (unsigned long long)c->rad_n, (unsigned long long)n_in);
         return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
     }
+    return SS_OK;
+}
+// The context's opt-in level sets combine: anisotropy excludes the averaged surface, the correction requires it
+static int check_level_set_modes(const ss_context *c) {
+    if (c->an_on && c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropic kernels and the averaged-position surface are exclusive");
+    if (c->ac_on && !c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "the Jacobian correction applies to the averaged-position surface, which is off");
+    return SS_OK;
+}
+
+extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint64_t n_in, const ss_params_f32 *p, ss_surface **out) {
+    if (!c || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    *out = nullptr;
+    int rc = validate_params(p);
+    if (rc) return rc;
+    if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
+    rc = check_radii_setting(c, n_in);
+    if (rc) return rc;
     return with_new_surface(c, out, [&](ss_surface *s) -> int {
         s->n_in = n_in;
         Prepared P;
@@ -1817,8 +1869,8 @@ extern "C" int ss_reconstruct_surface_f32(ss_context *c, const float *xyz, uint6
         s->n = P.n; s->grid = P.grid;
         // decomposition decision, lib.rs:421-464
         int use_dec = 0;
-        if (c->an_on && c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "anisotropic kernels and the averaged-position surface are exclusive");
-        if (c->ac_on && !c->avg_on) return ss_fail(SS_ERR_INVALID_PARAMETER, "the Jacobian correction applies to the averaged-position surface, which is off");
+        rc = check_level_set_modes(c);
+        if (rc) return rc;
         if (c->avg_on) {
             // averaged-position surface: subdomain path only, always decomposed (no auto-disable)
             if (p->spatial_decomposition != 1) return ss_fail(SS_ERR_UNSUPPORTED, "the averaged-position surface requires the subdomain grid (spatial_decomposition = UniformGrid)");
@@ -1999,6 +2051,140 @@ extern "C" int ss_surface_copy_anisotropy(const ss_surface *s, float *xbar, floa
     int rc = xbar ? copy_out(s, xbar, s->an_xbar.p, s->n * 12) : SS_OK;
     if (rc == SS_OK && g) rc = copy_out(s, g, s->an_g.p, s->n * 24);
     return rc;
+}
+
+// ------------------------------------------------------------------ level-set field at arbitrary points ----
+// DESIGN.md §13.  The handle is a surface without a mesh: the context's level set (standard, anisotropic or averaged, with the
+// context's settings) up to its records in the splat bins, which live in the context's scratch until the next reconstruction,
+// interpolator or field on that context.  Always decomposed: the grid, the densities, the filter and the refusals are those of
+// ss_reconstruct_surface_f32 with the subdomain grid.
+extern "C" int ss_levelset_field_create_f32(ss_context *c, const float *xyz, uint64_t n_in, const ss_params_f32 *p, ss_surface **out) {
+    if (!c || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    *out = nullptr;
+    int rc = validate_params(p);
+    if (rc) return rc;
+    if (p->subdomain_num_cubes_per_dim < 1) return ss_fail(SS_ERR_INVALID_PARAMETER, "subdomain_num_cubes_per_dim has to be >= 1");
+    if (n_in && !xyz) return ss_fail(SS_ERR_INVALID_PARAMETER, "xyz is NULL");
+    rc = check_radii_setting(c, n_in);
+    if (rc) return rc;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        s->n_in = n_in;
+        Prepared P;
+        int rc = prepare_particles(c, xyz, n_in, p, P, &s->inside_aabb);
+        if (rc) return rc;
+        s->n = P.n; s->grid = P.grid; s->used_decomposition = 1;
+        rc = check_level_set_modes(c);
+        if (rc) return rc;
+        Partition opt;
+        opt.field = 1;
+        rc = run_subdomain_grid(c, P, p, s, opt, /*global_mode=*/false);
+        if (rc) return rc;
+        front_timings(c, s);
+        return SS_OK;
+    });
+}
+
+// context of a field whose records are still in place (nullptr + error otherwise)
+static ss_context *field_context(const ss_surface *f, int *rc) {
+    *rc = SS_OK;
+    if (!f || !f->fld) { *rc = ss_fail(SS_ERR_INVALID_PARAMETER, "not a level-set field (ss_levelset_field_create_f32)"); return nullptr; }
+    ss_context *c = f->owner;
+    {
+        std::lock_guard<std::mutex> lk(g_ctx_mutex);
+        if (!c || !g_live_contexts.count(c)) { *rc = ss_fail(SS_ERR_INVALID_PARAMETER, "the context of this level-set field was destroyed"); return nullptr; }
+    }
+    if (c->frame != f->frame) {
+        *rc = ss_fail(SS_ERR_INVALID_PARAMETER, "the records of this level-set field are gone: use it before the next reconstruction / interpolator / field on its context");
+        return nullptr;
+    }
+    return c;
+}
+
+// The point groups of one query through the tiers of the fold F: 512-slot slice, 4096-slot slice, selection.
+template <class F>
+static void field_fold(ss_context *c, const SsDev &D, const SsFieldArgs &Q0, uint32_t n_groups, uint64_t *received) {
+    uint64_t launches = 0;
+    const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+        SsFieldArgs Q = Q0;
+        Q.groups = list; Q.n_groups = n; Q.fallback = left;
+        return Q;
+    };
+    run_cascade(c, nullptr, n_groups, {
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            LAUNCH(c, (k_field_fold<F, SS_AN_CAP, SS_FLD_WARPS>), (n + SS_FLD_WARPS - 1) / SS_FLD_WARPS, SS_FLD_WARPS * 32, D, args(list, n, left));
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_field_fold<F, SS_AN_BIG_CAP, 1>), n, 32, D, args(list, n, left)); },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_field_select<F>, n, 32, D, args(list, n, left)); },
+    }, launches, received);
+}
+
+extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint64_t m, float *out) {
+    int rc; ss_context *c = field_context(f, &rc);
+    if (!c) return rc;
+    if (m && (!points || !out)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many points for one call");
+    for (uint64_t &q : f->fld_paths) q = 0;
+    if (!m) return SS_OK;
+    return ss_guard([&]() -> int {
+        CK(cudaSetDevice(c->device));
+        cudaStream_t st = c->stream;
+        const uint32_t m32 = (uint32_t)m;
+        const SsDev &D = f->fld_D;
+        c->fld_pts.ensure((size_t)m32 * 12); c->fld_out.ensure((size_t)m32 * 4); c->fld_chk.ensure(8);
+        c->fld_key_a.ensure((size_t)m32 * 4); c->fld_key_b.ensure((size_t)m32 * 4); c->fld_idx_a.ensure((size_t)m32 * 4); c->fld_idx_b.ensure((size_t)m32 * 4);
+        CK(cudaMemcpyAsync(c->fld_pts.p, points, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        uint32_t chk[2] = { 0xffffffffu, 0u };
+        CK(cudaMemcpyAsync(c->fld_chk.p, chk, 8, cudaMemcpyHostToDevice, st));
+        const uint32_t nsub = f->fld_ready ? f->fld_nsub : 0u;            // no records: every point is 0
+        LAUNCH(c, k_field_keys, nblk(m32, 256), 256, D, c->fld_pts.as<float>(), m32, make_float3(f->grid.mx[0], f->grid.mx[1], f->grid.mx[2]),
+               c->sub_flat.as<uint32_t>(), nsub, c->fld_key_a.as<uint32_t>(), c->fld_idx_a.as<uint32_t>(), c->fld_out.as<float>(), c->fld_chk.as<uint32_t>());
+        CK(cudaMemcpyAsync(chk, c->fld_chk.p, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (chk[0] != 0xffffffffu) {
+            char msg[160];
+            snprintf(msg, sizeof msg, "level-set field: point %u has a non-finite coordinate", chk[0]);
+            return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+        }
+        const uint32_t nin = chk[1];
+        if (nin) {
+            cub_sort(c, c->fld_key_a.as<uint32_t>(), c->fld_key_b.as<uint32_t>(), m32, 32, c->fld_idx_a.as<uint32_t>(), c->fld_idx_b.as<uint32_t>());
+            c->fld_flag.ensure((size_t)nin * 4); c->fld_off.ensure((size_t)nin * 4 + 4); c->fld_starts.ensure((size_t)nin * 4 + 4);
+            LAUNCH(c, k_field_starts, nblk(nin, 256), 256, c->fld_key_b.as<uint32_t>(), nin, c->fld_flag.as<uint32_t>());
+            uint32_t lc[2] = { 0, 0 };
+            scan_compact(c, c->fld_flag.as<uint32_t>(), c->fld_off.as<uint32_t>(), nin, c->fld_starts.as<uint32_t>(), lc);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t n_groups = lc[0] + lc[1];
+            CK(cudaMemcpyAsync(c->fld_starts.as<uint32_t>() + n_groups, &nin, 4, cudaMemcpyHostToDevice, st));
+            SsFieldArgs Q{};
+            Q.A.bins = context_bins(c); Q.A.bins.brick_rng = c->fld_rng.as<int2>();
+            Q.A.grec = c->an_grec.as<float4>(); Q.A.rrec = c->av_rrec.as<float>();
+            Q.pts = c->fld_pts.as<float>(); Q.key = c->fld_key_b.as<uint32_t>(); Q.idx = c->fld_idx_b.as<uint32_t>();
+            Q.starts = c->fld_starts.as<uint32_t>(); Q.out = c->fld_out.as<float>();
+            switch (f->fld_mode) {
+            case SS_FLD_ANISO: field_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG: field_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_CORR: field_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_RAD: field_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_CORR_RAD: field_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+            default: field_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
+            }
+        }
+        CK(cudaMemcpyAsync(out, c->fld_out.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
+        CK(cudaStreamSynchronize(st));
+        return SS_OK;
+    });
+}
+
+extern "C" int ss_levelset_field_threshold_f32(const ss_surface *f, float *threshold) {
+    if (!f || !f->fld || !threshold) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or not a level-set field");
+    *threshold = f->fld_D.thr;
+    return SS_OK;
+}
+
+extern "C" int ss_levelset_field_paths(const ss_surface *f, uint64_t out[3]) {
+    if (!f || !f->fld || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or not a level-set field");
+    for (int t = 0; t < 3; ++t) out[t] = f->fld_paths[t];
+    return SS_OK;
 }
 
 #include "ss_post.cuh"
