@@ -380,6 +380,15 @@ int ss_levelset_field_at_f32(ss_surface *field, const float *points, uint64_t m,
 int ss_levelset_field_threshold_f32(const ss_surface *field, float *threshold);
 int ss_levelset_field_paths(const ss_surface *field, uint64_t out[3]);
 
+/* Gradient of the level-set field at arbitrary points (DESIGN.md section 13.1): the exact derivative, with respect to the point, of
+ * the value ss_levelset_field_at_f32 returns (same candidates, ascending particle index, every operation one f32 rounding).  values
+ * is [m] and bit-identical to ss_levelset_field_at_f32; gradients is [m][3]; both in host or device memory.  Where no candidate
+ * reaches a point both are 0.  The outward normal is -gradient / |gradient| (inside is value > threshold).  Refusals are those of
+ * ss_levelset_field_at_f32; a field created with the Jacobian correction on returns SS_ERR_UNSUPPORTED (the largest eigenvalue of
+ * its Jacobian is not differentiable where eigenvalues coincide, which is the bulk of the liquid).  The tier counters of
+ * ss_levelset_field_paths are set as for ss_levelset_field_at_f32. */
+int ss_levelset_field_gradient_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *gradients);
+
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.
  * The entries marked [bins] query the particles through the splat bins of the reconstruction that produced the surface and

@@ -207,6 +207,7 @@ def _bind(L):
     L.ss_surface_anisotropy_ms.argtypes = [vp]
     L.ss_levelset_field_create_f32.argtypes = [vp, vp, C.c_uint64, C.POINTER(_Params), C.POINTER(vp)]
     L.ss_levelset_field_at_f32.argtypes = [vp, vp, C.c_uint64, vp]
+    L.ss_levelset_field_gradient_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp]
     L.ss_levelset_field_threshold_f32.argtypes = [vp, C.POINTER(C.c_float)]
     L.ss_levelset_field_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.ss_surface_anisotropy_ms.restype = C.c_float
@@ -737,6 +738,7 @@ class Context:
         h = C.c_void_p()
         _check(self._L, self._L.ss_context_create(int(device), C.byref(h)))
         self._h = h
+        self.device = int(device)
         # opt-in: reconstruct_surface / reconstruction_pipeline return their big arrays (vertices, triangles, densities) as views of
         # page-locked buffers owned by this context -- no fresh pages, copies at PCIe speed -- that the NEXT reconstruction on the
         # context overwrites (copy what must outlive it)
@@ -1058,7 +1060,9 @@ class SphInterpolator:
 class LevelSetField:
     """The level set of ``reconstruct_surface`` at arbitrary points, on the GPU (DESIGN.md section 13): the field value and whether a
     point lies inside the liquid, for the standard, anisotropic and averaged-position level sets -- whitewater classification,
-    collision, sphere tracing, or the averaged field ``h - |g - x_bar(g)|`` as an approximate distance field.
+    collision, sphere tracing, or the averaged field ``h - |g - x_bar(g)|`` as an approximate distance field.  ``gradient`` and
+    ``normals`` give the field's exact gradient and outward normal (DESIGN.md section 13.1) for shading, contact normals and Newton
+    projection onto the surface, in every mode except the Jacobian-corrected averaged surface.
 
     The keywords mean what they mean in ``reconstruct_surface``; ``particles`` is an (N, 3) float32 array (float64 raises
     ``TypeError``).  The value at a point is the level set's tile formula with the point in place of the grid point; points no
@@ -1117,30 +1121,64 @@ class LevelSetField:
         _check(L, L.ss_surface_grid(self._s, C.byref(g)))
         self.grid = UniformGrid._from(g)
 
-    def evaluate(self, points):
-        """The field at the points: an (M, 3) float32 numpy array gives an (M,) float32 numpy array; a CUDA float32 torch tensor of
-        shape (M, 3) is read on the device and gives an (M,) CUDA tensor."""
+    def _query(self, points, gradient: bool):
+        """Values (and gradients) at (M, 3) float32 points: numpy in, numpy out; a CUDA torch tensor in, CUDA tensors out."""
         L = self._ctx._L
-        if hasattr(points, "data_ptr") and getattr(points, "is_cuda", False):
+        cuda = hasattr(points, "data_ptr") and getattr(points, "is_cuda", False)
+        if cuda:
             import torch
             if points.dtype != torch.float32:
                 raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
-            if points.ndim != 2 or points.shape[1] != 3:
-                raise ValueError("points must have shape (M, 3)")
-            x = points.contiguous()
-            out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
-            torch.cuda.current_stream(x.device).synchronize()
-            _check(L, L.ss_levelset_field_at_f32(self._s, x.data_ptr() if len(x) else None, len(x), out.data_ptr() if len(x) else None))
-            return out
-        x = np.asarray(points)
-        if x.dtype != np.float32:
-            raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
+            x = points
+        else:
+            x = np.asarray(points)
+            if x.dtype != np.float32:
+                raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
         if x.ndim != 2 or x.shape[1] != 3:
             raise ValueError("points must have shape (M, 3)")
-        x = np.ascontiguousarray(x)
-        out = np.empty(len(x), dtype=np.float32)
-        _check(L, L.ss_levelset_field_at_f32(self._s, x.ctypes.data if len(x) else None, len(x), out.ctypes.data if len(x) else None))
+        if cuda:
+            x = x.contiguous()
+            out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+            grad = torch.empty((x.shape[0], 3), dtype=torch.float32, device=x.device) if gradient else None
+            torch.cuda.current_stream(x.device).synchronize()
+            ptr = lambda a: a.data_ptr() if len(x) else None  # noqa: E731
+        else:
+            x = np.ascontiguousarray(x)
+            out = np.empty(len(x), dtype=np.float32)
+            grad = np.empty((len(x), 3), dtype=np.float32) if gradient else None
+            ptr = lambda a: a.ctypes.data if len(x) else None  # noqa: E731
+        if gradient:
+            _check(L, L.ss_levelset_field_gradient_at_f32(self._s, ptr(x), len(x), ptr(out), ptr(grad)))
+            return out, grad
+        _check(L, L.ss_levelset_field_at_f32(self._s, ptr(x), len(x), ptr(out)))
         return out
+
+    def evaluate(self, points):
+        """The field at the points: an (M, 3) float32 numpy array gives an (M,) float32 numpy array; a CUDA float32 torch tensor of
+        shape (M, 3) is read on the device and gives an (M,) CUDA tensor."""
+        return self._query(points, False)
+
+    def gradient(self, points):
+        """``(values, gradients)`` at the points (DESIGN.md section 13.1): the exact derivative of the field with respect to the point,
+        computed from the same candidates and records as ``evaluate``, whose values it returns bit for bit beside it.  An (M, 3)
+        float32 numpy array gives (M,) and (M, 3) float32 numpy arrays; a CUDA float32 torch tensor gives CUDA tensors.  Points no
+        particle reaches get value and gradient 0.  The checks are those of ``evaluate``.  A field of the Jacobian-corrected averaged
+        surface has no gradient and raises ``SplashsurfError`` (its largest Jacobian eigenvalue is not differentiable where
+        eigenvalues coincide, which is the bulk of the liquid).
+
+        Accuracy in float32: near the surface (the narrow band users shade and collide in) the normal is accurate; for the averaged
+        surfaces the gradient loses accuracy where every candidate sits near the edge of its support (about h outside the
+        surface), and deep inside the liquid it is close to 0 because the averaged field is not a distance field there."""
+        return self._query(points, True)
+
+    def normals(self, points):
+        """Outward unit normals ``-gradient / |gradient|`` at the points (inside is ``value > threshold``), as numpy or CUDA torch
+        like ``gradient``; NaN where the gradient is 0, like ``SphInterpolator.interpolate_normals``."""
+        _, g = self._query(points, True)
+        if isinstance(g, np.ndarray):
+            with np.errstate(invalid="ignore", divide="ignore"):
+                return (-g / np.linalg.norm(g, axis=1, keepdims=True)).astype(np.float32)
+        return -g / g.norm(dim=1, keepdim=True)
 
     def inside(self, points):
         """``evaluate(points) > threshold``."""
@@ -1458,7 +1496,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                             mesh_smoothing_weights_normalization: float = 13.0, output_mesh_smoothing_weights: bool = False,
                             output_raw_normals: bool = False, output_raw_mesh: bool = False, context: Optional[Context] = None,
                             with_debug: bool = False, anisotropy: Optional[Anisotropy] = None,
-                            averaged_surface: Optional[AveragedSurface] = None, particle_radii=None, **post):
+                            averaged_surface: Optional[AveragedSurface] = None, particle_radii=None, levelset_normals: bool = False,
+                            **post):
     """``pysplashsurf.reconstruction_pipeline`` (pysplashsurf/src/pipeline.rs:109-200) on the GPU: surface reconstruction plus
     the post-processing steps of splashsurf/src/reconstruct.rs:1094-1391 that run on the device -- smoothing weights, weighted
     Laplacian smoothing, SPH or area-weighted normals (at the smoothed vertices), normal smoothing and SPH interpolation of
@@ -1471,13 +1510,27 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     the returned mesh is then a MixedTriQuadMesh3d.  ``mesh_aabb_min`` / ``mesh_aabb_max`` (+ ``mesh_aabb_clamp_vertices``) clamp the
     finished mesh (reconstruct.rs:1394-1408) and ``check_mesh_closed`` / ``check_mesh_manifold`` raise SplashsurfError with the
     reference's message when the check fails (:1445-1470); ``check_mesh_orientation`` likewise (:1481-1541).  ``anisotropy``,
-    ``averaged_surface`` and ``particle_radii`` as in ``reconstruct_surface``."""
+    ``averaged_surface`` and ``particle_radii`` as in ``reconstruct_surface``.
+
+    ``levelset_normals=True`` (with ``compute_normals=True``; not part of the reference) takes the normals from the gradient of the
+    level set that was meshed (``LevelSetField.normals``, DESIGN.md section 13.1) instead of the isotropic SPH density gradient or
+    the area-weighted face normals: the normals of the anisotropic or averaged surface the call asked for.  The field is built with
+    this call's keywords on a context of its own (it repeats decomposition, densities and binning), evaluated at the vertices the
+    normals step sees (after Laplacian smoothing) and closed; ``normals_smoothing_iters`` and ``output_raw_normals`` apply to the
+    result.  Refused with ``sph_normals``, without ``compute_normals`` and for the Jacobian-corrected averaged surface."""
     passive = ("mesh_cleanup", "decimate_barnacles", "mesh_cleanup_snap_dist", "keep_vertices", "generate_quads", "quad_max_edge_diag_ratio",
                "quad_max_normal_angle", "quad_max_interior_angle", "mesh_aabb_min", "mesh_aabb_max", "mesh_aabb_clamp_vertices",
                "check_mesh_closed", "check_mesh_manifold", "check_mesh_orientation", "check_mesh_debug")
     enabled = [k for k, v in post.items() if v not in (False, None, 0) and k not in passive]
     if enabled:
         raise NotImplementedError(f"post-processing not provided by the device path: {enabled}")
+    if levelset_normals and not compute_normals:
+        raise ValueError("levelset_normals=True selects how normals are computed: add compute_normals=True")
+    if levelset_normals and sph_normals:
+        raise ValueError("levelset_normals=True and sph_normals=True are exclusive: choose one kind of normals")
+    if levelset_normals and averaged_surface is not None and averaged_surface.correction is not None:
+        raise ValueError("levelset_normals=True is not available for the Jacobian-corrected averaged surface: its level set has no "
+                         "gradient (DESIGN.md section 13.1)")
     mesh_cleanup, decimate_barnacles = bool(post.get("mesh_cleanup", False)), bool(post.get("decimate_barnacles", False))
     keep_vertices, snap_dist = bool(post.get("keep_vertices", False)), post.get("mesh_cleanup_snap_dist", None)
     arr = np.asarray(particles)
@@ -1531,8 +1584,22 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
         if mesh_smoothing_iters:
             verts = np.empty((nv, 3), np.float32)
             _check(L, L.ss_surface_copy_vertices(s, verts.ctypes.data))
-        if compute_normals:                                                     # reconstruct.rs:1282-1342
+        if compute_normals and levelset_normals:                                # DESIGN.md section 13.1
+            # a context of its own: a field on the pipeline's context would make this surface's post-processing state stale
+            fctx = Context(ctx.device)
+            try:
+                field = LevelSetField(arr, particle_radius=particle_radius, rest_density=rest_density, smoothing_length=smoothing_length,
+                                      cube_size=cube_size, iso_surface_threshold=iso_surface_threshold, aabb_min=aabb_min, aabb_max=aabb_max,
+                                      subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim, anisotropy=anisotropy,
+                                      averaged_surface=averaged_surface, particle_radii=radii, context=fctx)
+                nrm = np.ascontiguousarray(field.normals(np.ascontiguousarray(verts, np.float32)))
+                field.close()
+            finally:
+                fctx.close()
+            _check(L, L.ss_surface_set_normals_f32(s, nrm.ctypes.data if nv else None))
+        elif compute_normals:                                                   # reconstruct.rs:1282-1342
             _check(L, L.ss_surface_compute_normals_f32(s, int(bool(sph_normals))))
+        if compute_normals:
             raw = np.empty((nv, 3), np.float32)
             if nv:
                 _check(L, L.ss_surface_copy_normals(s, raw.ctypes.data))

@@ -125,6 +125,9 @@ def main(argv=None):
     r.add_argument("--averaged-correction-high", type=float, default=None)           # t_high: from this eigenvalue on the radius is 0 (default 3.5)
     # per-particle radii of the averaged-position surface (DESIGN.md section 12.2): the scalar point attribute NAME of each input frame
     r.add_argument("--averaged-radius-attribute", default=None, metavar="NAME")
+    # normals from the gradient of the level set that was meshed (splashsurf_b200.LevelSetField.normals, DESIGN.md section 13.1) --
+    # not part of the reference CLI; with --normals=on
+    r.add_argument("--levelset-normals", choices=["on", "off"], default="off")
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -283,6 +286,15 @@ def reconstruct(a) -> int:
     avg = AveragedSurface(1.0 if a.averaged_radius_factor is None else a.averaged_radius_factor, corr) if on(a.averaged_surface) else None
     if a.averaged_radius_attribute is not None and not on(a.averaged_surface):
         raise ValueError("--averaged-radius-attribute applies to the averaged-position surface: add --averaged-surface=on")
+    if on(a.levelset_normals):
+        if on(a.partition):
+            raise ValueError("--levelset-normals=on is not available with --partition=on: the level-set field runs on one GPU per frame")
+        if not on(a.normals):
+            raise ValueError("--levelset-normals=on selects how normals are computed: add --normals=on")
+        if on(a.sph_normals):
+            raise ValueError("--levelset-normals=on and --sph-normals=on are exclusive: choose one kind of normals")
+        if on(a.averaged_correction):
+            raise ValueError("--levelset-normals=on is not available with --averaged-correction=on: the corrected level set has no gradient")
     paths = collect_paths(a)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)
@@ -335,7 +347,7 @@ def reconstruct(a) -> int:
                     quad_max_normal_angle=a.quad_max_normal_angle, quad_max_interior_angle=a.quad_max_interior_angle, mesh_aabb_min=mmin,
                     mesh_aabb_max=mmax, mesh_aabb_clamp_vertices=on(a.mesh_aabb_clamp_verts), check_mesh_closed=closed, check_mesh_manifold=manifold,
                     check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso,
-                    averaged_surface=avg, particle_radii=radii, **base)
+                    averaged_surface=avg, particle_radii=radii, levelset_normals=on(a.levelset_normals), **base)
                 raw = rec.mesh
             else:
                 raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, averaged_surface=avg, particle_radii=radii, **base).mesh

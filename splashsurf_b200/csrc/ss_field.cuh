@@ -16,7 +16,10 @@
 //   k_field_select    per batch of 32 points the selection walk of k_fold_select (ss_select_next)
 // A group's candidate bins cover the cells [8b - R, 8b + 8 + R) along each axis (ss_pipeline.cu: upload_field_brick_ranges): a point lies
 // anywhere in the closed cell box [8b, 8b + 8]^3 of its brick, one cell further than the brick's grid points reach.
+// ss_levelset_field_gradient_at_f32 runs the same sequence with the gradient folds below (SsSphGradFold, SsAnisoGradFold,
+// SsAvgGradFold, SsAvgRadGradFold), which k_field_fold and k_field_select recognise at compile time and also write the gradient for.
 #pragma once
+#include <type_traits>
 
 #define SS_FLD_WARPS 4                  // groups per CTA of the default slice
 
@@ -39,6 +42,134 @@ struct SsSphFold {
     static __device__ __forceinline__ float value(const SsDev &, const Acc &a) { return a.phi; }
 };
 
+// ------------------------------------------------------------------ gradients (DESIGN.md §13.1) ----
+// The gradient of the value at the query point p, d_j = x_j - p.  A gradient fold wraps its value fold: its Acc holds the value
+// fold's Acc, its add calls the value fold's add first, and its value is the value fold's, so the value returned beside the gradient
+// is bit-identical to the one of ss_levelset_field_at_f32.  It adds
+//   void     F::gradient(P, acc, g)     the gradient (0 where no candidate reaches p)
+// which k_field_fold / k_field_select write to SsFieldArgs::grad.  The corrected modes have no gradient fold (DESIGN.md §13.1).
+template <class F, class = void> struct SsFoldHasGradient : std::false_type {};
+template <class F> struct SsFoldHasGradient<F, std::void_t<decltype(&F::gradient)>> : std::true_type {};
+
+// W'(r) of ss_kernel_scalar from the same constants: q = 2r / h, W' = sigma f'(q) (2 / h) with f' = c_inner q (1.5 q - 2) below 1,
+// -3 c_outer (2 - q)^2 below 2, 0 beyond (continuous at q = 1 and 2, 0 at q = 0)
+__device__ __forceinline__ float ss_kernel_scalar_dr(const SsDev &P, float r) {
+    const float q = __fdiv_rn(__fadd_rn(r, r), P.h);
+    float f;
+    if (q < 1.0f) f = __fmul_rn(P.s_c_inner, __fmul_rn(q, __fsub_rn(__fmul_rn(1.5f, q), 2.0f)));
+    else if (q < 2.0f) { const float x = __fsub_rn(2.0f, q); f = __fmul_rn(__fmul_rn(__fmul_rn(-3.0f, P.s_c_outer), x), x); }
+    else f = 0.0f;
+    return __fmul_rn(__fmul_rn(P.s_sigma, f), __fdiv_rn(2.0f, P.h));
+}
+
+// grad phi = -sum_j V_j W'(r) d_j / r over SsSphFold's candidates (d2 < 1.01 h^2); d2 == 0 is skipped (W'(0) = 0)
+struct SsSphGradFold {
+    using Cand = SsSphFold::Cand;
+    struct Acc { SsSphFold::Acc v; float gx, gy, gz; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsSphFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsSphFold::zero(), 0.0f, 0.0f, 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsSphFold::add(P, c, gx, gy, gz, a.v);
+        const float dx = __fsub_rn(c.r.x, gx), dy = __fsub_rn(c.r.y, gy), dz = __fsub_rn(c.r.z, gz);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+        if (!(d2 < P.h2m) || d2 == 0.0f) return;
+        const float r = __fsqrt_rn(d2);
+        const float t = __fdiv_rn(__fmul_rn(c.r.w, ss_kernel_scalar_dr(P, r)), r);
+        a.gx = __fsub_rn(a.gx, __fmul_rn(t, dx)); a.gy = __fsub_rn(a.gy, __fmul_rn(t, dy)); a.gz = __fsub_rn(a.gz, __fmul_rn(t, dz));
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsSphFold::value(P, a.v); }
+    static __device__ __forceinline__ void gradient(const SsDev &, const Acc &a, float (&g)[3]) { g[0] = a.gx; g[1] = a.gy; g[2] = a.gz; }
+};
+
+// grad phi = -sum_j (V_j det G_j) W'(|u_j|) (G_j u_j) / |u_j|, u_j = G_j d_j as in ss_aniso_term (G symmetric); |u| == 0 is skipped
+struct SsAnisoGradFold {
+    using Cand = SsAnisoFold::Cand;
+    struct Acc { SsAnisoFold::Acc v; float gx, gy, gz; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAnisoFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAnisoFold::zero(), 0.0f, 0.0f, 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAnisoFold::add(P, c, gx, gy, gz, a.v);
+        const float4 g0 = c.g0, g1 = c.g1;
+        const float dx = __fsub_rn(c.r.x, gx), dy = __fsub_rn(c.r.y, gy), dz = __fsub_rn(c.r.z, gz);
+        const float u0 = __fadd_rn(__fadd_rn(__fmul_rn(g0.x, dx), __fmul_rn(g0.y, dy)), __fmul_rn(g0.z, dz));
+        const float u1 = __fadd_rn(__fadd_rn(__fmul_rn(g0.y, dx), __fmul_rn(g0.w, dy)), __fmul_rn(g1.x, dz));
+        const float u2 = __fadd_rn(__fadd_rn(__fmul_rn(g0.z, dx), __fmul_rn(g1.x, dy)), __fmul_rn(g1.y, dz));
+        const float uu = __fadd_rn(__fadd_rn(__fmul_rn(u0, u0), __fmul_rn(u1, u1)), __fmul_rn(u2, u2));
+        if (!(uu < P.h2) || uu == 0.0f) return;
+        const float r = __fsqrt_rn(uu);
+        const float t = __fdiv_rn(__fmul_rn(c.r.w, ss_kernel_scalar_dr(P, r)), r);
+        const float v0 = __fadd_rn(__fadd_rn(__fmul_rn(g0.x, u0), __fmul_rn(g0.y, u1)), __fmul_rn(g0.z, u2));
+        const float v1 = __fadd_rn(__fadd_rn(__fmul_rn(g0.y, u0), __fmul_rn(g0.w, u1)), __fmul_rn(g1.x, u2));
+        const float v2 = __fadd_rn(__fadd_rn(__fmul_rn(g0.z, u0), __fmul_rn(g1.x, u1)), __fmul_rn(g1.y, u2));
+        a.gx = __fsub_rn(a.gx, __fmul_rn(t, v0)); a.gy = __fsub_rn(a.gy, __fmul_rn(t, v1)); a.gz = __fsub_rn(a.gz, __fmul_rn(t, v2));
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAnisoFold::value(P, a.v); }
+    static __device__ __forceinline__ void gradient(const SsDev &, const Acc &a, float (&g)[3]) { g[0] = a.gx; g[1] = a.gy; g[2] = a.gz; }
+};
+
+// f = h - |m|, m = X / S: grad f = (m - (6 / h^2) (M m - |m|^2 T) / S) / |m| = (I - J)^T m / |m| with §12.1's sums, which
+// SsAvgCorrFold::add accumulates (S, X, Y, Z first, through SsAvgFold::add); 0 where !(S > 0) or |m| == 0.  g gets grad f; the
+// return value is |m| (0 when g is the zero vector).
+struct SsAvgGradFold {
+    using Cand = SsAvgFold::Cand;
+    using Acc = SsAvgCorrFold::Acc;                 // .a: SsAvgFold::Acc
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return SsAvgCorrFold::zero(); }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgCorrFold::add(P, c, gx, gy, gz, a);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAvgFold::value(P, a.a); }
+    static __device__ __forceinline__ float grad_f(const SsDev &P, const Acc &a, float (&g)[3]) {
+        g[0] = 0.0f; g[1] = 0.0f; g[2] = 0.0f;
+        const float s = a.a.s;
+        if (!(s > 0.0f)) return 0.0f;
+        const float m[3] = { __fdiv_rn(a.a.x, s), __fdiv_rn(a.a.y, s), __fdiv_rn(a.a.z, s) };
+        const float m2 = __fadd_rn(__fadd_rn(__fmul_rn(m[0], m[0]), __fmul_rn(m[1], m[1])), __fmul_rn(m[2], m[2]));
+        const float nm = __fsqrt_rn(m2);
+        if (nm == 0.0f) return 0.0f;
+        const float k = __fdiv_rn(6.0f, P.h2);
+        const float M[3][3] = { { a.mxx, a.mxy, a.mxz }, { a.mxy, a.myy, a.myz }, { a.mxz, a.myz, a.mzz } };
+        const float T[3] = { a.tx, a.ty, a.tz };
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            const float mm = __fadd_rn(__fadd_rn(__fmul_rn(M[i][0], m[0]), __fmul_rn(M[i][1], m[1])), __fmul_rn(M[i][2], m[2]));
+            const float jm = __fdiv_rn(__fmul_rn(k, __fsub_rn(mm, __fmul_rn(m2, T[i]))), s);
+            g[i] = __fdiv_rn(__fsub_rn(m[i], jm), nm);
+        }
+        return nm;
+    }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) { grad_f(P, a, g); }
+};
+
+// With radii: v = (h - |m|) + b, b = Q / S; grad v = grad f + (6 / h^2) (U - b T) / S with U_b = sum_j u_j^2 delta_j d_jb.  Q is
+// SsAvgRadFold::add_q's sum; the value is SsAvgRadFold::value of (S, X, Y, Z, Q).
+struct SsAvgRadGradFold {
+    using Cand = SsAvgRadFold::Cand;
+    struct Acc { SsAvgGradFold::Acc a; float q, ux, uy, uz; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgRadFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgGradFold::zero(), 0.0f, 0.0f, 0.0f, 0.0f }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgGradFold::add(P, c.c, gx, gy, gz, a.a);
+        SsAvgRadFold::add_q(P, c, gx, gy, gz, a.q);
+        const float dx = __fsub_rn(c.c.r.x, gx), dy = __fsub_rn(c.c.r.y, gy), dz = __fsub_rn(c.c.r.z, gz);
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+        if (!(d2 < P.h2)) return;
+        const float u = __fsub_rn(1.0f, __fdiv_rn(d2, P.h2));
+        const float e = __fmul_rn(__fmul_rn(u, u), c.delta);
+        a.ux = __fadd_rn(a.ux, __fmul_rn(e, dx)); a.uy = __fadd_rn(a.uy, __fmul_rn(e, dy)); a.uz = __fadd_rn(a.uz, __fmul_rn(e, dz));
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAvgRadFold::value(P, SsAvgRadFold::Acc{ a.a.a, a.q }); }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) {
+        SsAvgGradFold::grad_f(P, a.a, g);
+        const float s = a.a.a.s;
+        if (!(s > 0.0f)) return;
+        const float k = __fdiv_rn(6.0f, P.h2), b = __fdiv_rn(a.q, s);
+        const float U[3] = { a.ux, a.uy, a.uz }, T[3] = { a.a.tx, a.a.ty, a.a.tz };
+#pragma unroll
+        for (int i = 0; i < 3; ++i) g[i] = __fadd_rn(g[i], __fdiv_rn(__fmul_rn(k, __fsub_rn(U[i], __fmul_rn(b, T[i]))), s));
+    }
+};
+
 struct SsFieldArgs {
     SsAnArgs A;                        // the mode's records (A.bins.brick_rng: the field's candidate ranges); bricks / tiles unused
     const float *pts;                  // [m][3] query points
@@ -49,7 +180,19 @@ struct SsFieldArgs {
     uint32_t n_groups;
     float *out;                        // [m] pre-zeroed
     uint32_t *fallback;                // groups left to the next tier: [0] = count, [1..] = group indices
+    float *grad;                       // [m][3] pre-zeroed, written by gradient folds only
 };
+
+// the value of a point, and its gradient when the fold has one
+template <class F>
+__device__ __forceinline__ void ss_field_store(const SsDev &P, const SsFieldArgs &Q, uint32_t dst, const typename F::Acc &acc) {
+    Q.out[dst] = F::value(P, acc);
+    if constexpr (SsFoldHasGradient<F>::value) {
+        float g[3];
+        F::gradient(P, acc, g);
+        Q.grad[3 * (size_t)dst] = g[0]; Q.grad[3 * (size_t)dst + 1] = g[1]; Q.grad[3 * (size_t)dst + 2] = g[2];
+    }
+}
 
 // Points outside [gmin, gmax] along an axis, or in a subdomain without members, get 0 and key 0xffffffff (sorted last); chk[0]:
 // lowest index with a non-finite coordinate (preset 0xffffffff), chk[1]: points with a group (preset 0).
@@ -160,7 +303,7 @@ k_field_fold(SsDev P, SsFieldArgs Q) {
         __syncwarp();
         typename F::Acc acc = F::zero();
         for (int n = 0; n < nlist; ++n) F::add(P, F::load(Q.A, (uint32_t)s_key[wib][s_list[wib][n]]), p.x, p.y, p.z, acc);
-        if (p.on) Q.out[p.dst] = F::value(P, acc);
+        if (p.on) ss_field_store<F>(P, Q, p.dst, acc);
         __syncwarp();                                        // the list is rebuilt for the next batch
     }
 }
@@ -184,6 +327,6 @@ k_field_select(SsDev P, SsFieldArgs Q) {
             last = best; first = false;
             F::add(P, F::load(Q.A, (uint32_t)best), p.x, p.y, p.z, acc);
         }
-        if (p.on) Q.out[p.dst] = F::value(P, acc);
+        if (p.on) ss_field_store<F>(P, Q, p.dst, acc);
     }
 }

@@ -148,7 +148,7 @@ struct ss_context {
     DevBuf av_radii, av_delta, av_rrec, av_chk;      // per-particle radii: the caller's copy, delta_j (filtered), per membership, check
     // level-set field queries (ss_field.cuh): points, group keys and caller indices (sorted and not), group starts, values, checks,
     // and the candidate bin ranges of a group
-    DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng;
+    DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng, fld_grad;
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
@@ -2118,11 +2118,15 @@ static void field_fold(ss_context *c, const SsDev &D, const SsFieldArgs &Q0, uin
     }, launches, received);
 }
 
-extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint64_t m, float *out) {
+// One query of ss_levelset_field_at_f32 or (gradient) ss_levelset_field_gradient_at_f32: keys, sort, group starts, then the cascade
+// of the mode's value fold or gradient fold.
+static int field_query(ss_surface *f, const float *points, uint64_t m, float *out, bool gradient, float *grads) {
     int rc; ss_context *c = field_context(f, &rc);
     if (!c) return rc;
-    if (m && (!points || !out)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    if (m && (!points || !out || (gradient && !grads))) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many points for one call");
+    if (gradient && (f->fld_mode == SS_FLD_AVG_CORR || f->fld_mode == SS_FLD_AVG_CORR_RAD))
+        return ss_fail(SS_ERR_UNSUPPORTED, "level-set field: the Jacobian-corrected averaged surface has no gradient (DESIGN.md 13.1)");
     for (uint64_t &q : f->fld_paths) q = 0;
     if (!m) return SS_OK;
     return ss_guard([&]() -> int {
@@ -2132,6 +2136,10 @@ extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint
         const SsDev &D = f->fld_D;
         c->fld_pts.ensure((size_t)m32 * 12); c->fld_out.ensure((size_t)m32 * 4); c->fld_chk.ensure(8);
         c->fld_key_a.ensure((size_t)m32 * 4); c->fld_key_b.ensure((size_t)m32 * 4); c->fld_idx_a.ensure((size_t)m32 * 4); c->fld_idx_b.ensure((size_t)m32 * 4);
+        if (gradient) {
+            c->fld_grad.ensure((size_t)m32 * 12);
+            CK(cudaMemsetAsync(c->fld_grad.p, 0, (size_t)m32 * 12, st));       // points without candidates: gradient 0
+        }
         CK(cudaMemcpyAsync(c->fld_pts.p, points, (size_t)m32 * 12, cudaMemcpyDefault, st));
         uint32_t chk[2] = { 0xffffffffu, 0u };
         CK(cudaMemcpyAsync(c->fld_chk.p, chk, 8, cudaMemcpyHostToDevice, st));
@@ -2160,19 +2168,38 @@ extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint
             Q.A.grec = c->an_grec.as<float4>(); Q.A.rrec = c->av_rrec.as<float>();
             Q.pts = c->fld_pts.as<float>(); Q.key = c->fld_key_b.as<uint32_t>(); Q.idx = c->fld_idx_b.as<uint32_t>();
             Q.starts = c->fld_starts.as<uint32_t>(); Q.out = c->fld_out.as<float>();
-            switch (f->fld_mode) {
-            case SS_FLD_ANISO: field_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
-            case SS_FLD_AVG: field_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
-            case SS_FLD_AVG_CORR: field_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
-            case SS_FLD_AVG_RAD: field_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
-            case SS_FLD_AVG_CORR_RAD: field_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
-            default: field_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
+            if (gradient) {
+                Q.grad = c->fld_grad.as<float>();
+                switch (f->fld_mode) {
+                case SS_FLD_ANISO: field_fold<SsAnisoGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG: field_fold<SsAvgGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG_RAD: field_fold<SsAvgRadGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+                default: field_fold<SsSphGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+                }
+            } else {
+                switch (f->fld_mode) {
+                case SS_FLD_ANISO: field_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG: field_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG_CORR: field_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG_RAD: field_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+                case SS_FLD_AVG_CORR_RAD: field_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+                default: field_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
+                }
             }
         }
         CK(cudaMemcpyAsync(out, c->fld_out.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
+        if (gradient) CK(cudaMemcpyAsync(grads, c->fld_grad.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
         return SS_OK;
     });
+}
+
+extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint64_t m, float *out) {
+    return field_query(f, points, m, out, false, nullptr);
+}
+
+extern "C" int ss_levelset_field_gradient_at_f32(ss_surface *f, const float *points, uint64_t m, float *values, float *gradients) {
+    return field_query(f, points, m, values, true, gradients);
 }
 
 extern "C" int ss_levelset_field_threshold_f32(const ss_surface *f, float *threshold) {

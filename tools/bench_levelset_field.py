@@ -9,8 +9,12 @@ Each query is timed over `--steps` calls after `--warmup` (CUDA events around th
 them, the same mode's level-set stage of reconstruct_surface and the grid points it evaluated, for ns per grid point.  The card name,
 power limit and SM clock are read at the start and at the end.  Prints one JSON line; writes nothing.
 
+With `--gradient` the corrected modes are left out (they have no gradient, DESIGN.md §13.1) and every query is also timed as a
+gradient query (LevelSetField.gradient, §13.1) on the same points, the two alternating call by call.
+
     python tools/bench_levelset_field.py                         # cfg-4: the 50 M-particle dam break
     python tools/bench_levelset_field.py --particles 1000000 --points 1000000
+    python tools/bench_levelset_field.py --gradient              # value and gradient queries side by side
 """
 import argparse
 import json
@@ -39,6 +43,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--modes", default="standard,anisotropic,averaged,averaged_corrected,averaged_radii,averaged_corrected_radii")
+    ap.add_argument("--gradient", action="store_true", help="also time the gradient query (modes with a gradient only)")
     a = ap.parse_args()
     import numpy as np
     import torch
@@ -58,6 +63,8 @@ def main():
            "steps": a.steps, "warmup": a.warmup, "runs": []}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for mode in a.modes.split(","):
+        if a.gradient and "corrected" in mode:
+            continue
         mk = modes[mode]
         # the same mode's reconstruction: level-set stage time, grid points it evaluated, and the mesh for the near-mesh points
         # (on a context of its own, closed before the field is built: the reconstruction keeps tile buffers of a third of the memory)
@@ -93,21 +100,34 @@ def main():
             torch.cuda.synchronize()
             for _ in range(a.warmup):
                 v = f.evaluate(dev)
-            ms = []
+                if a.gradient:
+                    f.gradient(dev)
+            ms, gms = [], []
             for _ in range(a.steps):
                 ev0.record()
                 v = f.evaluate(dev)
                 ev1.record()
                 torch.cuda.synchronize()
                 ms.append(ev0.elapsed_time(ev1))
+                if a.gradient:
+                    ev0.record()
+                    gv, g = f.gradient(dev)
+                    ev1.record()
+                    torch.cuda.synchronize()
+                    gms.append(ev0.elapsed_time(ev1))
             best = min(ms)
-            run["queries"][name] = {"points": len(pts), "ms": [round(t, 3) for t in ms], "ns_per_point": best * 1e6 / max(len(pts), 1),
-                                    "inside_fraction": float((v > f.threshold).sum()) / max(len(pts), 1),
-                                    "paths": f.paths}
+            q = {"points": len(pts), "ms": [round(t, 3) for t in ms], "ns_per_point": best * 1e6 / max(len(pts), 1),
+                 "inside_fraction": float((v > f.threshold).sum()) / max(len(pts), 1), "paths": f.paths}
+            if a.gradient:
+                q.update(gradient_ms=[round(t, 3) for t in gms], gradient_ns_per_point=min(gms) * 1e6 / max(len(pts), 1),
+                         values_equal=bool(torch.equal(gv, v)), zero_gradient_fraction=float((g == 0).all(1).float().mean()))
+                del gv, g
+            run["queries"][name] = q
             del dev, v
         f.close()
         out["runs"].append(run)
-        sys.stderr.write(f"{mode}: create {create_ms:.1f} ms, " + ", ".join(f"{k} {q['ns_per_point']:.2f} ns/pt" for k, q in run["queries"].items()) + "\n")
+        sys.stderr.write(f"{mode}: create {create_ms:.1f} ms, " + ", ".join(f"{k} {q['ns_per_point']:.2f} ns/pt" + (
+            f" (gradient {q['gradient_ns_per_point']:.2f})" if a.gradient else "") for k, q in run["queries"].items()) + "\n")
     out["card_after"] = card()
     ctx.close()
     print(json.dumps(out))
