@@ -389,6 +389,35 @@ int ss_levelset_field_paths(const ss_surface *field, uint64_t out[3]);
  * ss_levelset_field_paths are set as for ss_levelset_field_at_f32. */
 int ss_levelset_field_gradient_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *gradients);
 
+/* Narrow-band signed distance grid of a mesh on the field's lattice (DESIGN.md section 14).  The lattice is the field's grid
+ * (ss_surface_grid): points min + index * cell_size, index in [0, n] per axis, in bricks of 8 x 8 x 8 points (ceil((n + 1) / 8) per
+ * axis).  B = band * cell_size (band in [1, 8]).  d(p) is the f32 minimum over all triangles of the point-triangle distance, every
+ * operation one rounding.  A brick is listed iff one of its points inside the volume has d < B; listed bricks come in ascending
+ * (bx, by, bz) order.  Their values are [brick][i][j][k] (k fastest, an OpenVDB leaf's order): -min(d, B) where the field is inside
+ * (value > threshold), +min(d, B) elsewhere, +B at points past the volume.  brick_inside[bx][by][bz] is the field's inside test at
+ * the first point 8 b of every brick: the sign of every point of an unlisted brick when the mesh is the raw mesh of the field's
+ * reconstruction (section 14 states the conditions).  vertices [nv][3] and triangles [nt][3] may be in host or device memory.
+ * SS_ERR_INVALID_PARAMETER: NULL pointers, band outside [1, 8], a non-finite vertex, a triangle index >= nv (both naming the
+ * first), a stale field; SS_ERR_INDEX_TOO_SMALL: nv >= 2^32, 2^31 or more triangles or grid bricks, or one brick column with 2^31
+ * or more pairs.  The
+ * result owns its device memory and stays valid after later calls on the field's context; the field's query runs on the
+ * listed points, so ss_levelset_field_paths reports it.
+ * ss_sdf_copy_f32: brick_coords [B][3], values [B][8][8][8], brick_inside [nbx][nby][nbz] (1 = inside), host or device memory, each
+ * may be NULL.  ss_sdf_paths: candidate bricks through the shared-memory slice (out[0]) and the global-memory walk (out[1]). */
+typedef struct ss_sdf ss_sdf;
+int ss_levelset_field_sdf_f32(ss_surface *field, const float *vertices, uint64_t nv, const uint32_t *triangles, uint64_t nt,
+                              uint32_t band, ss_sdf **out);
+uint64_t ss_sdf_num_bricks(const ss_sdf *sdf);
+int ss_sdf_info(const ss_sdf *sdf, int64_t bricks_per_dim[3], float *background);
+int ss_sdf_copy_f32(const ss_sdf *sdf, int32_t *brick_coords, float *values, uint8_t *brick_inside);
+int ss_sdf_paths(const ss_sdf *sdf, uint64_t out[2]);
+/* The call runs in passes over slabs of whole brick columns (ascending bx), each holding at most `pairs` (brick, triangle) pairs
+ * (0: the default, 2^27) and 2^19 bricks, so its device memory stays bounded for any mesh; the result does not depend on the passes.
+ * ss_sdf_passes: out[0] passes that had candidates, out[1] (brick, triangle) pairs over all passes. */
+void ss_sdf_set_pass_pairs(uint64_t pairs);
+int ss_sdf_passes(const ss_sdf *sdf, uint64_t out[2]);
+void ss_sdf_free(ss_sdf *sdf);
+
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.
  * The entries marked [bins] query the particles through the splat bins of the reconstruction that produced the surface and

@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "LevelSetField", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "LevelSetField", "SignedDistanceGrid", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -210,6 +210,17 @@ def _bind(L):
     L.ss_levelset_field_gradient_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp]
     L.ss_levelset_field_threshold_f32.argtypes = [vp, C.POINTER(C.c_float)]
     L.ss_levelset_field_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.ss_levelset_field_sdf_f32.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint32, C.POINTER(vp)]
+    L.ss_sdf_num_bricks.argtypes = [vp]
+    L.ss_sdf_num_bricks.restype = C.c_uint64
+    L.ss_sdf_info.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_float)]
+    L.ss_sdf_copy_f32.argtypes = [vp, vp, vp, vp]
+    L.ss_sdf_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.ss_sdf_passes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.ss_sdf_set_pass_pairs.argtypes = [C.c_uint64]
+    L.ss_sdf_set_pass_pairs.restype = None
+    L.ss_sdf_free.argtypes = [vp]
+    L.ss_sdf_free.restype = None
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
         raise ImportError("libsplashsurf_b200.so ABI version mismatch")
@@ -1184,6 +1195,56 @@ class LevelSetField:
         """``evaluate(points) > threshold``."""
         return self.evaluate(points) > self.threshold
 
+    def signed_distance(self, mesh, *, band: int = 3) -> "SignedDistanceGrid":
+        """Narrow-band signed distance grid of ``mesh`` on this field's lattice (DESIGN.md section 14): per brick of 8^3 grid points
+        within ``band`` cells of the mesh, the f32 distance to the nearest triangle clamped to the background ``band * cell_size``,
+        negative where the field is inside; and for every brick of the grid whether its first point is inside.
+
+        ``mesh`` is a ``TriMesh3d`` (numpy arrays in, numpy arrays out) or a ``(vertices, triangles)`` pair: numpy arrays give numpy
+        arrays, CUDA torch tensors (float32 vertices, int32 or int64 triangles) give CUDA tensors.  Float64 vertices raise
+        ``TypeError``.  For the raw mesh of ``reconstruct_surface`` with this field's keywords (``simd=False`` for the standard
+        level set) the result is a complete level set: an unlisted brick has the sign of its ``brick_inside`` at every point.  Any
+        other mesh gives the distance to that mesh with the field's sign."""
+        L = self._ctx._L
+        if isinstance(mesh, TriMesh3d):
+            verts, tris = mesh.vertices, mesh.triangles
+        else:
+            verts, tris = mesh
+        cuda = hasattr(verts, "data_ptr") and getattr(verts, "is_cuda", False)
+        if cuda:
+            import torch
+            if verts.dtype != torch.float32:
+                raise TypeError("unsupported scalar type: the signed distance takes float32 vertices only")
+            if tris.dtype not in (torch.int32, torch.int64) or not getattr(tris, "is_cuda", False):
+                raise TypeError("triangles must be a CUDA int32 or int64 tensor beside CUDA vertices")
+            if verts.ndim != 2 or verts.shape[1] != 3 or tris.ndim != 2 or tris.shape[1] != 3:
+                raise ValueError("vertices and triangles must have shape (V, 3) and (T, 3)")
+            if len(tris) and (bool((tris < 0).any()) or (tris.dtype == torch.int64 and bool((tris >= 2 ** 32).any()))):
+                raise ValueError("triangle indices must lie in [0, 2^32)")
+            v = verts.contiguous()
+            t = tris.to(torch.int32).contiguous() if tris.dtype == torch.int64 else tris.contiguous()   # the low 32 bits: uint32
+            torch.cuda.current_stream(v.device).synchronize()
+            vp, tp = (v.data_ptr() if len(v) else None), (t.data_ptr() if len(t) else None)
+        else:
+            v = np.asarray(verts)
+            if v.dtype != np.float32:
+                raise TypeError("unsupported scalar type: the signed distance takes float32 vertices only")
+            t = np.asarray(tris)
+            if v.ndim != 2 or v.shape[1] != 3 or t.ndim != 2 or t.shape[1] != 3:
+                raise ValueError("vertices and triangles must have shape (V, 3) and (T, 3)")
+            if t.dtype.kind not in "iu":
+                raise TypeError("triangles must be an integer array")
+            if len(t) and (int(t.min()) < 0 or int(t.max()) >= 2 ** 32):
+                raise ValueError("triangle indices must lie in [0, 2^32)")
+            v, t = np.ascontiguousarray(v), np.ascontiguousarray(t, dtype=np.uint32)
+            vp, tp = (v.ctypes.data if len(v) else None), (t.ctypes.data if len(t) else None)
+        h = C.c_void_p()
+        _check(L, L.ss_levelset_field_sdf_f32(self._s, vp, len(v), tp, len(t), int(band), C.byref(h)))
+        try:
+            return SignedDistanceGrid._from(L, h, self.grid, int(band), v.device if cuda else None)
+        finally:
+            L.ss_sdf_free(h)
+
     @property
     def paths(self) -> dict:
         """The point groups of the last ``evaluate`` per tier of the cascade: 512-slot slice, 4096-slot slice, selection walk."""
@@ -1203,6 +1264,59 @@ class LevelSetField:
             self.close()
         except Exception:
             pass
+
+
+class SignedDistanceGrid:
+    """Narrow-band signed distance grid of ``LevelSetField.signed_distance`` (DESIGN.md section 14).
+
+    ``grid`` is the field's grid; the lattice points are ``grid.aabb.min + index * grid.cell_size``, ``index`` in
+    ``[0, npoints_per_dim)``, in bricks of 8^3 points.  ``background = band * cell_size``.  ``brick_coords`` (B, 3) int32 are the listed
+    bricks in ascending order, ``values`` (B, 8, 8, 8) float32 their signed distances (``[brick][i][j][k]``, k fastest: an OpenVDB
+    leaf's order; negative inside, clamped to +-background, +background past the grid), ``brick_inside`` (nbx, nby, nbz) bool the
+    field's inside test at the first point of every brick.  ``paths``: candidate bricks through the shared-memory slice and the
+    global-memory walk; ``passes``: the slabs of brick columns the call ran in and their (brick, triangle) pairs."""
+
+    @staticmethod
+    def _from(L, h, grid, band, device) -> "SignedDistanceGrid":
+        self = SignedDistanceGrid()
+        self.grid, self.band = grid, band
+        nb, bg = (C.c_int64 * 3)(), C.c_float()
+        _check(L, L.ss_sdf_info(h, nb, C.byref(bg)))
+        self.background = float(bg.value)
+        nbs = tuple(int(x) for x in nb)
+        nl = int(L.ss_sdf_num_bricks(h))
+        if device is not None:
+            import torch
+            self.brick_coords = torch.empty((nl, 3), dtype=torch.int32, device=device)
+            self.values = torch.empty((nl, 8, 8, 8), dtype=torch.float32, device=device)
+            inside = torch.empty(nbs, dtype=torch.uint8, device=device)
+            ptr = lambda a: a.data_ptr() if a.numel() else None  # noqa: E731
+        else:
+            self.brick_coords = np.empty((nl, 3), np.int32)
+            self.values = np.empty((nl, 8, 8, 8), np.float32)
+            inside = np.empty(nbs, np.uint8)
+            ptr = lambda a: a.ctypes.data if a.size else None  # noqa: E731
+        _check(L, L.ss_sdf_copy_f32(h, ptr(self.brick_coords), ptr(self.values), ptr(inside)))
+        self.brick_inside = inside.bool() if device is not None else inside.astype(bool)
+        p = (C.c_uint64 * 2)()
+        _check(L, L.ss_sdf_paths(h, p))
+        self.paths = {"shared": int(p[0]), "global": int(p[1])}
+        _check(L, L.ss_sdf_passes(h, p))
+        self.passes = {"passes": int(p[0]), "pairs": int(p[1])}
+        return self
+
+    def to_dense(self) -> np.ndarray:
+        """The grid's (n + 1)^3 points as a float32 numpy array: listed bricks from ``values``, every other point -background inside
+        and +background outside by its brick's ``brick_inside``."""
+        host = lambda a: a.cpu().numpy() if hasattr(a, "cpu") else np.asarray(a)  # noqa: E731
+        inside, coords, values = host(self.brick_inside).astype(bool), host(self.brick_coords), host(self.values)
+        b = np.float32(self.background)
+        nb = inside.shape
+        bricks = np.where(inside, -b, b).astype(np.float32)[:, :, :, None, None, None] * np.ones((8, 8, 8), np.float32)
+        bricks[coords[:, 0], coords[:, 1], coords[:, 2]] = values
+        dense = bricks.transpose(0, 3, 1, 4, 2, 5).reshape(nb[0] * 8, nb[1] * 8, nb[2] * 8)
+        n = self.grid.npoints_per_dim
+        return np.ascontiguousarray(dense[:n[0], :n[1], :n[2]])
 
 
 _DEFAULT_CTX: dict = {}

@@ -128,6 +128,10 @@ def main(argv=None):
     # normals from the gradient of the level set that was meshed (splashsurf_b200.LevelSetField.normals, DESIGN.md section 13.1) --
     # not part of the reference CLI; with --normals=on
     r.add_argument("--levelset-normals", choices=["on", "off"], default="off")
+    # narrow-band signed distance grid of the raw mesh (splashsurf_b200.LevelSetField.signed_distance, DESIGN.md section 14) -- not part
+    # of the reference CLI; FILE.npz, with "{}" for the frame index of a sequence
+    r.add_argument("--output-sdf", default=None, metavar="FILE.npz")
+    r.add_argument("--sdf-band", type=int, default=3, metavar="N")
     # `splashsurf convert` (splashsurf/src/convert.rs:13-56)
     cv = sub.add_parser("convert")
     cv.add_argument("--particles", dest="input_particles", default=None)
@@ -194,6 +198,48 @@ def collect_paths(a):
             continue
         paths.append((os.path.join(parent, entry), os.path.join(out_dir, out_pat.replace("{}", m.group(1)))))
     return paths
+
+
+def _sdf_paths(a, paths):
+    """The --output-sdf file of each (input, output) pair: "{}" is replaced by the frame index of a sequence, as in the mesh names;
+    --output-dir is prepended.  A list of None without --output-sdf."""
+    import os
+    import re
+    if a.output_sdf is None:
+        return [None] * len(paths)
+    seq = "{}" in os.path.basename(a.input)
+    if seq and "{}" not in a.output_sdf:
+        raise ValueError(f'The --output-sdf filename "{a.output_sdf}" does not contain a place holder "{{}}"')
+    out = os.path.join(a.output_dir, a.output_sdf) if a.output_dir is not None else a.output_sdf
+    if not seq:
+        return [out]
+    prefix, suffix = os.path.basename(a.input).split("{}", 1)
+    rx = re.compile(re.escape(prefix) + r"(\d+)" + re.escape(suffix))
+    return [out.replace("{}", rx.search(os.path.basename(src)).group(1)) for src, _ in paths]
+
+
+def write_sdf(path, particles, raw, device, band, *, aniso, avg, radii, **base):
+    """The narrow-band signed distance grid of the raw mesh `raw` (DESIGN.md section 14) with a LevelSetField of the call's keywords on
+    a context of its own, written as .npz: brick_coords, values, brick_inside, the grid's min, cell and points_per_dim, band and
+    background."""
+    import os
+    from . import Context, LevelSetField
+    keep = ("particle_radius", "rest_density", "smoothing_length", "cube_size", "iso_surface_threshold", "aabb_min", "aabb_max",
+            "subdomain_num_cubes_per_dim")
+    fctx = Context(device)
+    try:
+        field = LevelSetField(particles, anisotropy=aniso, averaged_surface=avg, particle_radii=radii, context=fctx,
+                              **{k: v for k, v in base.items() if k in keep})
+        g = field.signed_distance(raw, band=band)
+        field.close()
+    finally:
+        fctx.close()
+    d = os.path.dirname(path)
+    if d and not os.path.exists(d):
+        os.makedirs(d, exist_ok=True)
+    np.savez(path, brick_coords=g.brick_coords, values=g.values, brick_inside=g.brick_inside,
+             min=np.asarray(g.grid.aabb.min, np.float32), cell=np.float32(g.grid.cell_size),
+             points_per_dim=np.asarray(g.grid.npoints_per_dim, np.int64), band=np.int64(g.band), background=np.float32(g.background))
 
 
 def _aabb(lo, hi, what):
@@ -295,7 +341,10 @@ def reconstruct(a) -> int:
             raise ValueError("--levelset-normals=on and --sph-normals=on are exclusive: choose one kind of normals")
         if on(a.averaged_correction):
             raise ValueError("--levelset-normals=on is not available with --averaged-correction=on: the corrected level set has no gradient")
+    if a.output_sdf is not None and on(a.partition):
+        raise ValueError("--output-sdf is not available with --partition=on: the level-set field runs on one GPU per frame")
     paths = collect_paths(a)
+    sdf_paths = _sdf_paths(a, paths)
     if on(a.partition) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         return reconstruct_partitioned(a, paths)
     rank, world = 0, 1
@@ -305,7 +354,7 @@ def reconstruct(a) -> int:
         rank, world = int(os.environ.get("RANK", "0")), int(os.environ["WORLD_SIZE"])
     if not (0 <= rank < world):
         raise ValueError(f"invalid shard {rank}/{world}")
-    paths = paths[rank::world]
+    paths, sdf_paths = paths[rank::world], sdf_paths[rank::world]
     device = a.device if a.device is not None else int(os.environ.get("LOCAL_RANK", "0"))
     pmin, pmax = _aabb(a.particle_aabb_min, a.particle_aabb_max, "particle AABB")
     mmin, mmax = _aabb(a.mesh_aabb_min, a.mesh_aabb_max, "mesh AABB")
@@ -361,6 +410,8 @@ def reconstruct(a) -> int:
             t = time.perf_counter()
             if on(a.output_raw_mesh):                  # "raw_" + file name beside the output file (reconstruct.rs:1618-1650)
                 io.write_mesh(os.path.join(os.path.dirname(dst), "raw_" + os.path.basename(dst)), MeshWithData(raw, {}, {}))
+            if sdf_paths[k] is not None:
+                write_sdf(sdf_paths[k], p, raw, ctx.device, a.sdf_band, aniso=aniso, avg=avg, radii=radii, **base)
             if dst.endswith(".npz"):
                 np.savez(dst, vertices=out.mesh.vertices, triangles=tris, **({"quads": quads} if quads is not None else {}), **out.point_attributes)
             else:

@@ -11,6 +11,7 @@
 #include "ss_aniso.cuh"
 #include "ss_averaged.cuh"
 #include "ss_field.cuh"
+#include "ss_sdf.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
 
@@ -26,6 +27,7 @@
 #include <vector>
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <initializer_list>
 #include <type_traits>
 
@@ -2118,8 +2120,64 @@ static void field_fold(ss_context *c, const SsDev &D, const SsFieldArgs &Q0, uin
     }, launches, received);
 }
 
-// One query of ss_levelset_field_at_f32 or (gradient) ss_levelset_field_gradient_at_f32: keys, sort, group starts, then the cascade
-// of the mode's value fold or gradient fold.
+// The field at m device-resident points `pts` into `out` (and, with `grad`, the gradient fold into grad, pre-zeroed): keys, sort,
+// group starts, then the cascade of the mode's value fold or gradient fold.  Uses the context's query scratch (fld_key_*, fld_idx_*,
+// fld_flag, fld_off, fld_starts, fld_chk), never the field's records.  Returns the refusal of a non-finite point.
+static int field_run(ss_surface *f, ss_context *c, const float *pts, uint32_t m32, float *out, float *grad) {
+    cudaStream_t st = c->stream;
+    const SsDev &D = f->fld_D;
+    c->fld_chk.ensure(8);
+    c->fld_key_a.ensure((size_t)m32 * 4); c->fld_key_b.ensure((size_t)m32 * 4); c->fld_idx_a.ensure((size_t)m32 * 4); c->fld_idx_b.ensure((size_t)m32 * 4);
+    uint32_t chk[2] = { 0xffffffffu, 0u };
+    CK(cudaMemcpyAsync(c->fld_chk.p, chk, 8, cudaMemcpyHostToDevice, st));
+    const uint32_t nsub = f->fld_ready ? f->fld_nsub : 0u;            // no records: every point is 0
+    LAUNCH(c, k_field_keys, nblk(m32, 256), 256, D, pts, m32, make_float3(f->grid.mx[0], f->grid.mx[1], f->grid.mx[2]),
+           c->sub_flat.as<uint32_t>(), nsub, c->fld_key_a.as<uint32_t>(), c->fld_idx_a.as<uint32_t>(), out, c->fld_chk.as<uint32_t>());
+    CK(cudaMemcpyAsync(chk, c->fld_chk.p, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (chk[0] != 0xffffffffu) {
+        char msg[160];
+        snprintf(msg, sizeof msg, "level-set field: point %u has a non-finite coordinate", chk[0]);
+        return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+    }
+    const uint32_t nin = chk[1];
+    if (!nin) return SS_OK;
+    cub_sort(c, c->fld_key_a.as<uint32_t>(), c->fld_key_b.as<uint32_t>(), m32, 32, c->fld_idx_a.as<uint32_t>(), c->fld_idx_b.as<uint32_t>());
+    c->fld_flag.ensure((size_t)nin * 4); c->fld_off.ensure((size_t)nin * 4 + 4); c->fld_starts.ensure((size_t)nin * 4 + 4);
+    LAUNCH(c, k_field_starts, nblk(nin, 256), 256, c->fld_key_b.as<uint32_t>(), nin, c->fld_flag.as<uint32_t>());
+    uint32_t lc[2] = { 0, 0 };
+    scan_compact(c, c->fld_flag.as<uint32_t>(), c->fld_off.as<uint32_t>(), nin, c->fld_starts.as<uint32_t>(), lc);
+    CK(cudaStreamSynchronize(st));
+    const uint32_t n_groups = lc[0] + lc[1];
+    CK(cudaMemcpyAsync(c->fld_starts.as<uint32_t>() + n_groups, &nin, 4, cudaMemcpyHostToDevice, st));
+    SsFieldArgs Q{};
+    Q.A.bins = context_bins(c); Q.A.bins.brick_rng = c->fld_rng.as<int2>();
+    Q.A.grec = c->an_grec.as<float4>(); Q.A.rrec = c->av_rrec.as<float>();
+    Q.pts = pts; Q.key = c->fld_key_b.as<uint32_t>(); Q.idx = c->fld_idx_b.as<uint32_t>();
+    Q.starts = c->fld_starts.as<uint32_t>(); Q.out = out;
+    if (grad) {
+        Q.grad = grad;
+        switch (f->fld_mode) {
+        case SS_FLD_ANISO: field_fold<SsAnisoGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG: field_fold<SsAvgGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG_RAD: field_fold<SsAvgRadGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+        default: field_fold<SsSphGradFold>(c, D, Q, n_groups, f->fld_paths); break;
+        }
+    } else {
+        switch (f->fld_mode) {
+        case SS_FLD_ANISO: field_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG: field_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG_CORR: field_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG_RAD: field_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG_CORR_RAD: field_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+        default: field_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
+        }
+    }
+    return SS_OK;
+}
+
+// One query of ss_levelset_field_at_f32 or (gradient) ss_levelset_field_gradient_at_f32: the caller's points copied to the device,
+// field_run, the results copied back.
 static int field_query(ss_surface *f, const float *points, uint64_t m, float *out, bool gradient, float *grads) {
     int rc; ss_context *c = field_context(f, &rc);
     if (!c) return rc;
@@ -2133,60 +2191,14 @@ static int field_query(ss_surface *f, const float *points, uint64_t m, float *ou
         CK(cudaSetDevice(c->device));
         cudaStream_t st = c->stream;
         const uint32_t m32 = (uint32_t)m;
-        const SsDev &D = f->fld_D;
-        c->fld_pts.ensure((size_t)m32 * 12); c->fld_out.ensure((size_t)m32 * 4); c->fld_chk.ensure(8);
-        c->fld_key_a.ensure((size_t)m32 * 4); c->fld_key_b.ensure((size_t)m32 * 4); c->fld_idx_a.ensure((size_t)m32 * 4); c->fld_idx_b.ensure((size_t)m32 * 4);
+        c->fld_pts.ensure((size_t)m32 * 12); c->fld_out.ensure((size_t)m32 * 4);
         if (gradient) {
             c->fld_grad.ensure((size_t)m32 * 12);
             CK(cudaMemsetAsync(c->fld_grad.p, 0, (size_t)m32 * 12, st));       // points without candidates: gradient 0
         }
         CK(cudaMemcpyAsync(c->fld_pts.p, points, (size_t)m32 * 12, cudaMemcpyDefault, st));
-        uint32_t chk[2] = { 0xffffffffu, 0u };
-        CK(cudaMemcpyAsync(c->fld_chk.p, chk, 8, cudaMemcpyHostToDevice, st));
-        const uint32_t nsub = f->fld_ready ? f->fld_nsub : 0u;            // no records: every point is 0
-        LAUNCH(c, k_field_keys, nblk(m32, 256), 256, D, c->fld_pts.as<float>(), m32, make_float3(f->grid.mx[0], f->grid.mx[1], f->grid.mx[2]),
-               c->sub_flat.as<uint32_t>(), nsub, c->fld_key_a.as<uint32_t>(), c->fld_idx_a.as<uint32_t>(), c->fld_out.as<float>(), c->fld_chk.as<uint32_t>());
-        CK(cudaMemcpyAsync(chk, c->fld_chk.p, 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        if (chk[0] != 0xffffffffu) {
-            char msg[160];
-            snprintf(msg, sizeof msg, "level-set field: point %u has a non-finite coordinate", chk[0]);
-            return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
-        }
-        const uint32_t nin = chk[1];
-        if (nin) {
-            cub_sort(c, c->fld_key_a.as<uint32_t>(), c->fld_key_b.as<uint32_t>(), m32, 32, c->fld_idx_a.as<uint32_t>(), c->fld_idx_b.as<uint32_t>());
-            c->fld_flag.ensure((size_t)nin * 4); c->fld_off.ensure((size_t)nin * 4 + 4); c->fld_starts.ensure((size_t)nin * 4 + 4);
-            LAUNCH(c, k_field_starts, nblk(nin, 256), 256, c->fld_key_b.as<uint32_t>(), nin, c->fld_flag.as<uint32_t>());
-            uint32_t lc[2] = { 0, 0 };
-            scan_compact(c, c->fld_flag.as<uint32_t>(), c->fld_off.as<uint32_t>(), nin, c->fld_starts.as<uint32_t>(), lc);
-            CK(cudaStreamSynchronize(st));
-            const uint32_t n_groups = lc[0] + lc[1];
-            CK(cudaMemcpyAsync(c->fld_starts.as<uint32_t>() + n_groups, &nin, 4, cudaMemcpyHostToDevice, st));
-            SsFieldArgs Q{};
-            Q.A.bins = context_bins(c); Q.A.bins.brick_rng = c->fld_rng.as<int2>();
-            Q.A.grec = c->an_grec.as<float4>(); Q.A.rrec = c->av_rrec.as<float>();
-            Q.pts = c->fld_pts.as<float>(); Q.key = c->fld_key_b.as<uint32_t>(); Q.idx = c->fld_idx_b.as<uint32_t>();
-            Q.starts = c->fld_starts.as<uint32_t>(); Q.out = c->fld_out.as<float>();
-            if (gradient) {
-                Q.grad = c->fld_grad.as<float>();
-                switch (f->fld_mode) {
-                case SS_FLD_ANISO: field_fold<SsAnisoGradFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG: field_fold<SsAvgGradFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG_RAD: field_fold<SsAvgRadGradFold>(c, D, Q, n_groups, f->fld_paths); break;
-                default: field_fold<SsSphGradFold>(c, D, Q, n_groups, f->fld_paths); break;
-                }
-            } else {
-                switch (f->fld_mode) {
-                case SS_FLD_ANISO: field_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG: field_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG_CORR: field_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG_RAD: field_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
-                case SS_FLD_AVG_CORR_RAD: field_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
-                default: field_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
-                }
-            }
-        }
+        const int rc = field_run(f, c, c->fld_pts.as<float>(), m32, c->fld_out.as<float>(), gradient ? c->fld_grad.as<float>() : nullptr);
+        if (rc) return rc;
         CK(cudaMemcpyAsync(out, c->fld_out.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
         if (gradient) CK(cudaMemcpyAsync(grads, c->fld_grad.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
         CK(cudaStreamSynchronize(st));
@@ -2212,6 +2224,198 @@ extern "C" int ss_levelset_field_paths(const ss_surface *f, uint64_t out[3]) {
     if (!f || !f->fld || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or not a level-set field");
     for (int t = 0; t < 3; ++t) out[t] = f->fld_paths[t];
     return SS_OK;
+}
+
+// ------------------------------------------------------------------ narrow-band signed distance grid ----
+// DESIGN.md §14.  The result owns its device buffers: it outlives later queries, reconstructions and the field itself.
+struct ss_sdf {
+    int device = 0;
+    uint64_t nl = 0;                 // listed bricks
+    int64_t nb[3] = { 0, 0, 0 };     // bricks per axis
+    float B = 0.0f;                  // background
+    uint64_t paths[2] = { 0, 0 };    // candidate bricks through the shared slice, through the global walk
+    uint64_t passes = 0, pairs = 0;  // slabs with candidates, and their (brick, triangle) pairs
+    DevBuf coords, values, inside;   // [nl][3] int32, [nl][512] float, [nb0 nb1 nb2] uint8
+};
+
+// The working set of one pass: its (brick, triangle) pairs (16 bytes each in keys and values) and its bricks (up to 2 KB of distances
+// each, 16 KB of query points, keys and values per listed brick), also bounded by the free device memory.  A call runs as many passes
+// as its mesh needs.
+#define SS_SDF_PASS_BRICKS (1ull << 19)
+static uint64_t g_sdf_pass_pairs = 1ull << 27;
+extern "C" void ss_sdf_set_pass_pairs(uint64_t pairs) { g_sdf_pass_pairs = pairs ? std::min<uint64_t>(pairs, 0x7ffffffeull) : (1ull << 27); }
+
+extern "C" int ss_levelset_field_sdf_f32(ss_surface *f, const float *vertices, uint64_t nv, const uint32_t *triangles, uint64_t nt,
+                                         uint32_t band, ss_sdf **out) {
+    if (!out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    *out = nullptr;
+    int rc; ss_context *c = field_context(f, &rc);
+    if (!c) return rc;
+    if ((nv && !vertices) || (nt && !triangles)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    if (band < 1 || band > 8) return ss_fail(SS_ERR_INVALID_PARAMETER, "signed distance: band must lie in [1, 8] cells");
+    if (nv >= (1ull << 32)) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "signed distance: 2^32 or more vertices");
+    if (nt >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "signed distance: too many triangles for one call");
+    SsSdfGrid G{};
+    uint64_t nbtot = 1;
+    for (int d = 0; d < 3; ++d) {
+        G.gmin[d] = f->grid.mn[d];
+        G.np[d] = (int)f->grid.np[d];
+        G.nb[d] = (int)((f->grid.np[d] + 7) / 8);
+        nbtot *= (uint64_t)G.nb[d];
+    }
+    G.c = f->grid.cell;
+    { volatile float b = (float)band * G.c; G.B = b; volatile float r = G.B + G.c; G.reach = r; }
+    if (nbtot >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "signed distance: too many bricks in the grid");
+    std::unique_ptr<ss_sdf> R(new ss_sdf());
+    R->device = c->device; R->B = G.B;
+    for (int d = 0; d < 3; ++d) R->nb[d] = G.nb[d];
+    rc = ss_guard([&]() -> int {
+        CK(cudaSetDevice(c->device));
+        cudaStream_t st = c->stream;
+        const uint32_t nt32 = (uint32_t)nt;
+        // own buffers throughout: the context scratch holds the field's records
+        DevBuf verts, tris, chk, cnt, off, hist, key_a, key_b, val_a, val_b, flag, scan, starts, dist, listed, lpaths, list, pts, fv;
+        verts.ensure(nv * 12); tris.ensure((size_t)nt32 * 12); chk.ensure(16); lpaths.ensure(8); hist.ensure((size_t)G.nb[0] * 8);
+        if (nv) CK(cudaMemcpyAsync(verts.p, vertices, nv * 12, cudaMemcpyDefault, st));
+        if (nt32) CK(cudaMemcpyAsync(tris.p, triangles, (size_t)nt32 * 12, cudaMemcpyDefault, st));
+        unsigned long long hchk[2] = { ~0ull, ~0ull };
+        CK(cudaMemcpyAsync(chk.p, hchk, 16, cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(lpaths.p, 0, 8, st));
+        CK(cudaMemsetAsync(hist.p, 0, (size_t)G.nb[0] * 8, st));
+        if (nv) LAUNCH(c, k_sdf_check_verts, nblk(nv, 256), 256, verts.as<float>(), nv, chk.as<unsigned long long>());
+        // candidate bricks per brick column over the whole grid, and the index check
+        if (nt32) LAUNCH(c, k_sdf_count, nblk(nt32, 256), 256, G, verts.as<float>(), nv, tris.as<uint32_t>(), nt32, 0, G.nb[0],
+                         (unsigned long long *)nullptr, hist.as<unsigned long long>(), chk.as<unsigned long long>());
+        std::vector<unsigned long long> col((size_t)G.nb[0]);
+        CK(cudaMemcpyAsync(col.data(), hist.p, (size_t)G.nb[0] * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(hchk, chk.p, 16, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        char msg[200];
+        if (hchk[0] != ~0ull) {
+            snprintf(msg, sizeof msg, "signed distance: vertex %llu has a non-finite coordinate", hchk[0]);
+            return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+        }
+        if (hchk[1] != ~0ull) {
+            snprintf(msg, sizeof msg, "signed distance: triangle %llu has a vertex index >= the number of vertices (%llu)", hchk[1], (unsigned long long)nv);
+            return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+        }
+        // Passes over slabs of whole brick columns, ascending (the listed bricks stay in ascending order): a slab grows while its pairs
+        // stay within the pair bound and its bricks within SS_SDF_PASS_BRICKS; one column is the least a pass takes.
+        const uint64_t col_bricks = (uint64_t)G.nb[1] * (uint64_t)G.nb[2];
+        // a pass holds about 36 bytes per pair (keys, values, flags, scan, starts, sort scratch) and 25 KB per brick (distances, then
+        // query points, keys, indices and values of its listed bricks): both bounds also stay within a third of the free memory each
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        const uint64_t max_pairs = std::max<uint64_t>(1, std::min<uint64_t>(g_sdf_pass_pairs, free_b / 3 / 36));
+        const uint64_t max_bricks = std::max<uint64_t>(1, std::min<uint64_t>(SS_SDF_PASS_BRICKS, free_b / 3 / 25600));
+        int bx0 = 0;
+        while (bx0 < G.nb[0]) {
+            int bx1 = bx0 + 1;
+            uint64_t np_s = col[bx0];
+            while (bx1 < G.nb[0] && np_s + col[bx1] <= max_pairs && (uint64_t)(bx1 + 1 - bx0) * col_bricks <= max_bricks) np_s += col[bx1++];
+            const int sx0 = bx0;
+            bx0 = bx1;
+            if (!np_s) continue;
+            if (np_s >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "signed distance: one brick column has 2^31 or more (brick, triangle) pairs");
+            ++R->passes;
+            R->pairs += np_s;
+            const uint32_t np32 = (uint32_t)np_s;
+            cnt.ensure((size_t)nt32 * 8); off.ensure((size_t)nt32 * 8);
+            LAUNCH(c, k_sdf_count, nblk(nt32, 256), 256, G, verts.as<float>(), nv, tris.as<uint32_t>(), nt32, sx0, bx1, cnt.as<unsigned long long>(),
+                   (unsigned long long *)nullptr, chk.as<unsigned long long>());
+            cub_scan(c, cnt.as<unsigned long long>(), off.as<unsigned long long>(), nt32);
+            key_a.ensure((size_t)np32 * 4); key_b.ensure((size_t)np32 * 4); val_a.ensure((size_t)np32 * 4); val_b.ensure((size_t)np32 * 4);
+            LAUNCH(c, k_sdf_emit, nblk(nt32, 256), 256, G, verts.as<float>(), tris.as<uint32_t>(), nt32, sx0, bx1, off.as<unsigned long long>(),
+                   key_a.as<uint32_t>(), val_a.as<uint32_t>());
+            cub_sort(c, key_a.as<uint32_t>(), key_b.as<uint32_t>(), np32, bits_for(nbtot - 1), val_a.as<uint32_t>(), val_b.as<uint32_t>());
+            flag.ensure((size_t)np32 * 4); scan.ensure((size_t)np32 * 4); starts.ensure((size_t)np32 * 4 + 4);
+            LAUNCH(c, k_field_starts, nblk(np32, 256), 256, key_b.as<uint32_t>(), np32, flag.as<uint32_t>());
+            uint32_t lc[2] = { 0, 0 };
+            scan_compact(c, flag.as<uint32_t>(), scan.as<uint32_t>(), np32, starts.as<uint32_t>(), lc);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t ncand = lc[0] + lc[1];
+            CK(cudaMemcpyAsync(starts.as<uint32_t>() + ncand, &np32, 4, cudaMemcpyHostToDevice, st));
+            dist.ensure((size_t)ncand * 512 * 4); listed.ensure((size_t)ncand * 4);
+            SsSdfArgs A{};
+            A.G = G; A.verts = verts.as<float>(); A.tris = tris.as<uint32_t>(); A.key = key_b.as<uint32_t>(); A.val = val_b.as<uint32_t>();
+            A.starts = starts.as<uint32_t>(); A.ncand = ncand; A.dist = dist.as<float>(); A.listed = listed.as<uint32_t>(); A.paths = lpaths.as<uint32_t>();
+            LAUNCH(c, (k_sdf_brick<SS_SDF_WARPS, SS_SDF_CAP>), nblk(ncand, SS_SDF_WARPS), SS_SDF_WARPS * 32, A);
+            list.ensure((size_t)ncand * 4); scan.ensure((size_t)ncand * 4);
+            uint32_t ll[2] = { 0, 0 };
+            scan_compact(c, listed.as<uint32_t>(), scan.as<uint32_t>(), ncand, list.as<uint32_t>(), ll);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t nl = ll[0] + ll[1];
+            if (!nl) continue;
+            // this pass's listed bricks: coordinates, then distances with the field's sign, appended to the result
+            if ((uint64_t)nl * 512 >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "signed distance: one brick column lists 2^22 or more bricks");
+            const uint32_t m32 = nl * 512u;
+            R->coords.grow_keep((R->nl + nl) * 12, R->nl * 12, st); R->values.grow_keep((R->nl + nl) * 2048, R->nl * 2048, st);
+            pts.ensure((size_t)m32 * 12); fv.ensure((size_t)m32 * 4);
+            LAUNCH(c, k_sdf_points, nblk(m32, 256), 256, G, key_b.as<uint32_t>(), starts.as<uint32_t>(), list.as<uint32_t>(), nl, 0u,
+                   pts.as<float>(), R->coords.as<int32_t>() + 3 * R->nl);
+            int rc = field_run(f, c, pts.as<float>(), m32, fv.as<float>(), nullptr);
+            if (rc) return rc;
+            LAUNCH(c, k_sdf_sign, nblk(m32, 256), 256, G, f->fld_D.thr, dist.as<float>(), key_b.as<uint32_t>(), starts.as<uint32_t>(),
+                   list.as<uint32_t>(), nl, 0u, fv.as<float>(), R->values.as<float>() + 512 * R->nl, (uint8_t *)nullptr);
+            R->nl += nl;
+        }
+        uint32_t hp[2] = { 0, 0 };
+        CK(cudaMemcpyAsync(hp, lpaths.p, 8, cudaMemcpyDeviceToHost, st));
+        // the inside flag of every brick: the field at its first point
+        const uint32_t nb32 = (uint32_t)nbtot;
+        R->inside.ensure(nbtot);
+        pts.ensure((size_t)nb32 * 12); fv.ensure((size_t)nb32 * 4);
+        LAUNCH(c, k_sdf_points, nblk(nb32, 256), 256, G, key_b.as<uint32_t>(), starts.as<uint32_t>(), list.as<uint32_t>(), 0u, nb32,
+               pts.as<float>(), (int32_t *)nullptr);
+        int rc = field_run(f, c, pts.as<float>(), nb32, fv.as<float>(), nullptr);
+        if (rc) return rc;
+        LAUNCH(c, k_sdf_sign, nblk(nb32, 256), 256, G, f->fld_D.thr, dist.as<float>(), key_b.as<uint32_t>(), starts.as<uint32_t>(), list.as<uint32_t>(),
+               0u, nb32, fv.as<float>(), (float *)nullptr, R->inside.as<uint8_t>());
+        CK(cudaStreamSynchronize(st));
+        R->paths[0] = hp[0]; R->paths[1] = hp[1];
+        return SS_OK;
+    });
+    if (rc) return rc;
+    *out = R.release();
+    return SS_OK;
+}
+
+extern "C" uint64_t ss_sdf_num_bricks(const ss_sdf *s) { return s ? s->nl : 0; }
+
+extern "C" int ss_sdf_info(const ss_sdf *s, int64_t bricks_per_dim[3], float *background) {
+    if (!s) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL signed distance grid");
+    if (bricks_per_dim) for (int d = 0; d < 3; ++d) bricks_per_dim[d] = s->nb[d];
+    if (background) *background = s->B;
+    return SS_OK;
+}
+
+extern "C" int ss_sdf_copy_f32(const ss_sdf *s, int32_t *brick_coords, float *values, uint8_t *brick_inside) {
+    if (!s) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL signed distance grid");
+    return ss_guard([&]() -> int {
+        CK(cudaSetDevice(s->device));
+        if (brick_coords && s->nl) CK(cudaMemcpy(brick_coords, s->coords.p, s->nl * 12, cudaMemcpyDefault));
+        if (values && s->nl) CK(cudaMemcpy(values, s->values.p, s->nl * 2048, cudaMemcpyDefault));
+        if (brick_inside) CK(cudaMemcpy(brick_inside, s->inside.p, (size_t)(s->nb[0] * s->nb[1] * s->nb[2]), cudaMemcpyDefault));
+        return SS_OK;
+    });
+}
+
+extern "C" int ss_sdf_passes(const ss_sdf *s, uint64_t out[2]) {
+    if (!s || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    out[0] = s->passes; out[1] = s->pairs;
+    return SS_OK;
+}
+
+extern "C" int ss_sdf_paths(const ss_sdf *s, uint64_t out[2]) {
+    if (!s || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    out[0] = s->paths[0]; out[1] = s->paths[1];
+    return SS_OK;
+}
+
+extern "C" void ss_sdf_free(ss_sdf *s) {
+    if (!s) return;
+    cudaSetDevice(s->device);
+    delete s;
 }
 
 #include "ss_post.cuh"
