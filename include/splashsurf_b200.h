@@ -389,6 +389,22 @@ int ss_levelset_field_paths(const ss_surface *field, uint64_t out[3]);
  * ss_levelset_field_paths are set as for ss_levelset_field_at_f32. */
 int ss_levelset_field_gradient_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *gradients);
 
+/* Hessian and curvature of the level-set field at arbitrary points (DESIGN.md section 13.2).
+ * ss_levelset_field_hessian_at_f32: the exact second derivative, with respect to the point, of the value ss_levelset_field_at_f32
+ * returns (same candidates, ascending particle index, every operation one f32 rounding).  values [m] and gradients [m][3] are
+ * bit-identical to ss_levelset_field_gradient_at_f32; hessians is [m][6] (xx, xy, xz, yy, yz, zz).  Where no candidate reaches a
+ * point all three are 0.
+ * ss_levelset_field_curvature_at_f32: values [m] as above, curvatures [m][2] = (mean, Gaussian) curvature of the level set through
+ * the point, kappa_H = -(|g|^2 tr H - g^T H g) / (2 |g|^3) (a ball of liquid of radius rho has 1 / rho) and kappa_G =
+ * g^T adj(H) g / |g|^4 (1 / rho^2); both NaN where |g|^2 rounds to 0.  The gradients and Hessians go in buffers of the call.
+ * All arrays in host or device memory.  Refusals are those of ss_levelset_field_gradient_at_f32, including SS_ERR_UNSUPPORTED for a
+ * field created with the Jacobian correction on.  The tier counters of ss_levelset_field_paths are set as for
+ * ss_levelset_field_at_f32.  In float32 the Hessian of the averaged surfaces loses accuracy like 1 / b^2 where every candidate
+ * sits near the edge of its support (b = 1 - |d|^2 / h^2), and deep inside the liquid the gradient is close to 0, so the
+ * curvature there means nothing. */
+int ss_levelset_field_hessian_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *gradients, float *hessians);
+int ss_levelset_field_curvature_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *curvatures);
+
 /* Narrow-band signed distance grid of a mesh on the field's lattice (DESIGN.md section 14).  The lattice is the field's grid
  * (ss_surface_grid): points min + index * cell_size, index in [0, n] per axis, in bricks of 8 x 8 x 8 points (ceil((n + 1) / 8) per
  * axis).  B = band * cell_size (band in [1, 8]).  d(p) is the f32 minimum over all triangles of the point-triangle distance, every

@@ -208,6 +208,8 @@ def _bind(L):
     L.ss_levelset_field_create_f32.argtypes = [vp, vp, C.c_uint64, C.POINTER(_Params), C.POINTER(vp)]
     L.ss_levelset_field_at_f32.argtypes = [vp, vp, C.c_uint64, vp]
     L.ss_levelset_field_gradient_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp]
+    L.ss_levelset_field_hessian_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp, vp]
+    L.ss_levelset_field_curvature_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp]
     L.ss_levelset_field_threshold_f32.argtypes = [vp, C.POINTER(C.c_float)]
     L.ss_levelset_field_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.ss_levelset_field_sdf_f32.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint32, C.POINTER(vp)]
@@ -1132,8 +1134,9 @@ class LevelSetField:
         _check(L, L.ss_surface_grid(self._s, C.byref(g)))
         self.grid = UniformGrid._from(g)
 
-    def _query(self, points, gradient: bool):
-        """Values (and gradients) at (M, 3) float32 points: numpy in, numpy out; a CUDA torch tensor in, CUDA tensors out."""
+    def _query(self, points, kind: str = "value"):
+        """Values at (M, 3) float32 points, and with ``kind`` "gradient" the gradients, "hessian" the gradients and Hessians,
+        "curvature" the curvatures: numpy in, numpy out; a CUDA torch tensor in, CUDA tensors out."""
         L = self._ctx._L
         cuda = hasattr(points, "data_ptr") and getattr(points, "is_cuda", False)
         if cuda:
@@ -1147,27 +1150,27 @@ class LevelSetField:
                 raise TypeError("unsupported scalar type: the field is evaluated at float32 points only")
         if x.ndim != 2 or x.shape[1] != 3:
             raise ValueError("points must have shape (M, 3)")
+        shapes = {"value": (), "gradient": ((3,),), "hessian": ((3,), (6,)), "curvature": ((2,),)}[kind]
         if cuda:
             x = x.contiguous()
             out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
-            grad = torch.empty((x.shape[0], 3), dtype=torch.float32, device=x.device) if gradient else None
+            extra = [torch.empty((x.shape[0],) + sh, dtype=torch.float32, device=x.device) for sh in shapes]
             torch.cuda.current_stream(x.device).synchronize()
             ptr = lambda a: a.data_ptr() if len(x) else None  # noqa: E731
         else:
             x = np.ascontiguousarray(x)
             out = np.empty(len(x), dtype=np.float32)
-            grad = np.empty((len(x), 3), dtype=np.float32) if gradient else None
+            extra = [np.empty((len(x),) + sh, dtype=np.float32) for sh in shapes]
             ptr = lambda a: a.ctypes.data if len(x) else None  # noqa: E731
-        if gradient:
-            _check(L, L.ss_levelset_field_gradient_at_f32(self._s, ptr(x), len(x), ptr(out), ptr(grad)))
-            return out, grad
-        _check(L, L.ss_levelset_field_at_f32(self._s, ptr(x), len(x), ptr(out)))
-        return out
+        entry = {"value": L.ss_levelset_field_at_f32, "gradient": L.ss_levelset_field_gradient_at_f32,
+                 "hessian": L.ss_levelset_field_hessian_at_f32, "curvature": L.ss_levelset_field_curvature_at_f32}[kind]
+        _check(L, entry(self._s, ptr(x), len(x), ptr(out), *[ptr(a) for a in extra]))
+        return (out, *extra) if extra else out
 
     def evaluate(self, points):
         """The field at the points: an (M, 3) float32 numpy array gives an (M,) float32 numpy array; a CUDA float32 torch tensor of
         shape (M, 3) is read on the device and gives an (M,) CUDA tensor."""
-        return self._query(points, False)
+        return self._query(points)
 
     def gradient(self, points):
         """``(values, gradients)`` at the points (DESIGN.md section 13.1): the exact derivative of the field with respect to the point,
@@ -1180,16 +1183,40 @@ class LevelSetField:
         Accuracy in float32: near the surface (the narrow band users shade and collide in) the normal is accurate; for the averaged
         surfaces the gradient loses accuracy where every candidate sits near the edge of its support (about h outside the
         surface), and deep inside the liquid it is close to 0 because the averaged field is not a distance field there."""
-        return self._query(points, True)
+        return self._query(points, "gradient")
 
     def normals(self, points):
         """Outward unit normals ``-gradient / |gradient|`` at the points (inside is ``value > threshold``), as numpy or CUDA torch
         like ``gradient``; NaN where the gradient is 0, like ``SphInterpolator.interpolate_normals``."""
-        _, g = self._query(points, True)
+        _, g = self._query(points, "gradient")
         if isinstance(g, np.ndarray):
             with np.errstate(invalid="ignore", divide="ignore"):
                 return (-g / np.linalg.norm(g, axis=1, keepdims=True)).astype(np.float32)
         return -g / g.norm(dim=1, keepdim=True)
+
+    def hessian(self, points):
+        """``(values, gradients, hessians)`` at the points (DESIGN.md section 13.2): the exact second derivative of the field with
+        respect to the point, as (M, 6) entries ``xx, xy, xz, yy, yz, zz``, from the same candidates and records as ``evaluate``;
+        values and gradients equal those of ``evaluate`` and ``gradient`` bit for bit.  Numpy in gives numpy out, a CUDA float32
+        torch tensor gives CUDA tensors; points no particle reaches get 0.  The checks are those of ``evaluate``; a field of the
+        Jacobian-corrected averaged surface raises ``SplashsurfError`` as ``gradient`` does.
+
+        Accuracy in float32: for the averaged surfaces the Hessian's new sums carry the weight's ``b = 1 - |d|^2 / h^2`` against
+        ``b^3`` in the weights, so rounding grows like ``1 / b^2`` where every candidate sits near the edge of its support (about h
+        outside the surface); near the surface it is accurate."""
+        return self._query(points, "hessian")
+
+    def curvature(self, points):
+        """``(mean, gaussian)`` curvature of the level set through each point (DESIGN.md section 13.2), as (M,) float32 numpy arrays
+        or CUDA tensors like ``hessian``: with ``g`` the gradient and ``H`` the Hessian, ``mean = -(|g|^2 tr H - g^T H g) /
+        (2 |g|^3)`` (half the divergence of the outward normal; a ball of liquid of radius rho has 1 / rho) and ``gaussian =
+        g^T adj(H) g / |g|^4`` (1 / rho^2); both NaN where the gradient is 0, like ``normals``.  Deep inside the liquid the gradient
+        of the averaged surfaces is close to 0 and the curvature there means nothing; at and near the surface it is the
+        curvature of the surface that was meshed."""
+        _, c = self._query(points, "curvature")
+        if isinstance(c, np.ndarray):
+            return np.ascontiguousarray(c[:, 0]), np.ascontiguousarray(c[:, 1])
+        return c[:, 0].contiguous(), c[:, 1].contiguous()
 
     def inside(self, points):
         """``evaluate(points) > threshold``."""
@@ -1611,7 +1638,7 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                             output_raw_normals: bool = False, output_raw_mesh: bool = False, context: Optional[Context] = None,
                             with_debug: bool = False, anisotropy: Optional[Anisotropy] = None,
                             averaged_surface: Optional[AveragedSurface] = None, particle_radii=None, levelset_normals: bool = False,
-                            **post):
+                            levelset_curvature: bool = False, **post):
     """``pysplashsurf.reconstruction_pipeline`` (pysplashsurf/src/pipeline.rs:109-200) on the GPU: surface reconstruction plus
     the post-processing steps of splashsurf/src/reconstruct.rs:1094-1391 that run on the device -- smoothing weights, weighted
     Laplacian smoothing, SPH or area-weighted normals (at the smoothed vertices), normal smoothing and SPH interpolation of
@@ -1631,7 +1658,13 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     the area-weighted face normals: the normals of the anisotropic or averaged surface the call asked for.  The field is built with
     this call's keywords on a context of its own (it repeats decomposition, densities and binning), evaluated at the vertices the
     normals step sees (after Laplacian smoothing) and closed; ``normals_smoothing_iters`` and ``output_raw_normals`` apply to the
-    result.  Refused with ``sph_normals``, without ``compute_normals`` and for the Jacobian-corrected averaged surface."""
+    result.  Refused with ``sph_normals``, without ``compute_normals`` and for the Jacobian-corrected averaged surface.
+
+    ``levelset_curvature=True`` (not part of the reference; independent of ``compute_normals``) adds the point attributes
+    ``mean_curvature`` and ``gaussian_curvature`` (float32, shape ``(nv,)``): the curvature of the level set that was meshed
+    (``LevelSetField.curvature``, DESIGN.md section 13.2) at the vertices the normals step sees (after Laplacian smoothing).  The
+    field is built on a context of its own as for ``levelset_normals``; with both switches on, one field serves both.  Refused for
+    the Jacobian-corrected averaged surface."""
     passive = ("mesh_cleanup", "decimate_barnacles", "mesh_cleanup_snap_dist", "keep_vertices", "generate_quads", "quad_max_edge_diag_ratio",
                "quad_max_normal_angle", "quad_max_interior_angle", "mesh_aabb_min", "mesh_aabb_max", "mesh_aabb_clamp_vertices",
                "check_mesh_closed", "check_mesh_manifold", "check_mesh_orientation", "check_mesh_debug")
@@ -1645,6 +1678,9 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
     if levelset_normals and averaged_surface is not None and averaged_surface.correction is not None:
         raise ValueError("levelset_normals=True is not available for the Jacobian-corrected averaged surface: its level set has no "
                          "gradient (DESIGN.md section 13.1)")
+    if levelset_curvature and averaged_surface is not None and averaged_surface.correction is not None:
+        raise ValueError("levelset_curvature=True is not available for the Jacobian-corrected averaged surface: its level set has no "
+                         "Hessian (DESIGN.md section 13.2)")
     mesh_cleanup, decimate_barnacles = bool(post.get("mesh_cleanup", False)), bool(post.get("decimate_barnacles", False))
     keep_vertices, snap_dist = bool(post.get("keep_vertices", False)), post.get("mesh_cleanup_snap_dist", None)
     arr = np.asarray(particles)
@@ -1698,7 +1734,8 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
         if mesh_smoothing_iters:
             verts = np.empty((nv, 3), np.float32)
             _check(L, L.ss_surface_copy_vertices(s, verts.ctypes.data))
-        if compute_normals and levelset_normals:                                # DESIGN.md section 13.1
+        use_ln = compute_normals and levelset_normals
+        if use_ln or levelset_curvature:                                        # DESIGN.md sections 13.1, 13.2
             # a context of its own: a field on the pipeline's context would make this surface's post-processing state stale
             fctx = Context(ctx.device)
             try:
@@ -1706,10 +1743,15 @@ def reconstruction_pipeline(particles, *, attributes_to_interpolate=None, partic
                                       cube_size=cube_size, iso_surface_threshold=iso_surface_threshold, aabb_min=aabb_min, aabb_max=aabb_max,
                                       subdomain_num_cubes_per_dim=subdomain_num_cubes_per_dim, anisotropy=anisotropy,
                                       averaged_surface=averaged_surface, particle_radii=radii, context=fctx)
-                nrm = np.ascontiguousarray(field.normals(np.ascontiguousarray(verts, np.float32)))
+                vq = np.ascontiguousarray(verts, np.float32)
+                if use_ln:
+                    nrm = np.ascontiguousarray(field.normals(vq))
+                if levelset_curvature:
+                    point["mean_curvature"], point["gaussian_curvature"] = field.curvature(vq)
                 field.close()
             finally:
                 fctx.close()
+        if use_ln:
             _check(L, L.ss_surface_set_normals_f32(s, nrm.ctypes.data if nv else None))
         elif compute_normals:                                                   # reconstruct.rs:1282-1342
             _check(L, L.ss_surface_compute_normals_f32(s, int(bool(sph_normals))))

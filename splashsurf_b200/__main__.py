@@ -128,6 +128,10 @@ def main(argv=None):
     # normals from the gradient of the level set that was meshed (splashsurf_b200.LevelSetField.normals, DESIGN.md section 13.1) --
     # not part of the reference CLI; with --normals=on
     r.add_argument("--levelset-normals", choices=["on", "off"], default="off")
+    # the point attributes mean_curvature and gaussian_curvature: the curvature of the level set that was meshed at the vertices
+    # (splashsurf_b200.LevelSetField.curvature, DESIGN.md section 13.2) -- not part of the reference CLI
+    r.add_argument("--levelset-curvature", choices=["on", "off"], default="off",
+                   help="write the mean and Gaussian curvature of the level set at the mesh vertices as point attributes")
     # narrow-band signed distance grid of the raw mesh (splashsurf_b200.LevelSetField.signed_distance, DESIGN.md section 14) -- not part
     # of the reference CLI; FILE.npz, with "{}" for the frame index of a sequence
     r.add_argument("--output-sdf", default=None, metavar="FILE.npz")
@@ -341,6 +345,11 @@ def reconstruct(a) -> int:
             raise ValueError("--levelset-normals=on and --sph-normals=on are exclusive: choose one kind of normals")
         if on(a.averaged_correction):
             raise ValueError("--levelset-normals=on is not available with --averaged-correction=on: the corrected level set has no gradient")
+    if on(a.levelset_curvature):
+        if on(a.partition):
+            raise ValueError("--levelset-curvature=on is not available with --partition=on: the level-set field runs on one GPU per frame")
+        if on(a.averaged_correction):
+            raise ValueError("--levelset-curvature=on is not available with --averaged-correction=on: the corrected level set has no Hessian")
     if a.output_sdf is not None and on(a.partition):
         raise ValueError("--output-sdf is not available with --partition=on: the level-set field runs on one GPU per frame")
     paths = collect_paths(a)
@@ -368,7 +377,7 @@ def reconstruct(a) -> int:
     chk = on(a.check_mesh)
     closed, manifold, orient = chk or on(a.check_mesh_closed), chk or on(a.check_mesh_manifold), chk or on(a.check_mesh_orientation)
     post = any([bool(a.interpolate_attributes), on(a.normals), on(a.mesh_cleanup), on(a.decimate_barnacles), a.mesh_smoothing_iters is not None,
-                on(a.generate_quads), mmin is not None, closed, manifold, orient])
+                on(a.generate_quads), mmin is not None, closed, manifold, orient, on(a.levelset_curvature)])
     ctx = Context(device) if paths else None
     try:
         for k, (src, dst) in enumerate(paths):
@@ -396,7 +405,8 @@ def reconstruct(a) -> int:
                     quad_max_normal_angle=a.quad_max_normal_angle, quad_max_interior_angle=a.quad_max_interior_angle, mesh_aabb_min=mmin,
                     mesh_aabb_max=mmax, mesh_aabb_clamp_vertices=on(a.mesh_aabb_clamp_verts), check_mesh_closed=closed, check_mesh_manifold=manifold,
                     check_mesh_orientation=orient, check_mesh_debug=on(a.check_mesh_debug), context=ctx, anisotropy=aniso,
-                    averaged_surface=avg, particle_radii=radii, levelset_normals=on(a.levelset_normals), **base)
+                    averaged_surface=avg, particle_radii=radii, levelset_normals=on(a.levelset_normals),
+                    levelset_curvature=on(a.levelset_curvature), **base)
                 raw = rec.mesh
             else:
                 raw = reconstruct_surface(p, context=ctx, anisotropy=aniso, averaged_surface=avg, particle_radii=radii, **base).mesh

@@ -17,7 +17,9 @@
 // A group's candidate bins cover the cells [8b - R, 8b + 8 + R) along each axis (ss_pipeline.cu: upload_field_brick_ranges): a point lies
 // anywhere in the closed cell box [8b, 8b + 8]^3 of its brick, one cell further than the brick's grid points reach.
 // ss_levelset_field_gradient_at_f32 runs the same sequence with the gradient folds below (SsSphGradFold, SsAnisoGradFold,
-// SsAvgGradFold, SsAvgRadGradFold), which k_field_fold and k_field_select recognise at compile time and also write the gradient for.
+// SsAvgGradFold, SsAvgRadGradFold), which k_field_fold and k_field_select recognise at compile time and also write the gradient for;
+// ss_levelset_field_hessian_at_f32 likewise with the Hessian folds (SsSphHessFold, SsAnisoHessFold, SsAvgHessFold, SsAvgRadHessFold),
+// and ss_levelset_field_curvature_at_f32 turns their gradients and Hessians into curvatures (k_field_curvature).
 #pragma once
 #include <type_traits>
 
@@ -170,6 +172,275 @@ struct SsAvgRadGradFold {
     }
 };
 
+// ------------------------------------------------------------------ Hessians (DESIGN.md §13.2) ----
+// The second derivative of the value at the query point p, six entries xx, xy, xz, yy, yz, zz.  A Hessian fold wraps its gradient
+// fold as that wraps the value fold: its Acc holds the gradient fold's Acc, its add calls the gradient fold's add first, and its
+// value and gradient are the gradient fold's, bit for bit.  It adds
+//   void     F::hessian(P, acc, H)      the Hessian (0 where no candidate reaches p)
+// which k_field_fold / k_field_select write to SsFieldArgs::hess.
+template <class F, class = void> struct SsFoldHasHessian : std::false_type {};
+template <class F> struct SsFoldHasHessian<F, std::void_t<decltype(&F::hessian)>> : std::true_type {};
+
+// W'(r) / r and W''(r) of ss_kernel_scalar from the same constants, with s2 = (2 / h)^2: W' / r = sigma s2 f'(q) / q, f' / q =
+// c_inner (1.5 q - 2) below 1 (no division: finite at r = 0), -3 c_outer (2 - q)^2 / q below 2; W'' = sigma s2 f''(q), f'' =
+// c_inner (3 q - 2) below 1, 6 c_outer (2 - q) below 2 (continuous at q = 1 and 2); both 0 beyond
+__device__ __forceinline__ void ss_kernel_scalar_d2(const SsDev &P, float r, float &w1r, float &w2) {
+    const float q = __fdiv_rn(__fadd_rn(r, r), P.h);
+    const float t = __fdiv_rn(2.0f, P.h), s2 = __fmul_rn(t, t);
+    float f1q, f2;
+    if (q < 1.0f) {
+        f1q = __fmul_rn(P.s_c_inner, __fsub_rn(__fmul_rn(1.5f, q), 2.0f));
+        f2 = __fmul_rn(P.s_c_inner, __fsub_rn(__fmul_rn(3.0f, q), 2.0f));
+    } else if (q < 2.0f) {
+        const float x = __fsub_rn(2.0f, q);
+        f1q = __fdiv_rn(__fmul_rn(__fmul_rn(__fmul_rn(-3.0f, P.s_c_outer), x), x), q);
+        f2 = __fmul_rn(__fmul_rn(6.0f, P.s_c_outer), x);
+    } else { f1q = 0.0f; f2 = 0.0f; }
+    w1r = __fmul_rn(__fmul_rn(P.s_sigma, f1q), s2);
+    w2 = __fmul_rn(__fmul_rn(P.s_sigma, f2), s2);
+}
+
+// H += a v v^T + b K (K symmetric, entries xx xy xz yy yz zz): per entry t = (a v_i) v_j + b K_ij, then H_ij + t
+__device__ __forceinline__ void ss_hess_rank1(float (&H)[6], float a, const float (&v)[3], float b, const float (&K)[6]) {
+    const int I[6] = { 0, 0, 0, 1, 1, 2 }, J[6] = { 0, 1, 2, 1, 2, 2 };
+#pragma unroll
+    for (int e = 0; e < 6; ++e) H[e] = __fadd_rn(H[e], __fadd_rn(__fmul_rn(__fmul_rn(a, v[I[e]]), v[J[e]]), __fmul_rn(b, K[e])));
+}
+
+// H phi = sum_j V_j [ (W'' - W'/r) / r^2 d d^T + (W'/r) I ] over SsSphFold's candidates (d2 < 1.01 h^2); at d2 == 0 only the I term
+struct SsSphHessFold {
+    using Cand = SsSphFold::Cand;
+    struct Acc { SsSphGradFold::Acc g; float H[6]; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsSphFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsSphGradFold::zero(), { 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f } }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsSphGradFold::add(P, c, gx, gy, gz, a.g);
+        const float d[3] = { __fsub_rn(c.r.x, gx), __fsub_rn(c.r.y, gy), __fsub_rn(c.r.z, gz) };
+        const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2]));
+        if (!(d2 < P.h2m)) return;
+        float w1r, w2;
+        ss_kernel_scalar_d2(P, __fsqrt_rn(d2), w1r, w2);
+        const float ra = d2 == 0.0f ? 0.0f : __fdiv_rn(__fmul_rn(c.r.w, __fsub_rn(w2, w1r)), d2);
+        const float I6[6] = { 1.0f, 0.0f, 0.0f, 1.0f, 0.0f, 1.0f };
+        ss_hess_rank1(a.H, ra, d, __fmul_rn(c.r.w, w1r), I6);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsSphGradFold::value(P, a.g); }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) { SsSphGradFold::gradient(P, a.g, g); }
+    static __device__ __forceinline__ void hessian(const SsDev &, const Acc &a, float (&H)[6]) {
+#pragma unroll
+        for (int e = 0; e < 6; ++e) H[e] = a.H[e];
+    }
+};
+
+// H phi = sum_j (V_j det G_j) [ (W'' - W'/|u|) / |u|^2 (G u)(G u)^T + (W'/|u|) G^2 ], u = G d as in SsAnisoGradFold; candidates
+// |u|^2 < h^2, at |u| == 0 only the G^2 term
+struct SsAnisoHessFold {
+    using Cand = SsAnisoFold::Cand;
+    struct Acc { SsAnisoGradFold::Acc g; float H[6]; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAnisoFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAnisoGradFold::zero(), { 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f } }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAnisoGradFold::add(P, c, gx, gy, gz, a.g);
+        const float4 g0 = c.g0, g1 = c.g1;
+        const float dx = __fsub_rn(c.r.x, gx), dy = __fsub_rn(c.r.y, gy), dz = __fsub_rn(c.r.z, gz);
+        const float u0 = __fadd_rn(__fadd_rn(__fmul_rn(g0.x, dx), __fmul_rn(g0.y, dy)), __fmul_rn(g0.z, dz));
+        const float u1 = __fadd_rn(__fadd_rn(__fmul_rn(g0.y, dx), __fmul_rn(g0.w, dy)), __fmul_rn(g1.x, dz));
+        const float u2 = __fadd_rn(__fadd_rn(__fmul_rn(g0.z, dx), __fmul_rn(g1.x, dy)), __fmul_rn(g1.y, dz));
+        const float uu = __fadd_rn(__fadd_rn(__fmul_rn(u0, u0), __fmul_rn(u1, u1)), __fmul_rn(u2, u2));
+        if (!(uu < P.h2)) return;
+        float w1r, w2;
+        ss_kernel_scalar_d2(P, __fsqrt_rn(uu), w1r, w2);
+        const float ra = uu == 0.0f ? 0.0f : __fdiv_rn(__fmul_rn(c.r.w, __fsub_rn(w2, w1r)), uu);
+        const float v[3] = { __fadd_rn(__fadd_rn(__fmul_rn(g0.x, u0), __fmul_rn(g0.y, u1)), __fmul_rn(g0.z, u2)),
+                             __fadd_rn(__fadd_rn(__fmul_rn(g0.y, u0), __fmul_rn(g0.w, u1)), __fmul_rn(g1.x, u2)),
+                             __fadd_rn(__fadd_rn(__fmul_rn(g0.z, u0), __fmul_rn(g1.x, u1)), __fmul_rn(g1.y, u2)) };
+        // G^2 = G G: ((G_i0 G_0j + G_i1 G_1j) + G_i2 G_2j)
+        const float G[3][3] = { { g0.x, g0.y, g0.z }, { g0.y, g0.w, g1.x }, { g0.z, g1.x, g1.y } };
+        const int I[6] = { 0, 0, 0, 1, 1, 2 }, J[6] = { 0, 1, 2, 1, 2, 2 };
+        float K[6];
+#pragma unroll
+        for (int e = 0; e < 6; ++e)
+            K[e] = __fadd_rn(__fadd_rn(__fmul_rn(G[I[e]][0], G[0][J[e]]), __fmul_rn(G[I[e]][1], G[1][J[e]])), __fmul_rn(G[I[e]][2], G[2][J[e]]));
+        ss_hess_rank1(a.H, ra, v, __fmul_rn(c.r.w, w1r), K);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAnisoGradFold::value(P, a.g); }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) { SsAnisoGradFold::gradient(P, a.g, g); }
+    static __device__ __forceinline__ void hessian(const SsDev &, const Acc &a, float (&H)[6]) {
+#pragma unroll
+        for (int e = 0; e < 6; ++e) H[e] = a.H[e];
+    }
+};
+
+// The sums the averaged Hessian adds to §12.1's, with b = 1 - |d|^2 / h^2 over |d|^2 < h^2: S2 = sum b^2, N = sum b d d^T (xx xy xz
+// yy yz zz), O = sum b d (x) d (x) d (xxx xxy xxz xyy xyz xzz yyy yyz yzz zzz); per candidate e = b d, n_ab = e_a d_b, o_abc = n_ab d_c.
+struct SsAvgHessSums { float s2, n[6], o[10]; };
+__device__ __forceinline__ void ss_avg_hess_sums(const float (&d)[3], float u, SsAvgHessSums &e) {
+    e.s2 = __fadd_rn(e.s2, __fmul_rn(u, u));
+    const float ed[3] = { __fmul_rn(u, d[0]), __fmul_rn(u, d[1]), __fmul_rn(u, d[2]) };
+    const float n[6] = { __fmul_rn(ed[0], d[0]), __fmul_rn(ed[0], d[1]), __fmul_rn(ed[0], d[2]),
+                         __fmul_rn(ed[1], d[1]), __fmul_rn(ed[1], d[2]), __fmul_rn(ed[2], d[2]) };
+#pragma unroll
+    for (int i = 0; i < 6; ++i) e.n[i] = __fadd_rn(e.n[i], n[i]);
+    const float o[10] = { __fmul_rn(n[0], d[0]), __fmul_rn(n[0], d[1]), __fmul_rn(n[0], d[2]), __fmul_rn(n[1], d[1]), __fmul_rn(n[1], d[2]),
+                          __fmul_rn(n[2], d[2]), __fmul_rn(n[3], d[1]), __fmul_rn(n[3], d[2]), __fmul_rn(n[4], d[2]), __fmul_rn(n[5], d[2]) };
+#pragma unroll
+    for (int i = 0; i < 10; ++i) e.o[i] = __fadd_rn(e.o[i], o[i]);
+}
+
+// d, |d|^2 and b of a candidate of the averaged folds; false outside the support
+__device__ __forceinline__ bool ss_avg_offset(const SsDev &P, float4 r, float gx, float gy, float gz, float (&d)[3], float &u) {
+    d[0] = __fsub_rn(r.x, gx); d[1] = __fsub_rn(r.y, gy); d[2] = __fsub_rn(r.z, gz);
+    const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2]));
+    if (!(d2 < P.h2)) return false;
+    u = __fsub_rn(1.0f, __fdiv_rn(d2, P.h2));
+    return true;
+}
+
+// f = h - |m|: H f = -sum_a mh_a H m_a - (I - J)^T (I - mh mh^T) (I - J) / |m|, mh = m / |m|, J = (k / S)(M - m T^T), k = 6 / h^2,
+// which DESIGN.md §13.2 reduces to
+//   H f = -(k / S) [ A + sig I - T c^T - c T^T ] - (B^T B - g g^T) / |m|
+// with B = I - J, g = B^T mh = grad f (SsAvgGradFold::grad_f, bit for bit), c = J^T mh, A = (4 / h^2)(sum_a mh_a O_a.. - |m| N),
+// sig = |m| S2 - mh . T.  0 where !(S > 0) or |m| == 0.
+struct SsAvgHessFold {
+    using Cand = SsAvgFold::Cand;
+    struct Acc { SsAvgGradFold::Acc g; SsAvgHessSums e; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgGradFold::zero(), SsAvgHessSums{} }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgGradFold::add(P, c, gx, gy, gz, a.g);
+        float d[3], u;
+        if (ss_avg_offset(P, c.r, gx, gy, gz, d, u)) ss_avg_hess_sums(d, u, a.e);
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAvgGradFold::value(P, a.g); }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) { SsAvgGradFold::gradient(P, a.g, g); }
+    static __device__ __forceinline__ void hess_f(const SsDev &P, const SsAvgGradFold::Acc &a, const SsAvgHessSums &e, float (&H)[6]) {
+#pragma unroll
+        for (int i = 0; i < 6; ++i) H[i] = 0.0f;
+        float g[3];
+        const float nm = SsAvgGradFold::grad_f(P, a, g);
+        if (nm == 0.0f) return;                              // also !(S > 0)
+        const float s = a.a.s;
+        const float m[3] = { __fdiv_rn(a.a.x, s), __fdiv_rn(a.a.y, s), __fdiv_rn(a.a.z, s) };
+        const float mh[3] = { __fdiv_rn(m[0], nm), __fdiv_rn(m[1], nm), __fdiv_rn(m[2], nm) };
+        const float k = __fdiv_rn(6.0f, P.h2), kh = __fdiv_rn(4.0f, P.h2);
+        const float M[3][3] = { { a.mxx, a.mxy, a.mxz }, { a.mxy, a.myy, a.myz }, { a.mxz, a.myz, a.mzz } };
+        const float T[3] = { a.tx, a.ty, a.tz };
+        float J[3][3], B[3][3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                J[i][j] = __fdiv_rn(__fmul_rn(k, __fsub_rn(M[i][j], __fmul_rn(m[i], T[j]))), s);
+                B[i][j] = __fsub_rn(i == j ? 1.0f : 0.0f, J[i][j]);
+            }
+        }
+        float cv[3];                                         // c = J^T mh
+#pragma unroll
+        for (int j = 0; j < 3; ++j) cv[j] = __fadd_rn(__fadd_rn(__fmul_rn(J[0][j], mh[0]), __fmul_rn(J[1][j], mh[1])), __fmul_rn(J[2][j], mh[2]));
+        const float sig = __fsub_rn(__fmul_rn(nm, e.s2), __fadd_rn(__fadd_rn(__fmul_rn(mh[0], T[0]), __fmul_rn(mh[1], T[1])), __fmul_rn(mh[2], T[2])));
+        // O_aij of the six (i, j) entries for a = x, y, z (indices into SsAvgHessSums::o)
+        const int OX[6] = { 0, 1, 2, 3, 4, 5 }, OY[6] = { 1, 3, 4, 6, 7, 8 }, OZ[6] = { 2, 4, 5, 7, 8, 9 };
+        const int I[6] = { 0, 0, 0, 1, 1, 2 }, Jx[6] = { 0, 1, 2, 1, 2, 2 };
+#pragma unroll
+        for (int q = 0; q < 6; ++q) {
+            const int i = I[q], j = Jx[q];
+            const float om = __fadd_rn(__fadd_rn(__fmul_rn(e.o[OX[q]], mh[0]), __fmul_rn(e.o[OY[q]], mh[1])), __fmul_rn(e.o[OZ[q]], mh[2]));
+            float p = __fmul_rn(kh, __fsub_rn(om, __fmul_rn(nm, e.n[q])));
+            if (i == j) p = __fadd_rn(p, sig);
+            p = __fsub_rn(__fsub_rn(p, __fmul_rn(T[i], cv[j])), __fmul_rn(cv[i], T[j]));
+            const float first = __fdiv_rn(__fmul_rn(k, p), s);
+            const float bb = __fadd_rn(__fadd_rn(__fmul_rn(B[0][i], B[0][j]), __fmul_rn(B[1][i], B[1][j])), __fmul_rn(B[2][i], B[2][j]));
+            const float second = __fdiv_rn(__fsub_rn(bb, __fmul_rn(g[i], g[j])), nm);
+            H[q] = -__fadd_rn(first, second);
+        }
+    }
+    static __device__ __forceinline__ void hessian(const SsDev &P, const Acc &a, float (&H)[6]) { hess_f(P, a.g, a.e, H); }
+};
+
+// With radii: v = f + R, R = Q / S: H v = H f + (k / S) [ (4 / h^2)(Nd - R N) + (R S2 - S2d) I - T r^T - r T^T ] with r = grad R =
+// k (U - R T) / S (SsAvgRadGradFold's term), Nd = sum b delta d d^T, S2d = sum b^2 delta; the R part wherever S > 0.
+struct SsAvgRadHessFold {
+    using Cand = SsAvgRadFold::Cand;
+    struct Acc { SsAvgRadGradFold::Acc g; SsAvgHessSums e; float s2d, nd[6]; };
+    static __device__ __forceinline__ Cand load(const SsAnArgs &A, uint32_t src) { return SsAvgRadFold::load(A, src); }
+    static __device__ __forceinline__ Acc zero() { return Acc{ SsAvgRadGradFold::zero(), SsAvgHessSums{}, 0.0f, { 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f } }; }
+    static __device__ __forceinline__ void add(const SsDev &P, const Cand &c, float gx, float gy, float gz, Acc &a) {
+        SsAvgRadGradFold::add(P, c, gx, gy, gz, a.g);
+        float d[3], u;
+        if (!ss_avg_offset(P, c.c.r, gx, gy, gz, d, u)) return;
+        ss_avg_hess_sums(d, u, a.e);
+        const float ud = __fmul_rn(u, c.delta);
+        a.s2d = __fadd_rn(a.s2d, __fmul_rn(u, ud));
+        const float ed[3] = { __fmul_rn(ud, d[0]), __fmul_rn(ud, d[1]), __fmul_rn(ud, d[2]) };
+        const int I[6] = { 0, 0, 0, 1, 1, 2 }, J[6] = { 0, 1, 2, 1, 2, 2 };
+#pragma unroll
+        for (int q = 0; q < 6; ++q) a.nd[q] = __fadd_rn(a.nd[q], __fmul_rn(ed[I[q]], d[J[q]]));
+    }
+    static __device__ __forceinline__ float value(const SsDev &P, const Acc &a) { return SsAvgRadGradFold::value(P, a.g); }
+    static __device__ __forceinline__ void gradient(const SsDev &P, const Acc &a, float (&g)[3]) { SsAvgRadGradFold::gradient(P, a.g, g); }
+    static __device__ __forceinline__ void hessian(const SsDev &P, const Acc &a, float (&H)[6]) {
+        SsAvgHessFold::hess_f(P, a.g.a, a.e, H);
+        const float s = a.g.a.a.s;
+        if (!(s > 0.0f)) return;
+        const float k = __fdiv_rn(6.0f, P.h2), kh = __fdiv_rn(4.0f, P.h2), R = __fdiv_rn(a.g.q, s);
+        const float U[3] = { a.g.ux, a.g.uy, a.g.uz }, T[3] = { a.g.a.tx, a.g.a.ty, a.g.a.tz };
+        float r[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r[i] = __fdiv_rn(__fmul_rn(k, __fsub_rn(U[i], __fmul_rn(R, T[i]))), s);
+        const float dg = __fsub_rn(__fmul_rn(R, a.e.s2), a.s2d);
+        const int I[6] = { 0, 0, 0, 1, 1, 2 }, J[6] = { 0, 1, 2, 1, 2, 2 };
+#pragma unroll
+        for (int q = 0; q < 6; ++q) {
+            const int i = I[q], j = J[q];
+            float p = __fmul_rn(kh, __fsub_rn(a.nd[q], __fmul_rn(R, a.e.n[q])));
+            if (i == j) p = __fadd_rn(p, dg);
+            p = __fsub_rn(__fsub_rn(p, __fmul_rn(T[i], r[j])), __fmul_rn(r[i], T[j]));
+            H[q] = __fadd_rn(H[q], __fdiv_rn(__fmul_rn(k, p), s));
+        }
+    }
+};
+
+// Curvature of the level set through p from g = grad phi and H (DESIGN.md §13.2): n = g / |g|, kappa_H = -(tr H - n^T H n) / (2 |g|)
+// (half the divergence of the outward normal -g / |g|), kappa_G = n^T adj(H) n / |g|^2; both NaN where |g|^2 rounds to 0.
+__device__ __forceinline__ void ss_curvature(const float (&g)[3], const float (&H)[6], float &kh, float &kg) {
+    const float g2 = __fadd_rn(__fadd_rn(__fmul_rn(g[0], g[0]), __fmul_rn(g[1], g[1])), __fmul_rn(g[2], g[2]));
+    if (g2 == 0.0f) { kh = __int_as_float(0x7fc00000); kg = kh; return; }
+    const float ng = __fsqrt_rn(g2);
+    const float n[3] = { __fdiv_rn(g[0], ng), __fdiv_rn(g[1], ng), __fdiv_rn(g[2], ng) };
+    const float M[3][3] = { { H[0], H[1], H[2] }, { H[1], H[3], H[4] }, { H[2], H[4], H[5] } };
+    // adj(H) of the symmetric H: cofactors, e.g. adj_xx = Hyy Hzz - Hyz Hyz, adj_xy = Hxz Hyz - Hxy Hzz
+    const float A[3][3] = {
+        { __fsub_rn(__fmul_rn(H[3], H[5]), __fmul_rn(H[4], H[4])), __fsub_rn(__fmul_rn(H[2], H[4]), __fmul_rn(H[1], H[5])),
+          __fsub_rn(__fmul_rn(H[1], H[4]), __fmul_rn(H[2], H[3])) },
+        { 0.0f, __fsub_rn(__fmul_rn(H[0], H[5]), __fmul_rn(H[2], H[2])), __fsub_rn(__fmul_rn(H[1], H[2]), __fmul_rn(H[0], H[4])) },
+        { 0.0f, 0.0f, __fsub_rn(__fmul_rn(H[0], H[3]), __fmul_rn(H[1], H[1])) } };
+    const float As[3][3] = { { A[0][0], A[0][1], A[0][2] }, { A[0][1], A[1][1], A[1][2] }, { A[0][2], A[1][2], A[2][2] } };
+    float hn[3], an[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        hn[i] = __fadd_rn(__fadd_rn(__fmul_rn(M[i][0], n[0]), __fmul_rn(M[i][1], n[1])), __fmul_rn(M[i][2], n[2]));
+        an[i] = __fadd_rn(__fadd_rn(__fmul_rn(As[i][0], n[0]), __fmul_rn(As[i][1], n[1])), __fmul_rn(As[i][2], n[2]));
+    }
+    const float nHn = __fadd_rn(__fadd_rn(__fmul_rn(n[0], hn[0]), __fmul_rn(n[1], hn[1])), __fmul_rn(n[2], hn[2]));
+    const float nAn = __fadd_rn(__fadd_rn(__fmul_rn(n[0], an[0]), __fmul_rn(n[1], an[1])), __fmul_rn(n[2], an[2]));
+    const float tr = __fadd_rn(__fadd_rn(H[0], H[3]), H[5]);
+    kh = -__fdiv_rn(__fsub_rn(tr, nHn), __fmul_rn(2.0f, ng));
+    kg = __fdiv_rn(nAn, g2);
+}
+
+// (kappa_H, kappa_G) of m points from their gradients [m][3] and Hessians [m][6]
+__global__ void k_field_curvature(const float *__restrict__ grad, const float *__restrict__ hess, uint32_t m, float *__restrict__ curv) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const float g[3] = { grad[3 * (size_t)i], grad[3 * (size_t)i + 1], grad[3 * (size_t)i + 2] };
+    float H[6];
+#pragma unroll
+    for (int e = 0; e < 6; ++e) H[e] = hess[6 * (size_t)i + e];
+    float kh, kg;
+    ss_curvature(g, H, kh, kg);
+    curv[2 * (size_t)i] = kh; curv[2 * (size_t)i + 1] = kg;
+}
+
 struct SsFieldArgs {
     SsAnArgs A;                        // the mode's records (A.bins.brick_rng: the field's candidate ranges); bricks / tiles unused
     const float *pts;                  // [m][3] query points
@@ -181,9 +452,10 @@ struct SsFieldArgs {
     float *out;                        // [m] pre-zeroed
     uint32_t *fallback;                // groups left to the next tier: [0] = count, [1..] = group indices
     float *grad;                       // [m][3] pre-zeroed, written by gradient folds only
+    float *hess;                       // [m][6] pre-zeroed, written by Hessian folds only
 };
 
-// the value of a point, and its gradient when the fold has one
+// the value of a point, and its gradient and Hessian when the fold has them
 template <class F>
 __device__ __forceinline__ void ss_field_store(const SsDev &P, const SsFieldArgs &Q, uint32_t dst, const typename F::Acc &acc) {
     Q.out[dst] = F::value(P, acc);
@@ -191,6 +463,12 @@ __device__ __forceinline__ void ss_field_store(const SsDev &P, const SsFieldArgs
         float g[3];
         F::gradient(P, acc, g);
         Q.grad[3 * (size_t)dst] = g[0]; Q.grad[3 * (size_t)dst + 1] = g[1]; Q.grad[3 * (size_t)dst + 2] = g[2];
+    }
+    if constexpr (SsFoldHasHessian<F>::value) {
+        float H[6];
+        F::hessian(P, acc, H);
+#pragma unroll
+        for (int e = 0; e < 6; ++e) Q.hess[6 * (size_t)dst + e] = H[e];
     }
 }
 

@@ -150,7 +150,7 @@ struct ss_context {
     DevBuf av_radii, av_delta, av_rrec, av_chk;      // per-particle radii: the caller's copy, delta_j (filtered), per membership, check
     // level-set field queries (ss_field.cuh): points, group keys and caller indices (sorted and not), group starts, values, checks,
     // and the candidate bin ranges of a group
-    DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng, fld_grad;
+    DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng, fld_grad, fld_hess, fld_curv;
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
@@ -2120,10 +2120,11 @@ static void field_fold(ss_context *c, const SsDev &D, const SsFieldArgs &Q0, uin
     }, launches, received);
 }
 
-// The field at m device-resident points `pts` into `out` (and, with `grad`, the gradient fold into grad, pre-zeroed): keys, sort,
-// group starts, then the cascade of the mode's value fold or gradient fold.  Uses the context's query scratch (fld_key_*, fld_idx_*,
-// fld_flag, fld_off, fld_starts, fld_chk), never the field's records.  Returns the refusal of a non-finite point.
-static int field_run(ss_surface *f, ss_context *c, const float *pts, uint32_t m32, float *out, float *grad) {
+// The field at m device-resident points `pts` into `out` (and, with `grad`, the gradient fold into grad, pre-zeroed; with `grad` and
+// `hess`, the Hessian fold into both, pre-zeroed): keys, sort, group starts, then the cascade of the mode's value, gradient or
+// Hessian fold.  Uses the context's query scratch (fld_key_*, fld_idx_*, fld_flag, fld_off, fld_starts, fld_chk), never the field's
+// records.  Returns the refusal of a non-finite point.
+static int field_run(ss_surface *f, ss_context *c, const float *pts, uint32_t m32, float *out, float *grad, float *hess = nullptr) {
     cudaStream_t st = c->stream;
     const SsDev &D = f->fld_D;
     c->fld_chk.ensure(8);
@@ -2155,7 +2156,15 @@ static int field_run(ss_surface *f, ss_context *c, const float *pts, uint32_t m3
     Q.A.grec = c->an_grec.as<float4>(); Q.A.rrec = c->av_rrec.as<float>();
     Q.pts = pts; Q.key = c->fld_key_b.as<uint32_t>(); Q.idx = c->fld_idx_b.as<uint32_t>();
     Q.starts = c->fld_starts.as<uint32_t>(); Q.out = out;
-    if (grad) {
+    if (hess) {
+        Q.grad = grad; Q.hess = hess;
+        switch (f->fld_mode) {
+        case SS_FLD_ANISO: field_fold<SsAnisoHessFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG: field_fold<SsAvgHessFold>(c, D, Q, n_groups, f->fld_paths); break;
+        case SS_FLD_AVG_RAD: field_fold<SsAvgRadHessFold>(c, D, Q, n_groups, f->fld_paths); break;
+        default: field_fold<SsSphHessFold>(c, D, Q, n_groups, f->fld_paths); break;
+        }
+    } else if (grad) {
         Q.grad = grad;
         switch (f->fld_mode) {
         case SS_FLD_ANISO: field_fold<SsAnisoGradFold>(c, D, Q, n_groups, f->fld_paths); break;
@@ -2176,15 +2185,23 @@ static int field_run(ss_surface *f, ss_context *c, const float *pts, uint32_t m3
     return SS_OK;
 }
 
-// One query of ss_levelset_field_at_f32 or (gradient) ss_levelset_field_gradient_at_f32: the caller's points copied to the device,
-// field_run, the results copied back.
-static int field_query(ss_surface *f, const float *points, uint64_t m, float *out, bool gradient, float *grads) {
+// What one field query returns beside the values
+enum FieldQuery { FQ_VALUE, FQ_GRADIENT, FQ_HESSIAN, FQ_CURVATURE };
+
+// One query of ss_levelset_field_at_f32, ss_levelset_field_gradient_at_f32 (grads: [m][3]), ss_levelset_field_hessian_at_f32 (grads,
+// hess: [m][6]) or ss_levelset_field_curvature_at_f32 (curv: [m][2]; gradients and Hessians in the context's buffers): the caller's
+// points copied to the device, field_run, the curvature epilogue, the results copied back.
+static int field_query(ss_surface *f, const float *points, uint64_t m, float *out, FieldQuery kind, float *grads, float *hess, float *curv) {
     int rc; ss_context *c = field_context(f, &rc);
     if (!c) return rc;
-    if (m && (!points || !out || (gradient && !grads))) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    if (m && (!points || !out || ((kind == FQ_GRADIENT || kind == FQ_HESSIAN) && !grads) || (kind == FQ_HESSIAN && !hess) ||
+              (kind == FQ_CURVATURE && !curv)))
+        return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
     if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many points for one call");
-    if (gradient && (f->fld_mode == SS_FLD_AVG_CORR || f->fld_mode == SS_FLD_AVG_CORR_RAD))
+    if (kind == FQ_GRADIENT && (f->fld_mode == SS_FLD_AVG_CORR || f->fld_mode == SS_FLD_AVG_CORR_RAD))
         return ss_fail(SS_ERR_UNSUPPORTED, "level-set field: the Jacobian-corrected averaged surface has no gradient (DESIGN.md 13.1)");
+    if (kind >= FQ_HESSIAN && (f->fld_mode == SS_FLD_AVG_CORR || f->fld_mode == SS_FLD_AVG_CORR_RAD))
+        return ss_fail(SS_ERR_UNSUPPORTED, "level-set field: the Jacobian-corrected averaged surface has no Hessian or curvature (DESIGN.md 13.2)");
     for (uint64_t &q : f->fld_paths) q = 0;
     if (!m) return SS_OK;
     return ss_guard([&]() -> int {
@@ -2192,26 +2209,45 @@ static int field_query(ss_surface *f, const float *points, uint64_t m, float *ou
         cudaStream_t st = c->stream;
         const uint32_t m32 = (uint32_t)m;
         c->fld_pts.ensure((size_t)m32 * 12); c->fld_out.ensure((size_t)m32 * 4);
-        if (gradient) {
+        if (kind != FQ_VALUE) {
             c->fld_grad.ensure((size_t)m32 * 12);
             CK(cudaMemsetAsync(c->fld_grad.p, 0, (size_t)m32 * 12, st));       // points without candidates: gradient 0
         }
+        if (kind >= FQ_HESSIAN) {
+            c->fld_hess.ensure((size_t)m32 * 24);
+            CK(cudaMemsetAsync(c->fld_hess.p, 0, (size_t)m32 * 24, st));       // and Hessian 0
+        }
         CK(cudaMemcpyAsync(c->fld_pts.p, points, (size_t)m32 * 12, cudaMemcpyDefault, st));
-        const int rc = field_run(f, c, c->fld_pts.as<float>(), m32, c->fld_out.as<float>(), gradient ? c->fld_grad.as<float>() : nullptr);
+        const int rc = field_run(f, c, c->fld_pts.as<float>(), m32, c->fld_out.as<float>(), kind != FQ_VALUE ? c->fld_grad.as<float>() : nullptr,
+                                 kind >= FQ_HESSIAN ? c->fld_hess.as<float>() : nullptr);
         if (rc) return rc;
         CK(cudaMemcpyAsync(out, c->fld_out.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
-        if (gradient) CK(cudaMemcpyAsync(grads, c->fld_grad.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        if (kind == FQ_GRADIENT || kind == FQ_HESSIAN) CK(cudaMemcpyAsync(grads, c->fld_grad.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        if (kind == FQ_HESSIAN) CK(cudaMemcpyAsync(hess, c->fld_hess.p, (size_t)m32 * 24, cudaMemcpyDefault, st));
+        if (kind == FQ_CURVATURE) {
+            c->fld_curv.ensure((size_t)m32 * 8);
+            LAUNCH(c, k_field_curvature, nblk(m32, 256), 256, c->fld_grad.as<float>(), c->fld_hess.as<float>(), m32, c->fld_curv.as<float>());
+            CK(cudaMemcpyAsync(curv, c->fld_curv.p, (size_t)m32 * 8, cudaMemcpyDefault, st));
+        }
         CK(cudaStreamSynchronize(st));
         return SS_OK;
     });
 }
 
 extern "C" int ss_levelset_field_at_f32(ss_surface *f, const float *points, uint64_t m, float *out) {
-    return field_query(f, points, m, out, false, nullptr);
+    return field_query(f, points, m, out, FQ_VALUE, nullptr, nullptr, nullptr);
 }
 
 extern "C" int ss_levelset_field_gradient_at_f32(ss_surface *f, const float *points, uint64_t m, float *values, float *gradients) {
-    return field_query(f, points, m, values, true, gradients);
+    return field_query(f, points, m, values, FQ_GRADIENT, gradients, nullptr, nullptr);
+}
+
+extern "C" int ss_levelset_field_hessian_at_f32(ss_surface *f, const float *points, uint64_t m, float *values, float *gradients, float *hessians) {
+    return field_query(f, points, m, values, FQ_HESSIAN, gradients, hessians, nullptr);
+}
+
+extern "C" int ss_levelset_field_curvature_at_f32(ss_surface *f, const float *points, uint64_t m, float *values, float *curvatures) {
+    return field_query(f, points, m, values, FQ_CURVATURE, nullptr, nullptr, curvatures);
 }
 
 extern "C" int ss_levelset_field_threshold_f32(const ss_surface *f, float *threshold) {

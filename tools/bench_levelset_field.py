@@ -15,6 +15,10 @@ gradient query (LevelSetField.gradient, §13.1) on the same points, the two alte
     python tools/bench_levelset_field.py                         # cfg-4: the 50 M-particle dam break
     python tools/bench_levelset_field.py --particles 1000000 --points 1000000
     python tools/bench_levelset_field.py --gradient              # value and gradient queries side by side
+    python tools/bench_levelset_field.py --hessian               # value, gradient, Hessian and curvature queries side by side
+
+With `--hessian` (implies `--gradient`) the Hessian (LevelSetField.hessian, §13.2) and curvature (LevelSetField.curvature) queries
+are timed as well, the four alternating call by call.
 """
 import argparse
 import json
@@ -44,7 +48,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--modes", default="standard,anisotropic,averaged,averaged_corrected,averaged_radii,averaged_corrected_radii")
     ap.add_argument("--gradient", action="store_true", help="also time the gradient query (modes with a gradient only)")
+    ap.add_argument("--hessian", action="store_true", help="also time the gradient, Hessian and curvature queries (modes with a Hessian only)")
     a = ap.parse_args()
+    a.gradient = a.gradient or a.hessian
     import numpy as np
     import torch
     import splashsurf_b200 as ss
@@ -58,7 +64,6 @@ def main():
              "averaged_corrected": dict(averaged_surface=ss.AveragedSurface(correction=corr)),
              "averaged_radii": dict(averaged_surface=ss.AveragedSurface(), particle_radii=radii),
              "averaged_corrected_radii": dict(averaged_surface=ss.AveragedSurface(correction=corr), particle_radii=radii)}
-    ctx = ss.Context(0)
     out = {"tool": "bench_levelset_field", "particles": len(x), "workload": "dam break, r = 0.01, -l 2, -c 0.5", "card_before": card_before,
            "steps": a.steps, "warmup": a.warmup, "runs": []}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -84,6 +89,8 @@ def main():
         near = (verts + rng.uniform(-1, 1, verts.shape).astype(np.float32) * c).astype(np.float32)
         del rec
         rctx.close()
+        # the field's query scratch grows with the largest point set and stays with its context: one context per mode
+        ctx = ss.Context(0)
         t0 = time.perf_counter()
         f = ss.LevelSetField(x, context=ctx, **kw, **mk)
         create_ms = (time.perf_counter() - t0) * 1e3
@@ -98,38 +105,53 @@ def main():
         for name, pts in sets.items():
             dev = torch.from_numpy(pts).cuda()
             torch.cuda.synchronize()
+            extra = {"gradient": f.gradient} if a.gradient else {}
+            if a.hessian:
+                extra.update(hessian=f.hessian, curvature=f.curvature)
             for _ in range(a.warmup):
                 v = f.evaluate(dev)
-                if a.gradient:
-                    f.gradient(dev)
-            ms, gms = [], []
+                for call in extra.values():
+                    call(dev)
+            ms, xms = [], {k: [] for k in extra}
             for _ in range(a.steps):
                 ev0.record()
                 v = f.evaluate(dev)
                 ev1.record()
                 torch.cuda.synchronize()
                 ms.append(ev0.elapsed_time(ev1))
-                if a.gradient:
+                for k, call in extra.items():
                     ev0.record()
-                    gv, g = f.gradient(dev)
+                    r = call(dev)
                     ev1.record()
                     torch.cuda.synchronize()
-                    gms.append(ev0.elapsed_time(ev1))
+                    xms[k].append(ev0.elapsed_time(ev1))
+                    if k == "gradient":
+                        gv, g = r
+                    elif k == "hessian":
+                        hv, hg = r[0], r[1]
+                    del r
             best = min(ms)
             q = {"points": len(pts), "ms": [round(t, 3) for t in ms], "ns_per_point": best * 1e6 / max(len(pts), 1),
                  "inside_fraction": float((v > f.threshold).sum()) / max(len(pts), 1), "paths": f.paths}
+            for k, t in xms.items():
+                q[f"{k}_ms"] = [round(x, 3) for x in t]
+                q[f"{k}_ns_per_point"] = min(t) * 1e6 / max(len(pts), 1)
             if a.gradient:
-                q.update(gradient_ms=[round(t, 3) for t in gms], gradient_ns_per_point=min(gms) * 1e6 / max(len(pts), 1),
-                         values_equal=bool(torch.equal(gv, v)), zero_gradient_fraction=float((g == 0).all(1).float().mean()))
+                q.update(values_equal=bool(torch.equal(gv, v)), zero_gradient_fraction=float((g == 0).all(1).float().mean()))
+            if a.hessian:
+                q.update(hessian_values_equal=bool(torch.equal(hv, v)), hessian_gradients_equal=bool(torch.equal(hg, g)))
+                del hv, hg
+            if a.gradient:
                 del gv, g
             run["queries"][name] = q
             del dev, v
         f.close()
+        ctx.close()
         out["runs"].append(run)
-        sys.stderr.write(f"{mode}: create {create_ms:.1f} ms, " + ", ".join(f"{k} {q['ns_per_point']:.2f} ns/pt" + (
-            f" (gradient {q['gradient_ns_per_point']:.2f})" if a.gradient else "") for k, q in run["queries"].items()) + "\n")
+        sys.stderr.write(f"{mode}: create {create_ms:.1f} ms, " + ", ".join(f"{k} {q['ns_per_point']:.2f} ns/pt" + "".join(
+            f" ({x} {q[x + '_ns_per_point']:.2f})" for x in ("gradient", "hessian", "curvature") if x + "_ns_per_point" in q)
+            for k, q in run["queries"].items()) + "\n")
     out["card_after"] = card()
-    ctx.close()
     print(json.dumps(out))
 
 
