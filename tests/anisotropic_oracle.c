@@ -206,6 +206,80 @@ static void an_recon_task(int64_t s, void *ctx, void **tls) {
     subdomain_mc(&jb->patches[s], phi, smin, sijk, S, jb->c, jb->thr, ev);
 }
 
+/* lib.rs:369-406 particle AABB filter (half-open contains_point; inside, when not NULL, receives the flags) and
+ * dense_subdomains.rs:89-244 initialize_parameters: the filtered particles, the grid and the subdomain grid.  Returns the error of
+ * grid_for_reconstruction; s->filtered is the caller's to free either way. */
+typedef struct { const float *xyz; float *filtered; uint64_t n; so_grid gg, sg; float h, c, margin, rest_mass; int64_t S; } an_setup;
+
+static int an_setup_new(an_setup *s, const float *xyz_in, uint64_t n_in, const so_params *p, uint8_t *inside) {
+    s->xyz = xyz_in; s->filtered = NULL; s->n = n_in;
+    if (p->has_particle_aabb) {
+        s->filtered = (float *)malloc(sizeof(float) * 3 * (n_in ? n_in : 1));
+        s->n = 0;
+        for (uint64_t i = 0; i < n_in; ++i) {
+            int in = 1;
+            for (int d = 0; d < 3; ++d) { float v = xyz_in[3 * i + d]; if (!(v >= p->aabb_min[d] && v < p->aabb_max[d])) in = 0; }
+            if (inside) inside[i] = (uint8_t)in;
+            if (in) { memcpy(s->filtered + 3 * s->n, xyz_in + 3 * i, sizeof(float) * 3); ++s->n; }
+        }
+        s->xyz = s->filtered;
+    }
+    so_grid g0;
+    int err = grid_for_reconstruction(&g0, s->xyz, s->n, p);
+    if (err) return err;
+    int64_t S = (int64_t)p->subdomain_num_cubes_per_dim;
+    float r2 = p->particle_radius + p->particle_radius;
+    s->S = S;
+    s->rest_mass = (r2 * r2 * r2) * p->rest_density;
+    s->h = p->compact_support_radius; s->c = p->cube_size;
+    s->margin = f_ceil(s->h / s->c) * s->c * 1.01f;
+    int64_t nsubd[3], ncg[3];
+    for (int d = 0; d < 3; ++d) { nsubd[d] = (g0.nc[d] + S - 1) / S; ncg[d] = nsubd[d] * S; }
+    grid_new(&s->gg, g0.aabb_min, ncg, s->c);
+    float sub_size = s->c * (float)S;
+    grid_new(&s->sg, s->gg.aabb_min, nsubd, sub_size);
+    return 0;
+}
+
+/* The densities (rho), then x_bar (n x 3), G (n x 6) and V det G (n) of the set-up particles, on the standard decomposition; g_an
+ * keeps pointing at them for the level set. */
+static void an_records(const an_setup *s, float smoothing, float max_stretch, uint32_t min_neighbors, float *rho, float *xbar, float *g,
+                       float *vdet) {
+    so_decomp dstd; decompose(&dstd, s->xyz, s->n, &s->sg, s->margin);
+    so_result res;
+    memset(&res, 0, sizeof(res));
+    res.densities = rho;
+    memset(rho, 0, sizeof(float) * s->n);
+    g_an.on = 1; g_an.lambda = smoothing; g_an.kr = max_stretch; g_an.min_nb = min_neighbors;
+    g_an.xbar = xbar; g_an.g = g; g_an.vdet = vdet;
+    an_job job;
+    memset(&job, 0, sizeof(job));
+    job.xyz = s->xyz; job.sg = &s->sg; job.gg = &s->gg; job.dstd = &dstd; job.res = &res;
+    job.h = s->h; job.c = s->c; job.margin = s->margin; job.rest_mass = s->rest_mass; job.S = s->S;
+    parallel_for((int64_t)dstd.nsub, an_density_task, &job);
+    for (uint64_t i = 0; i < s->n; ++i) {
+        for (int d = 0; d < 3; ++d) g_an.xbar[3 * i + d] = s->xyz[3 * i + d];
+        float id[6] = { 1, 0, 0, 1, 0, 1 };
+        memcpy(g_an.g + 6 * i, id, sizeof(id));
+        g_an.vdet[i] = 1.0f;
+    }
+    parallel_for((int64_t)dstd.nsub, an_aniso_task, &job);
+    for (uint64_t i = 0; i < s->n; ++i) g_an.vdet[i] = (s->rest_mass / rho[i]) * g_an.vdet[i];
+    free(dstd.flat); free(dstd.offset); free(dstd.members);
+}
+
+/* The records of the anisotropic level set as so_reconstruct_aniso computes them: the densities (rho_out), x_bar (xbar_out, n x 3),
+ * G (g_out, n x 6) and V det G (vdet_out) of the n filtered particles (buffers of n_in); returns n, or -(error code). */
+int64_t so_aniso_records(const float *xyz_in, uint64_t n_in, const so_params *p, float smoothing, float max_stretch, uint32_t min_neighbors,
+                         float *xbar_out, float *g_out, float *vdet_out, float *rho_out) {
+    an_setup s;
+    int err = an_setup_new(&s, xyz_in, n_in, p, NULL);
+    if (!err) an_records(&s, smoothing, max_stretch, min_neighbors, rho_out, xbar_out, g_out, vdet_out);
+    memset(&g_an, 0, sizeof(g_an));
+    free(s.filtered);
+    return err ? -(int64_t)err : (int64_t)s.n;
+}
+
 /* so_reconstruct with anisotropic kernels: always decomposed (decomposition == 0 -> 7, SS_ERR_UNSUPPORTED).  xbar_out (>= n_in x 3)
  * and g_out (>= n_in x 6: g00 g01 g02 g11 g12 g22) receive x_bar and G of the n_filtered particles; tile_out the level-set tile of
  * subdomain tile_sub_flat (or -1). */
@@ -215,80 +289,45 @@ int so_reconstruct_aniso(const float *xyz_in, uint64_t n_in, const so_params *p,
     *out = res;
     lut_init();
     if (p->decomposition != 1) return 7;
-    /* lib.rs:369-406 particle AABB filter (half-open contains_point) */
-    const float *xyz = xyz_in; float *filtered = NULL; uint64_t n = n_in;
-    if (p->has_particle_aabb) {
-        res->inside_aabb = (uint8_t *)malloc(n_in ? n_in : 1);
-        filtered = (float *)malloc(sizeof(float) * 3 * (n_in ? n_in : 1));
-        n = 0;
-        for (uint64_t i = 0; i < n_in; ++i) {
-            int in = 1;
-            for (int d = 0; d < 3; ++d) { float v = xyz_in[3 * i + d]; if (!(v >= p->aabb_min[d] && v < p->aabb_max[d])) in = 0; }
-            res->inside_aabb[i] = (uint8_t)in;
-            if (in) { memcpy(filtered + 3 * n, xyz_in + 3 * i, sizeof(float) * 3); ++n; }
-        }
-        xyz = filtered;
-    }
-    res->n_filtered = n;
-    so_grid g0;
-    int err = grid_for_reconstruction(&g0, xyz, n, p);
-    if (err) { free(filtered); return err; }
+    if (p->has_particle_aabb) res->inside_aabb = (uint8_t *)malloc(n_in ? n_in : 1);
+    an_setup s;
+    int err = an_setup_new(&s, xyz_in, n_in, p, res->inside_aabb);
+    res->n_filtered = s.n;
+    if (err) { free(s.filtered); return err; }
     res->used_decomposition = 1;
-    /* dense_subdomains.rs:89-244 initialize_parameters */
-    int64_t S = (int64_t)p->subdomain_num_cubes_per_dim;
-    float r2 = p->particle_radius + p->particle_radius;
-    float rest_mass = (r2 * r2 * r2) * p->rest_density;
-    float h = p->compact_support_radius, c = p->cube_size, thr = p->iso_surface_threshold;
-    float margin = f_ceil(h / c) * c * 1.01f;
-    int64_t nsubd[3], ncg[3];
-    for (int d = 0; d < 3; ++d) { nsubd[d] = (g0.nc[d] + S - 1) / S; ncg[d] = nsubd[d] * S; }
-    so_grid gg; grid_new(&gg, g0.aabb_min, ncg, c);
-    float sub_size = c * (float)S;
-    so_grid sg; grid_new(&sg, gg.aabb_min, nsubd, sub_size);
-    res->grid = gg; res->subdomain_grid = sg;
+    res->grid = s.gg; res->subdomain_grid = s.sg;
+    uint64_t n = s.n;
     /* memberships within 2h (kernel centres move by up to smoothing * h); densities and anisotropy on the standard margin */
-    so_decomp dc; decompose(&dc, xyz, n, &sg, f_ceil((2.0f * h) / c) * c * 1.01f);
-    so_decomp dstd; decompose(&dstd, xyz, n, &sg, margin);
+    so_decomp dc; decompose(&dc, s.xyz, n, &s.sg, f_ceil((2.0f * s.h) / s.c) * s.c * 1.01f);
     res->n_subdomains = dc.nsub;
     res->subdomain_flat = (int64_t *)malloc(sizeof(int64_t) * (dc.nsub ? dc.nsub : 1));
     res->subdomain_count = (uint64_t *)malloc(sizeof(uint64_t) * (dc.nsub ? dc.nsub : 1));
     res->subdomain_sparse = (uint8_t *)malloc(dc.nsub ? dc.nsub : 1);
     uint64_t maxp = 0;
-    for (uint64_t s = 0; s < dc.nsub; ++s) {
-        res->subdomain_flat[s] = dc.flat[s];
-        res->subdomain_count[s] = dc.offset[s + 1] - dc.offset[s];
-        if (res->subdomain_count[s] > maxp) maxp = res->subdomain_count[s];
+    for (uint64_t k = 0; k < dc.nsub; ++k) {
+        res->subdomain_flat[k] = dc.flat[k];
+        res->subdomain_count[k] = dc.offset[k + 1] - dc.offset[k];
+        if (res->subdomain_count[k] > maxp) maxp = res->subdomain_count[k];
     }
     res->max_particles = maxp; res->sparse_limit = maxp / 20 < 100 ? 100 : maxp / 20;
     res->densities = (float *)calloc(n ? n : 1, sizeof(float));
+    float *vdet = (float *)malloc(sizeof(float) * (n ? n : 1));
+    an_records(&s, smoothing, max_stretch, min_neighbors, res->densities, xbar_out, g_out, vdet);
 
-    g_an.on = 1; g_an.lambda = smoothing; g_an.kr = max_stretch; g_an.min_nb = min_neighbors;
-    g_an.xbar = xbar_out; g_an.g = g_out; g_an.vdet = (float *)malloc(sizeof(float) * (n ? n : 1));
     an_job job;
     memset(&job, 0, sizeof(job));
-    job.xyz = xyz; job.sg = &sg; job.gg = &gg; job.dc = &dc; job.dstd = &dstd; job.res = res;
-    job.h = h; job.c = c; job.thr = thr; job.margin = margin; job.rest_mass = rest_mass; job.S = S;
+    job.xyz = s.xyz; job.sg = &s.sg; job.gg = &s.gg; job.dc = &dc; job.res = res;
+    job.h = s.h; job.c = s.c; job.thr = p->iso_surface_threshold; job.margin = s.margin; job.rest_mass = s.rest_mass; job.S = s.S;
     job.tile_sub_flat = tile_sub_flat; job.tile_out = tile_out;
-    parallel_for((int64_t)dstd.nsub, an_density_task, &job);
-    for (uint64_t i = 0; i < n; ++i) {
-        for (int d = 0; d < 3; ++d) g_an.xbar[3 * i + d] = xyz[3 * i + d];
-        float id[6] = { 1, 0, 0, 1, 0, 1 };
-        memcpy(g_an.g + 6 * i, id, sizeof(id));
-        g_an.vdet[i] = 1.0f;
-    }
-    parallel_for((int64_t)dstd.nsub, an_aniso_task, &job);
-    for (uint64_t i = 0; i < n; ++i) g_an.vdet[i] = (rest_mass / res->densities[i]) * g_an.vdet[i];
-
     so_patch *patches = (so_patch *)calloc(dc.nsub ? dc.nsub : 1, sizeof(so_patch));
     job.patches = patches;
     parallel_for((int64_t)dc.nsub, an_recon_task, &job);
     stitch(res, patches, dc.nsub);
-    for (uint64_t s = 0; s < dc.nsub; ++s) { free(patches[s].v); free(patches[s].vkey); free(patches[s].vinterior); free(patches[s].t); }
+    for (uint64_t k = 0; k < dc.nsub; ++k) { free(patches[k].v); free(patches[k].vkey); free(patches[k].vinterior); free(patches[k].t); }
     free(patches);
     free(dc.flat); free(dc.offset); free(dc.members);
-    free(dstd.flat); free(dstd.offset); free(dstd.members);
-    free(g_an.vdet);
+    free(vdet);
     memset(&g_an, 0, sizeof(g_an));
-    free(filtered);
+    free(s.filtered);
     return 0;
 }

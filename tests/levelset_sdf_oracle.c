@@ -103,7 +103,7 @@ int64_t so_sdf_grid(int mode, const float *ctr, const float *w, const float *g6,
             if (in && dist[r] < B) listed = 1;
         }
         if (!listed) continue;
-        if (n) so_field_scan(mode, ctr, w, g6, dlt, n, h, rs, t_low, t_high, pts, 512, fv);
+        if (n) so_field_scan(mode, ctr, w, g6, dlt, n, h, rs, t_low, t_high, pts, 512, fv, NULL, NULL, NULL);
         else memset(fv, 0, sizeof(float) * 512);
         for (int d = 0; d < 3; ++d) coords[3 * nl + d] = (int32_t)b[d];
         for (int r = 0; r < 512; ++r) {
@@ -116,7 +116,7 @@ int64_t so_sdf_grid(int mode, const float *ctr, const float *w, const float *g6,
     for (int64_t bx = 0; bx < nb[0]; ++bx) for (int64_t by = 0; by < nb[1]; ++by) for (int64_t bz = 0; bz < nb[2]; ++bz) {
         const float p[3] = { sd_coord(gmin, c, 8 * bx, 0), sd_coord(gmin, c, 8 * by, 1), sd_coord(gmin, c, 8 * bz, 2) };
         float v = 0.0f;
-        if (n) so_field_scan(mode, ctr, w, g6, dlt, n, h, rs, t_low, t_high, p, 1, &v);
+        if (n) so_field_scan(mode, ctr, w, g6, dlt, n, h, rs, t_low, t_high, p, 1, &v, NULL, NULL, NULL);
         inside[(bx * nb[1] + by) * nb[2] + bz] = v > thr;
     }
     free(box); free(sel); free(sub); free(pts); free(dist); free(fv);

@@ -12,6 +12,7 @@ import os
 import numpy as np
 import pytest
 
+import c_oracle
 from test_emulated_pipeline import emu  # noqa: F401  (fixture: the package bound to the CPU executor)
 
 R = 0.025
@@ -19,28 +20,15 @@ KW = dict(particle_radius=R, smoothing_length=2.0, cube_size=0.5)
 
 
 # ------------------------------------------------------------------ the anisotropic oracle (tests/anisotropic_oracle.c) ----
-_ANISO_LIB = None
-
-
 def _aniso_lib():
-    """Compiles tests/anisotropic_oracle.c (it includes the pinned oracle/splashsurf_oracle.c unchanged) into a temporary directory, with
-    the oracle's compiler flags, and binds its entry point."""
-    global _ANISO_LIB
-    if _ANISO_LIB is None:
-        import subprocess
-        import tempfile
-        from oracle import _Params, _Result
-        so = os.path.join(tempfile.mkdtemp(prefix="anisotropic_oracle_"), "libanisotropic_oracle.so")
-        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-shared", "-std=c11", "-ffp-contract=off", "-fno-fast-math",
-                               "-mfma", "-mavx2", "-o", so, os.path.join(os.path.dirname(os.path.abspath(__file__)), "anisotropic_oracle.c"),
-                               "-lm", "-lpthread"])
-        L = C.CDLL(so)
-        L.so_reconstruct_aniso.restype = C.c_int
-        L.so_reconstruct_aniso.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_uint32,
-                                           C.POINTER(C.POINTER(_Result)), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.so_free.argtypes = [C.POINTER(_Result)]
-        _ANISO_LIB = L
-    return _ANISO_LIB
+    """tests/anisotropic_oracle.c (it includes the pinned oracle/splashsurf_oracle.c unchanged) with its entry points bound."""
+    from oracle import _Params, _Result
+    vp = C.c_void_p
+    return c_oracle.build("anisotropic_oracle.c", {
+        "so_reconstruct_aniso": (C.c_int, [vp, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_uint32, C.POINTER(C.POINTER(_Result)),
+                                           C.c_int64, vp, vp, vp]),
+        "so_aniso_records": (C.c_int64, [vp, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_uint32, vp, vp, vp, vp]),
+        "so_free": (None, [C.POINTER(_Result)])})
 
 
 def _aniso_params(particle_radius, smoothing_length, cube_size, rest_density, iso_surface_threshold, aabb_min, aabb_max,

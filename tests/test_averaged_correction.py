@@ -14,6 +14,7 @@ import os
 import numpy as np
 import pytest
 
+import c_oracle
 from test_anisotropic import KW, R, _aniso_params, _sphere
 from test_averaged_surface import (CASES, ORACLE_CLOUDS, SHELL_KW, _busiest_tile, _edge_shell_particle, _shell_point,
                                    _tile_points, mesh_topology, numpy_averaged, oracle_reconstruct_averaged)
@@ -24,28 +25,14 @@ T_LOW, T_HIGH = 0.4, 3.5       # the paper's thresholds (JacobianCorrection())
 
 
 # ------------------------------------------------------------------ the corrected oracle (tests/averaged_correction_oracle.c) ----
-_CORR_LIB = None
-
-
 def _corr_lib():
-    """Compiles tests/averaged_correction_oracle.c (it includes tests/averaged_oracle.c and the pinned oracle unchanged) into a
-    temporary directory, with the oracle's compiler flags, and binds its entry points."""
-    global _CORR_LIB
-    if _CORR_LIB is None:
-        import subprocess
-        import tempfile
-        from oracle import _Params, _Result
-        so = os.path.join(tempfile.mkdtemp(prefix="averaged_correction_oracle_"), "libaveraged_correction_oracle.so")
-        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-shared", "-std=c11", "-ffp-contract=off", "-fno-fast-math",
-                               "-mfma", "-mavx2", "-o", so, os.path.join(os.path.dirname(os.path.abspath(__file__)), "averaged_correction_oracle.c"),
-                               "-lm", "-lpthread"])
-        L = C.CDLL(so)
-        L.so_reconstruct_averaged_corrected.restype = C.c_int
-        L.so_reconstruct_averaged_corrected.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_float,
-                                                        C.POINTER(C.POINTER(_Result)), C.c_int64, C.c_void_p]
-        L.so_free.argtypes = [C.POINTER(_Result)]
-        _CORR_LIB = L
-    return _CORR_LIB
+    """tests/averaged_correction_oracle.c (it includes tests/averaged_oracle.c and the pinned oracle unchanged) with its entry points
+    bound."""
+    from oracle import _Params, _Result
+    return c_oracle.build("averaged_correction_oracle.c", {
+        "so_reconstruct_averaged_corrected": (C.c_int, [C.c_void_p, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_float,
+                                                        C.POINTER(C.POINTER(_Result)), C.c_int64, C.c_void_p]),
+        "so_free": (None, [C.POINTER(_Result)])})
 
 
 def oracle_reconstruct_corrected(particles, *, particle_radius, smoothing_length, cube_size, rest_density=1000.0, iso_surface_threshold=0.6,

@@ -12,6 +12,7 @@ import os
 import numpy as np
 import pytest
 
+import c_oracle
 from test_anisotropic import KW, R, _aniso_params, _clustered, _cube, _lattice, _sphere, _splash
 from test_emulated_pipeline import emu  # noqa: F401  (fixture: the package bound to the CPU executor)
 
@@ -19,28 +20,13 @@ H = 4 * R                      # compact support radius of KW
 EPS = 2.0 ** -24               # unit roundoff of f32
 
 # ------------------------------------------------------------------ the averaged oracle (tests/averaged_oracle.c) ----
-_AVG_LIB = None
-
-
 def _avg_lib():
-    """Compiles tests/averaged_oracle.c (it includes the pinned oracle/splashsurf_oracle.c unchanged) into a temporary directory, with
-    the oracle's compiler flags, and binds its entry point."""
-    global _AVG_LIB
-    if _AVG_LIB is None:
-        import subprocess
-        import tempfile
-        from oracle import _Params, _Result
-        so = os.path.join(tempfile.mkdtemp(prefix="averaged_oracle_"), "libaveraged_oracle.so")
-        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-shared", "-std=c11", "-ffp-contract=off", "-fno-fast-math",
-                               "-mfma", "-mavx2", "-o", so, os.path.join(os.path.dirname(os.path.abspath(__file__)), "averaged_oracle.c"),
-                               "-lm", "-lpthread"])
-        L = C.CDLL(so)
-        L.so_reconstruct_averaged.restype = C.c_int
-        L.so_reconstruct_averaged.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(_Params), C.c_float, C.POINTER(C.POINTER(_Result)),
-                                              C.c_int64, C.c_void_p]
-        L.so_free.argtypes = [C.POINTER(_Result)]
-        _AVG_LIB = L
-    return _AVG_LIB
+    """tests/averaged_oracle.c (it includes the pinned oracle/splashsurf_oracle.c unchanged) with its entry point bound."""
+    from oracle import _Params, _Result
+    return c_oracle.build("averaged_oracle.c", {
+        "so_reconstruct_averaged": (C.c_int, [C.c_void_p, C.c_uint64, C.POINTER(_Params), C.c_float, C.POINTER(C.POINTER(_Result)),
+                                              C.c_int64, C.c_void_p]),
+        "so_free": (None, [C.POINTER(_Result)])})
 
 
 def oracle_reconstruct_averaged(particles, *, particle_radius, smoothing_length, cube_size, rest_density=1000.0, iso_surface_threshold=0.6,

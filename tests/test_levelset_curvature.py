@@ -3,73 +3,28 @@ ss_levelset_field_hessian_at_f32 / ss_levelset_field_curvature_at_f32, DESIGN.md
 sources (also run with SS_EMUL_GUARD=1):
 
 * the float64 analytic Hessian of every supported mode is the derivative of the float64 analytic gradient of
-  tests/test_levelset_gradient.py (central differences);
-* the f32 point-scan oracle (tests/levelset_hessian_oracle.c) lies within a per-point float64 bound at every point: a first-order
+  tests/levelset_field_harness.py (central differences);
+* the f32 point-scan oracle (tests/levelset_field_oracle.c) lies within a per-point float64 bound at every point: a first-order
   propagation of every rounding of the fold, including the 1/b^2 growth at the edge of the support of the averaged modes;
 * the device equals the oracle bit for bit (Hessian and curvature), and its values and gradients equal evaluate() and gradient()
-  bit for bit, on the point sets of tests/test_levelset_gradient.py;
+  bit for bit: the device-versus-oracle cases of every query live in tests/test_levelset_field.py;
 * properties (one particle: kappa_H = 1 / rho and kappa_G = 1 / rho^2; a jittered ball and a flat slab; equal radii), refusals, and
   reconstruction_pipeline(levelset_curvature=True) / reconstruct --levelset-curvature=on.
 The GPU-marked counterpart is tests/test_zzz_gpu_levelset_curvature.py."""
-import ctypes as C
 import os
 
 import numpy as np
 import pytest
 
-from test_anisotropic import KW, R, _clustered, _cube, _lattice
+import splashsurf_b200
+from levelset_field_harness import (GRAD_MODES as MODES, _ball, _kw_abs, _same, f64_field, f64_records, mode_kwargs, oracle_field,
+                                    random_points, records)
+from test_anisotropic import KW, _cube, _lattice
 from test_averaged_surface import CASES, ORACLE_CLOUDS
 from test_emulated_pipeline import emu  # noqa: F401  (fixture: the package bound to the CPU executor)
-from test_levelset_field import _kw_abs, face_points, mode_kwargs, random_points, shell_points
-from test_levelset_gradient import MODE_ID, MODES, _cloud_radii, _ball, f64_field, f64_records, records
 
 U = 2.0 ** -24
 HIJ = [(0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2)]       # the six entries xx xy xz yy yz zz
-
-# ------------------------------------------------------------------ the point-scan oracle ----
-_LIBS = {}
-
-
-def _hess_lib(aniso: bool):
-    """Compiles tests/levelset_hessian_oracle.c (on top of tests/levelset_gradient_oracle.c, with or without SO_FIELD_ANISO) into a
-    temporary directory with the oracle's compiler flags."""
-    if aniso not in _LIBS:
-        import subprocess
-        import tempfile
-        from oracle import _Params
-        so = os.path.join(tempfile.mkdtemp(prefix="levelset_hessian_oracle_"), "liblevelset_hessian_oracle.so")
-        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-shared", "-std=c11", "-ffp-contract=off", "-fno-fast-math",
-                               "-mfma", "-mavx2", *(["-DSO_FIELD_ANISO"] if aniso else []), "-o", so,
-                               os.path.join(os.path.dirname(os.path.abspath(__file__)), "levelset_hessian_oracle.c"), "-lm", "-lpthread"])
-        L = C.CDLL(so)
-        vp = C.c_void_p
-        L.so_hessian_scan.restype = None
-        L.so_hessian_scan.argtypes = [C.c_int, vp, vp, vp, vp, C.c_uint64, C.c_float, C.c_float, vp, C.c_uint64, vp, vp, vp]
-        L.so_curvature_scan.restype = None
-        L.so_curvature_scan.argtypes = [C.c_int, vp, vp, vp, vp, C.c_uint64, C.c_float, C.c_float, vp, C.c_uint64, vp, vp]
-        if aniso:
-            L.so_field_aniso_records.restype = C.c_int64
-            L.so_field_aniso_records.argtypes = [vp, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_uint32, vp, vp, vp, vp]
-        _LIBS[aniso] = L
-    return _LIBS[aniso]
-
-
-def oracle_hessian(p, kw, mode, pts, radii=None):
-    """(values, gradients, Hessians, curvatures (m, 2), densities) at `pts` by the point-scan oracle."""
-    r, h, _ = _kw_abs(kw)
-    ctr, w, g6, dlt, rho = records(p, kw, mode, radii)
-    pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 3)
-    m = len(pts)
-    val, grad, hess = np.zeros(m, np.float32), np.zeros((m, 3), np.float32), np.zeros((m, 6), np.float32)
-    cv, curv = np.zeros(m, np.float32), np.full((m, 2), np.nan, np.float32)
-    if m and len(ctr):
-        L = _hess_lib(mode == "aniso")
-        arr = [np.ascontiguousarray(a) if a is not None else None for a in (ctr, w, g6, dlt)]
-        ptr = [a.ctypes.data if a is not None else None for a in arr]
-        L.so_hessian_scan(MODE_ID[mode], *ptr, len(ctr), h, r, pts.ctypes.data, m, val.ctypes.data, grad.ctypes.data, hess.ctypes.data)
-        L.so_curvature_scan(MODE_ID[mode], *ptr, len(ctr), h, r, pts.ctypes.data, m, cv.ctypes.data, curv.ctypes.data)
-        assert np.array_equal(cv.view(np.uint32), val.view(np.uint32))
-    return val, grad, hess, curv, rho
 
 
 # ------------------------------------------------------------------ float64 restatement with a rounding bound ----
@@ -284,7 +239,7 @@ def _hess_matrix(H):
 @pytest.mark.parametrize("cloud", sorted(ORACLE_CLOUDS))
 def test_formula_is_the_derivative(cloud):
     """The float64 analytic Hessian of every supported mode against central differences (step 1e-5 h) of the float64 analytic
-    gradient of test_levelset_gradient.f64_field, at random off-grid points, relative to the largest Hessian norm; only the kink
+    gradient of levelset_field_harness.f64_field, at random off-grid points, relative to the largest Hessian norm; only the kink
     points of section 13.1 (|m| < 1e-3 h, averaged modes) are left out."""
     p = ORACLE_CLOUDS[cloud]()
     r, h, _ = _kw_abs(KW)
@@ -292,7 +247,7 @@ def test_formula_is_the_derivative(cloud):
     lo, hi = p.min(0) - h, p.max(0) + h
     pts = np.random.default_rng(191).uniform(lo, hi, (400, 3))
     for mode in MODES:
-        radii = _cloud_radii(p, KW) if mode == "rad" else None
+        radii = mode_kwargs(splashsurf_b200, mode, p, KW).get("particle_radii")
         ctr, w, g6, dlt = f64_records(p, KW, mode, radii)
         v = f64_field(mode, ctr, w, g6, dlt, h, float(r), pts)[0]
         Hm = _hess_matrix(f64_hessian(mode, ctr, w, g6, dlt, h, pts)[0])
@@ -323,9 +278,9 @@ def test_oracle_within_float64_bounds(cloud):
     lo, hi = p.min(0) - float(h), p.max(0) + float(h)
     pts = np.random.default_rng(193).uniform(lo, hi, (1500, 3)).astype(np.float32)
     for mode in MODES:
-        radii = _cloud_radii(p, KW) if mode == "rad" else None
+        radii = mode_kwargs(splashsurf_b200, mode, p, KW).get("particle_radii")
         ctr, w, g6, dlt, _ = records(p, KW, mode, radii)
-        _, _, oh, _, _ = oracle_hessian(p, KW, mode, pts, radii)
+        oh = oracle_field(p, KW, mode, pts, radii)[2]
         H, reach = f64_hessian(mode, ctr, w, g6, dlt, float(h), pts)
         ref = np.stack([x.v for x in H], 1)
         bnd = 1.25 * np.stack([x.e for x in H], 1)
@@ -336,125 +291,6 @@ def test_oracle_within_float64_bounds(cloud):
             ratio = np.where(bnd > 0, err / bnd, np.where(err > 0, np.inf, 0.0))
         print(cloud, mode, "largest error / bound", float(ratio[reach].max()), "points", int(reach.sum()))
         assert np.all(err <= bnd), (mode, float(ratio.max()))
-
-
-# ------------------------------------------------------------------ 3. device == oracle, values == evaluate ----
-def _same(a, b):
-    """Bit equality, with every NaN equal to every NaN (device and host NaN payloads differ)."""
-    a, b = np.asarray(a), np.asarray(b)
-    return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(np.where(np.isnan(a), 0, a).view(np.uint32),
-                                                                        np.where(np.isnan(b), 0, b).view(np.uint32))
-
-
-def check_hessian_vs_oracle(ss, p, kw, mode, pts, expect_tier=None):
-    """Device values, gradients, Hessians and curvatures == the point-scan oracle bit for bit; values == evaluate() and gradients ==
-    gradient() bit for bit.  Returns the tier counters of the Hessian query."""
-    mk = mode_kwargs(ss, mode, p, kw)
-    f = ss.LevelSetField(p, **kw, **mk)
-    try:
-        v, g, H = f.hessian(pts)
-        paths = f.paths
-        kh, kg = f.curvature(pts)
-        assert v.shape == (len(pts),) and g.shape == (len(pts), 3) and H.shape == (len(pts), 6)
-        assert kh.shape == (len(pts),) and kg.shape == (len(pts),) and kh.dtype == np.float32
-        assert np.array_equal(v.view(np.uint32), f.evaluate(pts).view(np.uint32)), mode
-        assert np.array_equal(g.view(np.uint32), f.gradient(pts)[1].view(np.uint32)), mode
-        ov, og, oh, oc, rho = oracle_hessian(p, kw, mode, pts, radii=mk.get("particle_radii"))
-        assert np.array_equal(f.particle_densities, rho)
-        assert np.array_equal(v.view(np.uint32), ov.view(np.uint32)) and np.array_equal(g.view(np.uint32), og.view(np.uint32)), mode
-        bad = np.flatnonzero(np.any(H.view(np.uint32) != oh.view(np.uint32), axis=1))
-        assert len(bad) == 0, (mode, len(bad), pts[bad[:3]], H[bad[:3]], oh[bad[:3]])
-        assert _same(kh, oc[:, 0]) and _same(kg, oc[:, 1]), mode
-        assert np.all(np.isnan(kh[np.all(g == 0, axis=1)]))
-        if expect_tier:
-            assert paths[expect_tier] > 0, paths
-        return paths
-    finally:
-        f.close()
-
-
-@pytest.mark.parametrize("mode", MODES)
-def test_emulated_random_points_equal_oracle(emu, mode):  # noqa: F811
-    gen, kw, _ = CASES["splash_S24"]
-    p = gen()
-    f = emu.LevelSetField(p, **kw)
-    pts = np.concatenate([random_points(f.grid, 2000, 141), random_points(f.grid, 200, 142, pad=0.3)])
-    f.close()
-    assert check_hessian_vs_oracle(emu, p, kw, mode, pts)["512"] > 0
-
-
-@pytest.mark.parametrize("Rc", [1, 6, 7, 8, 9, 17])
-def test_emulated_faces_and_last_cells_equal_oracle(emu, Rc):  # noqa: F811
-    p = _cube(7, 900 + Rc)
-    kw = dict(particle_radius=R, smoothing_length=2.0, cube_size=4.0 / (Rc - 0.5), subdomain_num_cubes_per_dim=16)
-    f = emu.LevelSetField(p, **kw)
-    pts = face_points(f.grid, 16, 177 + Rc)
-    f.close()
-    for mode in ("sph", "avg"):
-        check_hessian_vs_oracle(emu, p, kw, mode, pts)
-
-
-@pytest.mark.parametrize("mode", MODES)
-def test_emulated_lone_particle_shells(emu, mode):  # noqa: F811
-    p = np.array([[0.1, 0.2, 0.3]], np.float32)
-    _, h, _ = _kw_abs(KW)
-    check_hessian_vs_oracle(emu, p, KW, mode, np.concatenate([shell_points(p[0], h), p]))
-
-
-@pytest.mark.parametrize("mode", MODES)
-def test_emulated_outside_and_empty_subdomains_are_zero(emu, mode):  # noqa: F811
-    gen, kw, _ = CASES["droplets_sparse"]
-    p = gen()
-    mk = mode_kwargs(emu, mode, p, kw)
-    f = emu.LevelSetField(p, **kw, **mk)
-    try:
-        far = np.array([[1e6, 0, 0], [-1e6, 5, 5], [0, 0, 3e38]], np.float32)
-        outside = random_points(f.grid, 500, 151, pad=2.0)
-        lo, hi = np.asarray(f.grid.aabb.min), np.asarray(f.grid.aabb.max)
-        outside = np.concatenate([far, outside[np.any((outside < lo) | (outside > hi), axis=1)]])
-        v, g, H = f.hessian(outside)
-        assert np.all(v == 0.0) and np.all(g == 0.0) and np.all(H == 0.0)
-        kh, kg = f.curvature(outside)
-        assert np.all(np.isnan(kh)) and np.all(np.isnan(kg))
-        inside = random_points(f.grid, 3000, 152)
-        v, g, H = f.hessian(inside)
-        empty = (v == 0) & np.all(g == 0, axis=1) & np.all(H == 0, axis=1)
-        assert empty.sum() > 100
-        assert np.all(np.isnan(f.curvature(inside[empty])[0]))
-    finally:
-        f.close()
-    check_hessian_vs_oracle(emu, p, kw, mode, inside)
-
-
-@pytest.mark.parametrize("mode", ["sph", "avg"])
-def test_emulated_clustered_reaches_select(emu, mode):  # noqa: F811
-    p = _clustered(507)
-    kw = dict(KW, subdomain_num_cubes_per_dim=16)
-    _, h, _ = _kw_abs(kw)
-    pts = np.concatenate([shell_points(np.full(3, 0.2), h * np.float32(0.5)),
-                          np.random.default_rng(161).uniform(0.1, 0.3, (200, 3)).astype(np.float32)])
-    check_hessian_vs_oracle(emu, p, kw, mode, pts, expect_tier="select")
-
-
-def test_emulated_empty_inputs(emu):  # noqa: F811
-    f = emu.LevelSetField(np.zeros((0, 3), np.float32), **KW)
-    try:
-        v, g, H = f.hessian(np.zeros((0, 3), np.float32))
-        assert v.shape == (0,) and g.shape == (0, 3) and H.shape == (0, 6)
-        kh, kg = f.curvature(np.zeros((0, 3), np.float32))
-        assert kh.shape == (0,) and kg.shape == (0,)
-        v, g, H = f.hessian(np.array([[0, 0, 0], [1, 1, 1]], np.float32))
-        assert np.all(v == 0.0) and np.all(g == 0.0) and np.all(H == 0.0)
-        assert np.all(np.isnan(f.curvature(np.array([[0, 0, 0]], np.float32))[0]))
-    finally:
-        f.close()
-    p = _cube(6, 5)
-    f = emu.LevelSetField(p, **KW)
-    try:
-        kh, kg = f.curvature(np.zeros((0, 3), np.float32))
-        assert kh.shape == (0,) and kg.shape == (0,)
-    finally:
-        f.close()
 
 
 # ------------------------------------------------------------------ 4. one particle ----
@@ -548,7 +384,7 @@ def test_emulated_refusals(emu):  # noqa: F811
     for corr_rad in (False, True):
         mk = dict(averaged_surface=ss.AveragedSurface(1.0, ss.JacobianCorrection()))
         if corr_rad:
-            mk["particle_radii"] = _cloud_radii(p, KW)
+            mk["particle_radii"] = mode_kwargs(ss, "rad", p, KW)["particle_radii"]
         f = ss.LevelSetField(p, **KW, **mk)
         try:
             pts = random_points(f.grid, 10, 3)

@@ -1,7 +1,7 @@
 """Narrow-band signed distance grids (LevelSetField.signed_distance / ss_levelset_field_sdf_f32, DESIGN.md section 14) on the CPU
 executor of the CUDA sources (also run with SS_EMUL_GUARD=1):
 
-* the device equals the brute-force oracle (tests/levelset_sdf_oracle.c) bit for bit -- brick list, values and brick_inside -- in
+* the device equals the brute-force oracle (tests/levelset_sdf_oracle.c, bound by tests/levelset_field_harness.py) bit for bit -- brick list, values and brick_inside -- in
   every mode (standard with simd off and on, anisotropic, averaged, corrected, radii), on section 12's clouds, at band 1 / 3 / 8,
   S = 16 / 24 / 64 and at cube sizes giving R = 1, 6, 7, 8, 9, 17;
 * hand-made meshes through the C entry: single triangles on brick faces and corners, zero-area triangles, a triangle outside the
@@ -13,128 +13,18 @@ executor of the CUDA sources (also run with SS_EMUL_GUARD=1):
 * refusals, one context reused across fields, queries and grids, and the CLI's --output-sdf.
 The GPU-marked counterpart is tests/test_zzz_gpu_levelset_sdf.py."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
-from test_anisotropic import KW, R, _aniso_params, _cube
+from levelset_field_harness import (SDF_MODES, assert_sdf_equal, check_properties, check_sdf_vs_oracle, mode_kwargs, oracle_distance,
+                                    oracle_sdf, raw_case)
+from test_anisotropic import KW, R, _cube
 from test_averaged_surface import CASES
 from test_emulated_pipeline import emu  # noqa: F401  (fixture: the package bound to the CPU executor)
-from test_levelset_field import MODE_ID, T_HIGH, T_LOW, _filtered, _kw_abs, mode_kwargs
-
-SDF_MODES = ["sph", "sph_simd", "aniso", "avg", "corr", "rad"]
-
-# ------------------------------------------------------------------ the brute-force oracle ----
-_LIBS = {}
-
-
-def sdf_lib(aniso: bool):
-    """Compiles tests/levelset_sdf_oracle.c (on top of the field oracle; SO_FIELD_ANISO as in test_levelset_field) into a temporary
-    directory with the oracle's compiler flags."""
-    if aniso not in _LIBS:
-        import subprocess
-        import tempfile
-        from oracle import _Params
-        so = os.path.join(tempfile.mkdtemp(prefix="levelset_sdf_oracle_"), "liblevelset_sdf_oracle.so")
-        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-shared", "-std=c11", "-ffp-contract=off", "-fno-fast-math",
-                               "-mfma", "-mavx2", *(["-DSO_FIELD_ANISO"] if aniso else []), "-o", so,
-                               os.path.join(os.path.dirname(os.path.abspath(__file__)), "levelset_sdf_oracle.c"), "-lm", "-lpthread"])
-        L = C.CDLL(so)
-        vp = C.c_void_p
-        L.so_sdf_distance.restype = None
-        L.so_sdf_distance.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, vp]
-        L.so_sdf_grid.restype = C.c_int64
-        L.so_sdf_grid.argtypes = [C.c_int, vp, vp, vp, vp, C.c_uint64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
-                                  vp, vp, C.c_uint64, vp, C.c_float, vp, C.c_uint32, vp, vp, vp]
-        if aniso:
-            L.so_field_aniso_records.restype = C.c_int64
-            L.so_field_aniso_records.argtypes = [vp, C.c_uint64, C.POINTER(_Params), C.c_float, C.c_float, C.c_uint32, vp, vp, vp, vp]
-        _LIBS[aniso] = L
-    return _LIBS[aniso]
-
-
-def _ptr(a):
-    return None if a is None or a.size == 0 else a.ctypes.data
-
-
-def oracle_distance(verts, tris, pts):
-    """f32 unsigned distance of section 14 at `pts` by a scan over the given triangles."""
-    verts, tris = np.ascontiguousarray(verts, np.float32), np.ascontiguousarray(tris, np.uint32)
-    pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 3)
-    d = np.empty(len(pts), np.float32)
-    if len(pts):
-        sdf_lib(False).so_sdf_distance(_ptr(verts), _ptr(tris), len(tris), _ptr(pts), len(pts), d.ctypes.data)
-    return d
-
-
-def oracle_sdf(p, kw, mode, verts, tris, band, grid, thr, radii=None):
-    """(brick_coords, values, brick_inside) of section 14 by the oracle; the field records are those of
-    test_levelset_field.oracle_field (the anisotropic oracle for x_bar, G and V det G)."""
-    from test_averaged_surface import oracle_reconstruct_averaged
-    r, h, c = _kw_abs(kw)
-    rs = np.float32(r)
-    fmode = "sph" if mode == "sph_simd" else mode
-    if fmode == "aniso":
-        L = sdf_lib(True)
-        xyz = np.ascontiguousarray(p, np.float32)
-        prm = _aniso_params(kw["particle_radius"], kw["smoothing_length"], kw["cube_size"], kw.get("rest_density", 1000.0), 0.6,
-                            kw.get("aabb_min"), kw.get("aabb_max"), True, kw.get("subdomain_num_cubes_per_dim", 64))
-        n = max(len(xyz), 1)
-        ctr, g, w, rho = np.zeros((n, 3), np.float32), np.zeros((n, 6), np.float32), np.zeros(n, np.float32), np.zeros(n, np.float32)
-        nf = L.so_field_aniso_records(_ptr(xyz), len(xyz), C.byref(prm), 0.9, 4.0, 10, ctr.ctypes.data, g.ctypes.data, w.ctypes.data,
-                                      rho.ctypes.data)
-        delta = None
-    else:
-        L = sdf_lib(False)
-        g = None
-        rho = oracle_reconstruct_averaged(p, **kw)["particle_densities"]
-        ctr, rr = _filtered(np.ascontiguousarray(p, np.float32), kw, radii)
-        nf = len(ctr)
-        r2 = np.float32(r + r)
-        w = (np.float32(r2 * r2 * r2 * np.float32(kw.get("rest_density", 1000.0))) / rho).astype(np.float32)
-        delta = np.ascontiguousarray(rr.astype(np.float32) - rs, np.float32) if fmode in ("rad", "corr_rad") else None
-    npd = np.asarray(grid.npoints_per_dim, np.int64)
-    nb = (npd + 7) // 8
-    nbt = int(np.prod(nb))
-    coords, values, inside = np.zeros((nbt, 3), np.int32), np.zeros((nbt, 8, 8, 8), np.float32), np.zeros(nb, np.uint8)
-    verts, tris = np.ascontiguousarray(verts, np.float32), np.ascontiguousarray(tris, np.uint32)
-    gmin = np.asarray(grid.aabb.min, np.float32)
-    nl = L.so_sdf_grid(MODE_ID[fmode], _ptr(ctr), _ptr(w), _ptr(g), _ptr(delta), nf, h, rs, T_LOW, T_HIGH, np.float32(thr), _ptr(verts),
-                       _ptr(tris), len(tris), gmin.ctypes.data, np.float32(grid.cell_size), npd.ctypes.data, band, coords.ctypes.data,
-                       values.ctypes.data, inside.ctypes.data)
-    return coords[:nl], values[:nl], inside.astype(bool)
-
-
-def assert_sdf_equal(got, coords, values, inside, what=""):
-    assert np.array_equal(np.asarray(got.brick_coords), coords), (what, len(got.brick_coords), len(coords))
-    bad = np.flatnonzero(np.asarray(got.values).view(np.uint32).ravel() != values.view(np.uint32).ravel())
-    assert len(bad) == 0, (what, len(bad), np.asarray(got.values).ravel()[bad[:4]], values.ravel()[bad[:4]])
-    assert np.array_equal(np.asarray(got.brick_inside), inside), what
 
 
 # ------------------------------------------------------------------ device vs oracle ----
-def raw_case(ss, p, kw, mode, ctx=None):
-    """(field, raw mesh, reconstruction keywords) of a mode: the standard mode reconstructs with simd off except in sph_simd."""
-    mk = mode_kwargs(ss, "sph" if mode == "sph_simd" else mode, p, kw)
-    rec = ss.reconstruct_surface(p, simd=(mode == "sph_simd"), subdomain_grid_auto_disable=False, context=ctx, **kw, **mk)
-    f = ss.LevelSetField(p, **kw, **mk)
-    return f, rec, mk
-
-
-def check_sdf_vs_oracle(ss, p, kw, mode, band):
-    f, rec, mk = raw_case(ss, p, kw, mode)
-    try:
-        got = f.signed_distance(rec.mesh, band=band)
-        o = oracle_sdf(p, kw, mode, rec.mesh.vertices, rec.mesh.triangles, band, f.grid, f.threshold, radii=mk.get("particle_radii"))
-        assert_sdf_equal(got, *o, what=(mode, band))
-        assert got.background == np.float32(band) * np.float32(f.grid.cell_size)
-        return f, rec, got
-    except Exception:
-        f.close()
-        raise
-
-
 @pytest.mark.parametrize("mode", SDF_MODES)
 @pytest.mark.parametrize("name", ["cube_S16", "splash_S24", "cube_S64"])
 def test_emulated_sdf_equals_oracle(emu, name, mode):  # noqa: F811
@@ -358,45 +248,6 @@ def test_emulated_distance_within_float64_bound(emu):  # noqa: F811
 
 
 # ------------------------------------------------------------------ properties on raw meshes ----
-def check_properties(ss, f, rec, got):
-    """Sign bit = field.inside at listed points; adjacent listed unclamped values within a cell; every vertex's edge listed with opposite
-    signs and |s| <= cell; to_dense() has the field's sign everywhere."""
-    c = np.float32(f.grid.cell_size)
-    B = np.float32(got.background)
-    n = np.asarray(f.grid.npoints_per_dim)
-    lo = np.asarray(f.grid.aabb.min, np.float32)
-    dense = got.to_dense()
-    assert dense.shape == tuple(n)
-    idx = np.stack(np.meshgrid(*[np.arange(k) for k in n], indexing="ij"), -1).reshape(-1, 3)
-    pts = (lo + idx.astype(np.float32) * c).astype(np.float32)
-    inside = f.inside(pts).reshape(tuple(n))
-    assert np.array_equal(np.signbit(dense), inside)                # -0.0: an inside point on the mesh
-    listed = np.zeros(tuple((n + 7) // 8 * 8), bool)
-    for b in np.asarray(got.brick_coords):
-        listed[8 * b[0]:8 * b[0] + 8, 8 * b[1]:8 * b[1] + 8, 8 * b[2]:8 * b[2] + 8] = True
-    listed = listed[:n[0], :n[1], :n[2]]
-    unclamped = listed & (np.abs(dense) < B)
-    # the distances are 1-Lipschitz; the f32 coordinates of points and vertices round relative to their magnitude, not to the cell
-    tol = float(c) * (1 + 1e-5) + 8 * float(np.spacing(np.float32(np.abs(np.concatenate([pts[[0, -1]].ravel(), lo])).max())))
-    for ax in range(3):
-        a = [slice(None)] * 3
-        b = [slice(None)] * 3
-        a[ax], b[ax] = slice(0, -1), slice(1, None)
-        both = unclamped[tuple(a)] & unclamped[tuple(b)]
-        diff = np.abs(dense[tuple(a)].astype(np.float64) - dense[tuple(b)])
-        assert np.all(diff[both] <= tol), (ax, float(diff[both].max()), tol)
-    if rec.mesh.nvertices:
-        keys = np.asarray(rec.vertex_edge_keys, np.int64).reshape(-1, 4) if rec.vertex_edge_keys is not None else None
-        if keys is not None:
-            i0 = keys[:, :3]
-            i1 = i0.copy()
-            i1[np.arange(len(i1)), keys[:, 3]] += 1
-            s0, s1 = dense[tuple(i0.T)], dense[tuple(i1.T)]
-            assert np.all(listed[tuple(i0.T)] & listed[tuple(i1.T)])
-            assert np.all(np.signbit(s0) != np.signbit(s1))
-            assert np.all((np.abs(s0) <= tol) & (np.abs(s1) <= tol))
-
-
 @pytest.mark.parametrize("mode", ["sph", "aniso", "avg", "corr", "rad"])
 def test_emulated_properties_on_raw_meshes(emu, mode):  # noqa: F811
     gen, kw, _ = CASES["splash_S24"]

@@ -1,79 +1,15 @@
 """The Hessian and curvature of the level set at arbitrary points (LevelSetField.hessian / .curvature, DESIGN.md section 13.2) on
-the device: the device cases of tests/test_levelset_curvature.py on the H100 (values, gradients, Hessians and curvatures equal the
-point-scan oracle bit for bit, values and gradients equal evaluate() and gradient() bit for bit, the tier of each case printed),
-host and device point arrays give identical results, and on a 1 M-particle dam break in every mode with a Hessian the values and
-gradients equal evaluate() and gradient() at the mesh vertices and at 10 M uniform points, value, gradient and Hessian are 0 outside
-the grid, and the curvature is finite at every vertex with a nonzero gradient."""
+the device (the device-versus-oracle cases of every query live in tests/test_zzz_gpu_levelset_field.py): host and device point
+arrays give identical results, and on a 1 M-particle dam break in every mode with a Hessian the values and gradients equal
+evaluate() and gradient() at the mesh vertices and at 10 M uniform points, value, gradient and Hessian are 0 outside the grid, and
+the curvature is finite at every vertex with a nonzero gradient."""
 import numpy as np
 import pytest
 
-from test_anisotropic import KW, R, _clustered, _cube
-from test_averaged_surface import CASES
-from test_levelset_curvature import _same, check_hessian_vs_oracle
-from test_levelset_field import _kw_abs, face_points, mode_kwargs, random_points, shell_points
-from test_levelset_gradient import MODES
+from levelset_field_harness import GRAD_MODES as MODES, _ball, _same, mode_kwargs, random_points
+from test_anisotropic import KW, R, _cube
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.mark.parametrize("mode", MODES)
-def test_cuda_points_equal_oracle(ss, mode):
-    gen, kw, _ = CASES["splash_S24"]
-    p = gen()
-    f = ss.LevelSetField(p, **kw)
-    pts = np.concatenate([random_points(f.grid, 20000, 141), random_points(f.grid, 2000, 142, pad=0.3)])
-    f.close()
-    print(mode, check_hessian_vs_oracle(ss, p, kw, mode, pts))
-    one = np.array([[0.1, 0.2, 0.3]], np.float32)
-    print(mode, "lone particle", check_hessian_vs_oracle(ss, one, KW, mode, np.concatenate([shell_points(one[0], _kw_abs(KW)[1]), one])))
-
-
-@pytest.mark.parametrize("Rc", [1, 6, 7, 8, 9, 17])
-def test_cuda_faces_and_last_cells_equal_oracle(ss, Rc):
-    p = _cube(7, 900 + Rc)
-    kw = dict(particle_radius=R, smoothing_length=2.0, cube_size=4.0 / (Rc - 0.5), subdomain_num_cubes_per_dim=16)
-    f = ss.LevelSetField(p, **kw)
-    pts = face_points(f.grid, 16, 177 + Rc)
-    f.close()
-    for mode in MODES:
-        print(Rc, mode, check_hessian_vs_oracle(ss, p, kw, mode, pts))
-
-
-@pytest.mark.parametrize("mode", ["sph", "avg"])
-def test_cuda_clustered_reaches_select(ss, mode):
-    p = _clustered(507)
-    kw = dict(KW, subdomain_num_cubes_per_dim=16)
-    _, h, _ = _kw_abs(kw)
-    pts = np.concatenate([shell_points(np.full(3, 0.2), h * np.float32(0.5)),
-                          np.random.default_rng(161).uniform(0.1, 0.3, (200, 3)).astype(np.float32)])
-    print(mode, check_hessian_vs_oracle(ss, p, kw, mode, pts, expect_tier="select"))
-
-
-def test_cuda_outside_and_empty_inputs(ss):
-    gen, kw, _ = CASES["droplets_sparse"]
-    p = gen()
-    for mode in MODES:
-        mk = mode_kwargs(ss, mode, p, kw)
-        f = ss.LevelSetField(p, **kw, **mk)
-        try:
-            pts = random_points(f.grid, 5000, 151, pad=2.0)
-            lo, hi = np.asarray(f.grid.aabb.min), np.asarray(f.grid.aabb.max)
-            out = np.any((pts < lo) | (pts > hi), axis=1)
-            v, g, H = f.hessian(pts)
-            assert np.all(v[out] == 0.0) and np.all(g[out] == 0.0) and np.all(H[out] == 0.0)
-            assert np.all(np.isnan(f.curvature(pts)[0][out]))
-            inside = random_points(f.grid, 3000, 152)
-            print(mode, "empty subdomains", check_hessian_vs_oracle(ss, p, kw, mode, inside))
-            v, g, H = f.hessian(np.zeros((0, 3), np.float32))
-            assert v.shape == (0,) and g.shape == (0, 3) and H.shape == (0, 6)
-        finally:
-            f.close()
-    f = ss.LevelSetField(np.zeros((0, 3), np.float32), **KW)
-    v, g, H = f.hessian(np.array([[0, 0, 0], [1, 1, 1]], np.float32))
-    assert np.all(v == 0.0) and np.all(g == 0.0) and np.all(H == 0.0)
-    kh, kg = f.curvature(np.array([[0, 0, 0]], np.float32))
-    assert np.isnan(kh).all() and np.isnan(kg).all()
-    f.close()
 
 
 def test_cuda_host_and_device_points_agree(ss):
@@ -110,7 +46,6 @@ def test_cuda_refusals(ss):
 
 @pytest.mark.parametrize("mode", MODES)
 def test_cuda_pipeline_levelset_curvature(ss, mode):
-    from test_levelset_gradient import _ball
     p = _ball(0.1, 111)
     mk = mode_kwargs(ss, mode, p, KW)
     mesh, _ = ss.reconstruction_pipeline(p, levelset_curvature=True, mesh_smoothing_iters=2, **KW, **mk)

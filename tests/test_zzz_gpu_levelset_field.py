@@ -1,14 +1,15 @@
-"""The level set at arbitrary points (LevelSetField, DESIGN.md section 13) on the device: the device cases of
-tests/test_levelset_field.py on the H100 (the field equals the reconstruction's tile and the point-scan oracle bit for bit in every
-mode, the tier of each case read back), host and device point arrays give identical values, and on a 1 M-particle dam break the two
-grid points of every mesh vertex's edge straddle the threshold while 10 M random points are evaluated."""
+"""The level set at arbitrary points and its derivatives (LevelSetField, DESIGN.md sections 13, 13.1 and 13.2) on the device: the
+device cases of tests/test_levelset_field.py on the H100 (the field equals the reconstruction's tile in every mode, and every query
+a mode supports -- values, gradients, Hessians, curvatures -- equals the point-scan oracle bit for bit, the tiers of each case
+printed), host and device point arrays give identical values, and on a 1 M-particle dam break the two grid points of every mesh
+vertex's edge straddle the threshold while 10 M random points are evaluated."""
 import numpy as np
 import pytest
 
-from test_anisotropic import KW, _clustered, _cube
+from levelset_field_harness import (GRAD_MODES, MODES, _kw_abs, check_field_vs_oracle, check_field_vs_reconstruction, face_points,
+                                    mode_kwargs, random_points, shell_points)
+from test_anisotropic import KW, R, _clustered, _cube
 from test_averaged_surface import CASES
-from test_levelset_field import (MODES, _kw_abs, check_field_vs_oracle, check_field_vs_reconstruction, face_points, mode_kwargs,
-                                 random_points, shell_points)
 
 pytestmark = pytest.mark.gpu
 
@@ -24,23 +25,23 @@ def test_cuda_points_equal_oracle(ss, mode):
     gen, kw, _ = CASES["splash_S24"]
     p = gen()
     f = ss.LevelSetField(p, **kw)
-    pts = np.concatenate([random_points(f.grid, 20000, 41), random_points(f.grid, 2000, 42, pad=0.3)])
+    pts = np.concatenate([random_points(f.grid, 20000, 41), random_points(f.grid, 2000, 42, pad=0.3),
+                          random_points(f.grid, 20000, 141), random_points(f.grid, 2000, 142, pad=0.3)])
     f.close()
     print(mode, check_field_vs_oracle(ss, p, kw, mode, pts))
     one = np.array([[0.1, 0.2, 0.3]], np.float32)
-    check_field_vs_oracle(ss, one, KW, mode, np.concatenate([shell_points(one[0], _kw_abs(KW)[1]), one]))
+    print(mode, "lone particle", check_field_vs_oracle(ss, one, KW, mode, np.concatenate([shell_points(one[0], _kw_abs(KW)[1]), one])))
 
 
 @pytest.mark.parametrize("Rc", [1, 6, 7, 8, 9, 17])
 def test_cuda_faces_and_last_cells_equal_oracle(ss, Rc):
-    from test_anisotropic import R
     p = _cube(7, 900 + Rc)
     kw = dict(particle_radius=R, smoothing_length=2.0, cube_size=4.0 / (Rc - 0.5), subdomain_num_cubes_per_dim=16)
     f = ss.LevelSetField(p, **kw)
-    pts = face_points(f.grid, 16, 77 + Rc)
+    pts = np.concatenate([face_points(f.grid, 16, 77 + Rc), face_points(f.grid, 16, 177 + Rc)])
     f.close()
     for mode in MODES:
-        check_field_vs_oracle(ss, p, kw, mode, pts)
+        print(Rc, mode, check_field_vs_oracle(ss, p, kw, mode, pts))
 
 
 @pytest.mark.parametrize("mode", ["sph", "avg", "corr"])
@@ -49,8 +50,39 @@ def test_cuda_clustered_reaches_select(ss, mode):
     kw = dict(KW, subdomain_num_cubes_per_dim=16)
     _, h, _ = _kw_abs(kw)
     pts = np.concatenate([shell_points(np.full(3, 0.2), h * np.float32(0.5)),
-                          np.random.default_rng(61).uniform(0.1, 0.3, (200, 3)).astype(np.float32)])
+                          np.random.default_rng(61).uniform(0.1, 0.3, (200, 3)).astype(np.float32),
+                          np.random.default_rng(161).uniform(0.1, 0.3, (200, 3)).astype(np.float32)])
     print(mode, check_field_vs_oracle(ss, p, kw, mode, pts, expect_tier="select"))
+
+
+def test_cuda_outside_and_empty_inputs(ss):
+    gen, kw, _ = CASES["droplets_sparse"]
+    p = gen()
+    none = np.zeros((0, 3), np.float32)
+    for mode in MODES:
+        grad = mode in GRAD_MODES
+        f = ss.LevelSetField(p, **kw, **mode_kwargs(ss, mode, p, kw))
+        try:
+            pts = np.concatenate([random_points(f.grid, 5000, 51, pad=2.0), random_points(f.grid, 5000, 151, pad=2.0)])
+            lo, hi = np.asarray(f.grid.aabb.min), np.asarray(f.grid.aabb.max)
+            out = np.any((pts < lo) | (pts > hi), axis=1)
+            inside = random_points(f.grid, 3000, 152)
+            assert np.all(f.evaluate(pts)[out] == 0.0) and f.evaluate(none).shape == (0,)
+            if grad:
+                v, g, H = f.hessian(pts)
+                assert np.all(v[out] == 0.0) and np.all(g[out] == 0.0) and np.all(H[out] == 0.0)
+                assert np.all(np.isnan(f.curvature(pts)[0][out]))
+                v, g, H = f.hessian(none)
+                assert v.shape == (0,) and g.shape == (0, 3) and H.shape == (0, 6)
+        finally:
+            f.close()
+        print(mode, "empty subdomains", check_field_vs_oracle(ss, p, kw, mode, inside))
+    f = ss.LevelSetField(none, **KW)
+    v, g, H = f.hessian(np.array([[0, 0, 0], [1, 1, 1]], np.float32))
+    assert np.all(v == 0.0) and np.all(g == 0.0) and np.all(H == 0.0)
+    kh, kg = f.curvature(np.array([[0, 0, 0]], np.float32))
+    assert np.isnan(kh).all() and np.isnan(kg).all()
+    f.close()
 
 
 def test_cuda_host_and_device_points_agree(ss):

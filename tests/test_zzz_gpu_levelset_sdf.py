@@ -5,11 +5,10 @@ listed bricks (the oracle gets the triangles near each brick; the signs come fro
 import numpy as np
 import pytest
 
+from levelset_field_harness import (SDF_MODES, assert_sdf_equal, check_properties, check_sdf_vs_oracle, mode_kwargs, oracle_distance,
+                                    oracle_sdf, raw_case)
 from test_anisotropic import KW, R, _cube
 from test_averaged_surface import CASES
-from test_levelset_field import mode_kwargs
-from test_levelset_sdf import (SDF_MODES, assert_sdf_equal, check_properties, check_sdf_vs_oracle, oracle_distance, oracle_sdf,
-                               raw_case)
 
 pytestmark = pytest.mark.gpu
 
