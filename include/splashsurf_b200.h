@@ -218,6 +218,14 @@ int ss_surface_copy_subdomains(const ss_surface *s, int64_t *flat, uint64_t *cou
  * reconstruction on this context; pass -1 to disable. */
 int ss_context_keep_levelset_tile(ss_context *ctx, int64_t flat_subdomain);
 int ss_surface_copy_levelset_tile(const ss_surface *s, float *dst);
+/* The same tile without forcing exact evaluation: the production launch sequence runs unchanged, and the tile is copied as the
+ * certification and exact pass left it, before the fix-up pass.  Certified points hold SS_MARKER (3.0e38f), evaluated points
+ * their exact values.  brick_state receives one byte per 8^3-point brick of the tile, nb^3 with nb = ceil((S + 1) / 8), i-major:
+ * 0 untouched (contents undefined: untouched bricks are not zero-filled beforehand), 1 every point certified, 2 exact values
+ * (and possibly markers in other boxes of the brick).  Independent of ss_context_keep_levelset_tile; pass -1 to disable.
+ * Either destination may be NULL. */
+int ss_context_keep_levelset_tile_raw(ss_context *ctx, int64_t flat_subdomain);
+int ss_surface_copy_levelset_tile_raw(const ss_surface *s, float *tile, uint8_t *brick_state);
 
 /* Timings / launch counts of the reconstruction that produced `s`. */
 int ss_surface_timings(const ss_surface *s, ss_timings *out);

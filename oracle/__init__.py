@@ -101,6 +101,8 @@ def reconstruct(particles, *, particle_radius, smoothing_length, cube_size, rest
                 subdomain_grid_auto_disable=True, subdomain_num_cubes_per_dim=64, multi_threading=True, tile_of_subdomain=None,
                 want_neighbor_counts=False, want_neighbors=False, num_threads=None):
     """C-oracle counterpart of pysplashsurf.reconstruct_surface (same RELATIVE smoothing_length / cube_size).
+    `tile_of_subdomain`: flat index of a tile whose level-set values are returned as d["tile"]: (S + 1)^3 on the subdomain path,
+    65^3 on the global path (its grid cut into 64-cube tiles, as the device tiles it).
     `multi_threading` is accepted and ignored: the global path is restated with its sequential (deterministic) semantics."""
     L = lib()
     if num_threads is not None:
@@ -117,7 +119,10 @@ def reconstruct(particles, *, particle_radius, smoothing_length, cube_size, rest
     p.enable_simd, p.decomposition = int(simd), int(subdomain_grid)
     p.subdomain_num_cubes_per_dim, p.auto_disable = int(subdomain_num_cubes_per_dim), int(subdomain_grid_auto_disable)
     S = int(subdomain_num_cubes_per_dim)
-    tile = np.zeros((S + 1,) * 3, dtype=np.float32) if tile_of_subdomain is not None else None
+    # the subdomain path writes (S + 1)^3 floats, the global path the 65^3 points of a 64-cube tile of its grid (whatever S is):
+    # room for both, shaped below by the path taken
+    tmax = max(S, 64) + 1
+    tile = np.zeros(tmax ** 3, dtype=np.float32) if tile_of_subdomain is not None else None
     ncnt = np.zeros(len(xyz), dtype=np.int64) if (want_neighbor_counts or want_neighbors) else None
     out = C.POINTER(_Result)()
     rc = L.so_reconstruct(xyz.ctypes.data, len(xyz), C.byref(p), C.byref(out),
@@ -150,6 +155,9 @@ def reconstruct(particles, *, particle_radius, smoothing_length, cube_size, rest
         d["subdomain_count"] = np.ctypeslib.as_array(res.subdomain_count, (ns,)).copy() if ns else np.zeros(0, np.uint64)
         d["subdomain_sparse"] = np.ctypeslib.as_array(res.subdomain_sparse, (ns,)).astype(bool).copy() if ns else np.zeros(0, bool)
         d["max_particles"], d["sparse_limit"] = int(res.max_particles), int(res.sparse_limit)
+        if tile is not None:
+            tn = S + 1 if res.used_decomposition else 65
+            tile = tile[:tn ** 3].reshape((tn,) * 3)
         d["tile"], d["neighbor_counts"], d["neighbors"] = tile, ncnt, nbr
         return d
     finally:

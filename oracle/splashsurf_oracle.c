@@ -571,7 +571,7 @@ static void stitch(so_result *res, so_patch *patches, uint64_t npatch) {
  *   sequential_generate_sparse_density_map (density_map.rs:370-412, support loop :677-736),
  *   construct_mc_input + triangulate (marching_cubes/narrow_band_extraction.rs:51-219, triangulation.rs:23-57). */
 static int reconstruct_global(so_result *res, const float *xyz, uint64_t n, const so_params *p, const so_grid *g,
-                              int64_t *neighbor_counts, const int64_t *nbr_off, int64_t *nbr_out) {
+                              int64_t *neighbor_counts, const int64_t *nbr_off, int64_t *nbr_out, int64_t tile_sub_flat, float *tile_out) {
     const float h = p->compact_support_radius, c = p->cube_size, thr = p->iso_surface_threshold;
     float r2 = p->particle_radius + p->particle_radius;
     const float rest_mass = (r2 * r2 * r2) * p->rest_density;
@@ -657,6 +657,17 @@ static int reconstruct_global(so_result *res, const float *xyz, uint64_t n, cons
                     if (rr < rev2) phi[(i * np1 + j) * np2 + k] += vol * k_scalar_eval(&kern, sqrtf(rr));
                 }
             }
+        }
+    }
+    /* debug tap: the 65^3 points of tile `tile_sub_flat` of the global grid cut into 64-cube tiles (the device's tiling of this
+     * path); points past the grid stay 0 */
+    if (tile_out && tile_sub_flat >= 0) {
+        const int64_t T = 64, tn = T + 1, nsd1 = (g->nc[1] + T - 1) / T, nsd2 = (g->nc[2] + T - 1) / T;
+        const int64_t ti = tile_sub_flat / (nsd1 * nsd2), tj = (tile_sub_flat / nsd2) % nsd1, tk = tile_sub_flat % nsd2;
+        memset(tile_out, 0, sizeof(float) * (size_t)(tn * tn * tn));
+        for (int64_t a = 0; a < tn; ++a) for (int64_t b = 0; b < tn; ++b) for (int64_t e = 0; e < tn; ++e) {
+            const int64_t i = ti * T + a, j = tj * T + b, k = tk * T + e;
+            if (i < np0 && j < np1 && k < np2) tile_out[(a * tn + b) * tn + e] = phi[(i * np1 + j) * np2 + k];
         }
     }
     /* ---- marching cubes input: vertices on edges from a point >= thr to a neighbour < thr */
@@ -804,7 +815,8 @@ void so_free(so_result *r) {
 }
 
 /* Optional debug taps: if tile_sub_flat >= 0, the level-set tile of that subdomain is copied to tile_out
- * ((S+1)^3 floats). */
+ * ((S+1)^3 floats; on the global path the tile of that flat index in 64-cube tiles of the global grid, 65^3 floats whatever S
+ * is, so tile_out must hold (max(S, 64) + 1)^3 floats). */
 int so_reconstruct(const float *xyz_in, uint64_t n_in, const so_params *p, so_result **out,
                    int64_t tile_sub_flat, float *tile_out, int64_t *neighbor_counts, const int64_t *nbr_off, int64_t *nbr_out) {
     so_result *res = (so_result *)calloc(1, sizeof(so_result));
@@ -839,7 +851,7 @@ int so_reconstruct(const float *xyz_in, uint64_t n_in, const so_params *p, so_re
         } else use_dec = 1;
     }
     res->used_decomposition = use_dec;
-    if (!use_dec) { int rcg = reconstruct_global(res, xyz, n, p, &g0, neighbor_counts, nbr_off, nbr_out); free(filtered); return rcg; }
+    if (!use_dec) { int rcg = reconstruct_global(res, xyz, n, p, &g0, neighbor_counts, nbr_off, nbr_out, tile_sub_flat, tile_out); free(filtered); return rcg; }
 
     /* dense_subdomains.rs:89-244 initialize_parameters */
     int64_t S = (int64_t)p->subdomain_num_cubes_per_dim;

@@ -149,6 +149,8 @@ def _bind(L):
     L.ss_surface_num_neighbors.restype = u64
     L.ss_surface_copy_neighbor_lists.argtypes = [vp, vp, vp]
     L.ss_context_keep_levelset_tile.argtypes = [vp, i64]
+    L.ss_context_keep_levelset_tile_raw.argtypes = [vp, i64]
+    L.ss_surface_copy_levelset_tile_raw.argtypes = [vp, vp, vp]
     L.ss_surface_timings.argtypes = [vp, C.POINTER(_Timings)]
     L.ss_surface_levelset_paths.argtypes = [vp, vp, C.c_int]
     L.ss_context_set_tile_batch.argtypes = [vp, C.c_uint32]

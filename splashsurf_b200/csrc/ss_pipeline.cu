@@ -124,7 +124,8 @@ struct ss_context {
     cudaEvent_t ev[12];
     uint32_t max_tiles = 0;          // 0 = auto
     int64_t keep_tile_flat = -1;
-    int ls_exact_all = 0;            // 1: evaluate every grid point exactly (no certification)
+    int64_t keep_raw_flat = -1;      // ss_context_keep_levelset_tile_raw (does not force exact evaluation)
+    int ls_exact_all = 0;           // 1: evaluate every grid point exactly (no certification)
     int ls_variant = 2;              // 2 (default): warp-per-brick certification + exact kernels (ss_certify.cuh, ss_exact.cuh); 1: CTA-per-brick certification kernel; 0: fused k_levelset
     int count_pairs = 0;             // 1: count in-support evaluations (work model; slower)
     int density_variant = 0;         // 0 (default): thread-per-particle k_density; 1 / 2: cell-cooperative kernel (ss_density.cuh), candidates staged by bulk copies / 16-byte loads
@@ -185,6 +186,8 @@ struct ss_surface {
     std::vector<int64_t> sub_flat; std::vector<uint64_t> sub_count; std::vector<uint8_t> sub_sparse, sub_owned;
     uint64_t max_particles = 0;
     std::vector<float> tile;
+    std::vector<float> tile_raw;     // ss_context_keep_levelset_tile_raw: the tile before the fix-up pass, and its per-brick states
+    std::vector<uint8_t> tile_raw_bstate;
     ss_timings tm{};
     uint64_t ls_paths[SS_LSP_N] = {};                        // ss_surface_levelset_paths
     // level-set field (ss_levelset_field_create_f32): the level set's device constants, its fold, whether records were binned
@@ -350,6 +353,7 @@ extern "C" void ss_context_destroy(ss_context *c) {
 }
 
 extern "C" int ss_context_keep_levelset_tile(ss_context *c, int64_t flat) { if (!c) return SS_ERR_INVALID_PARAMETER; c->keep_tile_flat = flat; return SS_OK; }
+extern "C" int ss_context_keep_levelset_tile_raw(ss_context *c, int64_t flat) { if (!c) return SS_ERR_INVALID_PARAMETER; c->keep_raw_flat = flat; return SS_OK; }
 extern "C" int ss_context_set_tile_batch(ss_context *c, uint32_t m) { if (!c) return SS_ERR_INVALID_PARAMETER; c->max_tiles = m; return SS_OK; }
 extern "C" int ss_context_set_levelset_exact_everywhere(ss_context *c, int on) { if (!c) return SS_ERR_INVALID_PARAMETER; c->ls_exact_all = on ? 1 : 0; return SS_OK; }
 extern "C" int ss_context_set_density_variant(ss_context *c, int v) {
@@ -904,7 +908,7 @@ static uint32_t launch_fold_levelset(ss_context *c, const SsDev &D, uint32_t nba
 // exact pass), brick classification, fix-up sweep.  Leaves the tiles, the per-brick states and the marching-cubes brick list
 // (c->list_mc, *n_mc_out entries) in the context scratch.
 static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsigned nbricks, bool exact_all, int certify_runs, bool global_mode,
-                          bool averaged, ss_surface *out, uint64_t &ls_launches, uint64_t &fix_points, uint32_t *n_mc_out) {
+                          bool averaged, ss_surface *out, uint64_t &ls_launches, uint64_t &fix_points, uint32_t *n_mc_out, int raw_q) {
     cudaStream_t st = c->stream;
     SsLsArgs A{};
     A.bins = context_bins(c); A.tiles = c->tiles.as<float>();
@@ -977,6 +981,15 @@ static int levelset_batch(ss_context *c, const SsDev &D, uint32_t nbatch, unsign
         }
     }
     out->tm.bricks_levelset += n_work;
+    if (raw_q >= 0) {
+        // raw tap (ss_context_keep_levelset_tile_raw): tile q as certification and exact pass left it -- markers where the sweep
+        // certified, before the fix-up pass replaces the ones next to outside points -- and its per-brick states
+        const size_t np3 = (size_t)D.np * D.np * D.np;
+        out->tile_raw.resize(np3); out->tile_raw_bstate.resize(nbricks);
+        CK(cudaMemcpyAsync(out->tile_raw.data(), c->tiles.as<float>() + (size_t)raw_q * np3, np3 * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(out->tile_raw_bstate.data(), c->bstate.as<uint8_t>() + (size_t)raw_q * nbricks, nbricks, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
     // bricks that can carry surface (for marching cubes) / markers next to outside points (for the fix-up sweep)
     const uint32_t nbr_b = nbatch * nbricks;
     c->flag_mc.ensure((size_t)nbr_b * 4); c->flag_fix.ensure((size_t)nbr_b * 4); c->off_mc.ensure((size_t)nbr_b * 4 + 4); c->off_fix.ensure((size_t)nbr_b * 4 + 4);
@@ -1399,7 +1412,7 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
     out->verts.ensure(vcap * 12); out->vkeys.ensure(vcap * 8); out->tris.ensure(tcap * 12);
     float ls_ms = 0.f, mc_ms = 0.f, setup_ms = 0.f;
     uint64_t ls_launches = 0, fix_points = 0;
-    out->tile.clear();
+    out->tile.clear(); out->tile_raw.clear(); out->tile_raw_bstate.clear();
     const bool exact_all = c->ls_exact_all || c->keep_tile_flat >= 0 || aniso || averaged;
     for (uint32_t s0 = 0; s0 < nown; s0 += (uint32_t)max_tiles) {
         const uint32_t nbatch = std::min<uint32_t>((uint32_t)max_tiles, nown - s0);
@@ -1426,7 +1439,10 @@ static int run_subdomain_grid(ss_context *c, const Prepared &PP, const ss_params
             setup_ms += su;
         }
         uint32_t n_mc = 0;
-        rc = levelset_batch(c, D, nbatch, nbricks, exact_all, certify_runs, global_mode, averaged, out, ls_launches, fix_points, &n_mc);
+        int raw_q = -1;
+        if (c->keep_raw_flat >= 0)
+            for (uint32_t q = 0; q < nbatch; ++q) if ((int64_t)h_flat[owned_list[s0 + q]] == c->keep_raw_flat) raw_q = (int)q;
+        rc = levelset_batch(c, D, nbatch, nbricks, exact_all, certify_runs, global_mode, averaged, out, ls_launches, fix_points, &n_mc, raw_q);
         if (rc) return rc;
         CK(cudaEventRecord(c->ev[11], st));
         // optional parity tap
@@ -2029,6 +2045,13 @@ extern "C" int ss_surface_copy_levelset_tile(const ss_surface *s, float *dst) {
     if (!s || !dst) return SS_ERR_INVALID_PARAMETER;
     if (s->tile.empty()) return ss_fail(SS_ERR_INVALID_PARAMETER, "no level-set tile was kept (ss_context_keep_levelset_tile)");
     memcpy(dst, s->tile.data(), s->tile.size() * 4);
+    return SS_OK;
+}
+extern "C" int ss_surface_copy_levelset_tile_raw(const ss_surface *s, float *tile, uint8_t *brick_state) {
+    if (!s) return SS_ERR_INVALID_PARAMETER;
+    if (s->tile_raw.empty()) return ss_fail(SS_ERR_INVALID_PARAMETER, "no raw level-set tile was kept (ss_context_keep_levelset_tile_raw)");
+    if (tile) memcpy(tile, s->tile_raw.data(), s->tile_raw.size() * 4);
+    if (brick_state) memcpy(brick_state, s->tile_raw_bstate.data(), s->tile_raw_bstate.size());
     return SS_OK;
 }
 extern "C" uint64_t ss_surface_num_neighbors(const ss_surface *s) { return (s && s->has_neighbors) ? s->n_neighbors : 0; }
