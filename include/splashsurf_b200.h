@@ -413,6 +413,22 @@ int ss_levelset_field_gradient_at_f32(ss_surface *field, const float *points, ui
 int ss_levelset_field_hessian_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *gradients, float *hessians);
 int ss_levelset_field_curvature_at_f32(ss_surface *field, const float *points, uint64_t m, float *values, float *curvatures);
 
+/* First crossing of the level-set field's surface along m rays or segments (DESIGN.md section 15).  Ray i is p(t) = o + t d
+ * (origins, directions: [m][3]) for t in [0, t_max[i]] (t_max NULL: +inf for every ray).  Samples are t = 0, then k dt for
+ * k = 1, 2, ... while k dt < t_max and k < 2^24, with dt = step / |d| (step is a length), then t_max itself if it is finite and > 0;
+ * the march also ends at the first sample outside the grid on an axis the ray does not move back from.  The first sample whose
+ * inside test (value > threshold, the values of ss_levelset_field_at_f32) differs from the origin's gives a bracket [a, b], halved
+ * up to `refine` times.  Per ray: status +1 (enters the liquid), -1 (leaves it), 0 (no crossing) or 2 (2^24 samples without a
+ * crossing); t = b, positions [m][3] = p(b), values = the field at p(b); without a crossing t = +inf and position, value (and
+ * gradient) NaN.  gradients ([m][3] or NULL): the gradient at the position, bit-identical to ss_levelset_field_gradient_at_f32.
+ * rounds (or NULL): the rounds the device march took.  A segment x0 -> x1 is o = x0, d = x1 - x0, t_max = 1.  All arrays in host
+ * or device memory.  SS_ERR_INVALID_PARAMETER for NULL arrays, step not finite or <= 0, refine > 64, a stale field, and (naming
+ * the first such ray) a non-finite origin or direction, a zero direction or a zero or non-finite dt, a NaN or negative t_max;
+ * SS_ERR_INDEX_TOO_SMALL for m >= 2^31 - 1; SS_ERR_UNSUPPORTED for gradients on a field created with the Jacobian correction on.
+ * The tier counters of ss_levelset_field_paths are summed over the call's rounds and its gradient pass. */
+int ss_levelset_field_raycast_f32(ss_surface *field, const float *origins, const float *directions, const float *t_max, uint64_t m, float step,
+                                  uint32_t refine, float *t, float *positions, float *values, int8_t *status, float *gradients, uint64_t *rounds);
+
 /* Narrow-band signed distance grid of a mesh on the field's lattice (DESIGN.md section 14).  The lattice is the field's grid
  * (ss_surface_grid): points min + index * cell_size, index in [0, n] per axis, in bricks of 8 x 8 x 8 points (ceil((n + 1) / 8) per
  * axis).  B = band * cell_size (band in [1, 8]).  d(p) is the f32 minimum over all triangles of the point-triangle distance, every

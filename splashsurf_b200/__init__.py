@@ -27,7 +27,7 @@ from . import build as _build
 __all__ = ["reconstruct_surface", "reconstruction_pipeline", "marching_cubes", "marching_cubes_cleanup", "barnacle_decimation", "convert_tris_to_quads",
            "laplacian_smoothing_parallel", "laplacian_smoothing_normals_parallel", "check_mesh_consistency", "neighborhood_search_spatial_hashing_parallel",
            "SphInterpolator", "run_splashsurf", "run_pysplashsurf", "TriMesh3d", "MixedTriQuadMesh3d", "MeshWithData", "MeshAttribute", "MeshType",
-           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "LevelSetField", "SignedDistanceGrid", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
+           "SurfaceReconstruction", "Anisotropy", "AveragedSurface", "JacobianCorrection", "LevelSetField", "RayHits", "SignedDistanceGrid", "UniformGrid", "Aabb3d", "NeighborhoodLists", "VertexVertexConnectivity",
            "density_grid_loop", "write_mesh", "Context", "default_context", "make_params", "SplashsurfError", "library_path", "load_library"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -214,6 +214,7 @@ def _bind(L):
     L.ss_levelset_field_curvature_at_f32.argtypes = [vp, vp, C.c_uint64, vp, vp]
     L.ss_levelset_field_threshold_f32.argtypes = [vp, C.POINTER(C.c_float)]
     L.ss_levelset_field_paths.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.ss_levelset_field_raycast_f32.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_float, C.c_uint32, vp, vp, vp, vp, vp, C.POINTER(C.c_uint64)]
     L.ss_levelset_field_sdf_f32.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint32, C.POINTER(vp)]
     L.ss_sdf_num_bricks.argtypes = [vp]
     L.ss_sdf_num_bricks.restype = C.c_uint64
@@ -1224,6 +1225,77 @@ class LevelSetField:
         """``evaluate(points) > threshold``."""
         return self.evaluate(points) > self.threshold
 
+    def raycast(self, origins, directions, *, t_max=None, step: Optional[float] = None, refine: int = 24, normals: bool = True) -> "RayHits":
+        """First crossing of the surface along each ray ``origins + t * directions``, ``0 <= t <= t_max`` (DESIGN.md section 15), for
+        collision, visibility, ray-marched previews and depth probes without a mesh.
+
+        The field is sampled ``step`` apart in length (default half a cell; a crossing closer to the origin than that, or two
+        crossings within one step, can be missed), and the first sample whose inside test differs from the origin's is refined by
+        ``refine`` bisection steps (0 to 64).  ``t`` is measured in units of ``directions``: a segment ``x0 -> x1`` is
+        ``raycast(x0, x1 - x0, t_max=1.0)``.  ``t_max`` is None (+inf), a float, or an (M,) array.
+
+        ``origins`` and ``directions`` are (M, 3) float32 numpy arrays (numpy results) or CUDA float32 torch tensors (CUDA results);
+        float64 raises ``TypeError``.  The result's ``status`` is +1 where the ray enters the liquid, -1 where it leaves it, 0
+        without a crossing and 2 where 2^24 samples found none; ``positions`` is the first point found on the far side, within one
+        ``step * 2^-refine`` of the crossing along the ray, and ``values`` the field there, equal to ``evaluate(positions)`` bit for
+        bit.  ``normals`` (``normals=True``) are those of ``normals(positions)``.  A field of the Jacobian-corrected averaged surface
+        has no gradient: pass ``normals=False`` there, or ``SplashsurfError`` is raised."""
+        L = self._ctx._L
+        cuda = hasattr(origins, "data_ptr") and getattr(origins, "is_cuda", False)
+        if cuda:
+            import torch
+            o, d = origins, directions
+            if o.dtype != torch.float32 or not hasattr(d, "data_ptr") or d.dtype != torch.float32:
+                raise TypeError("unsupported scalar type: rays are cast from float32 origins and directions only")
+            d = d.to(o.device)
+        else:
+            o, d = np.asarray(origins), np.asarray(directions)
+            if o.dtype != np.float32 or d.dtype != np.float32:
+                raise TypeError("unsupported scalar type: rays are cast from float32 origins and directions only")
+        if o.ndim != 2 or o.shape[1] != 3 or tuple(d.shape) != tuple(o.shape):
+            raise ValueError("origins and directions must have the same shape (M, 3)")
+        m = int(o.shape[0])
+        step = 0.5 * self.grid.cell_size if step is None else float(step)
+        if cuda:
+            o, d = o.contiguous(), d.contiguous()
+            tm = None
+            if t_max is not None:
+                if getattr(t_max, "dtype", None) in (torch.float64, np.float64) and getattr(t_max, "ndim", 0):
+                    raise TypeError("unsupported scalar type: t_max must be float32")
+                tm = torch.as_tensor(t_max, dtype=torch.float32, device=o.device)
+                tm = (tm.expand(m) if tm.ndim == 0 else tm).contiguous()
+            new = lambda *sh, dt=torch.float32: torch.empty((m,) + sh, dtype=dt, device=o.device)  # noqa: E731
+            out = [new(), new(3), new(), new(dt=torch.int8)]
+            grad = new(3) if normals else None
+            torch.cuda.current_stream(o.device).synchronize()
+            ptr = lambda a: a.data_ptr() if m and a is not None else None  # noqa: E731
+        else:
+            o, d = np.ascontiguousarray(o), np.ascontiguousarray(d)
+            tm = None
+            if t_max is not None:
+                tm = np.asarray(t_max)
+                if tm.dtype.kind == "f" and tm.dtype != np.float32 and tm.ndim:
+                    raise TypeError("unsupported scalar type: t_max must be float32")
+                tm = np.ascontiguousarray(np.broadcast_to(tm.astype(np.float32), (m,)))
+            out = [np.empty(m, np.float32), np.empty((m, 3), np.float32), np.empty(m, np.float32), np.empty(m, np.int8)]
+            grad = np.empty((m, 3), np.float32) if normals else None
+            ptr = lambda a: a.ctypes.data if m and a is not None else None  # noqa: E731
+        if tm is not None and tuple(tm.shape) != (m,):
+            raise ValueError("t_max must be a float or have shape (M,)")
+        rounds = C.c_uint64()
+        _check(L, L.ss_levelset_field_raycast_f32(self._s, ptr(o), ptr(d), ptr(tm), m, C.c_float(step), int(refine), *[ptr(a) for a in out],
+                                                  ptr(grad), C.byref(rounds)))
+        hits = RayHits()
+        hits.t, hits.positions, hits.values, hits.status = out
+        hits.gradients, hits.rounds, hits.normals = grad, int(rounds.value), None
+        if grad is not None:
+            if cuda:
+                hits.normals = -grad / grad.norm(dim=1, keepdim=True)
+            else:
+                with np.errstate(invalid="ignore", divide="ignore"):
+                    hits.normals = (-grad / np.linalg.norm(grad, axis=1, keepdims=True)).astype(np.float32)
+        return hits
+
     def signed_distance(self, mesh, *, band: int = 3) -> "SignedDistanceGrid":
         """Narrow-band signed distance grid of ``mesh`` on this field's lattice (DESIGN.md section 14): per brick of 8^3 grid points
         within ``band`` cells of the mesh, the f32 distance to the nearest triangle clamped to the background ``band * cell_size``,
@@ -1293,6 +1365,16 @@ class LevelSetField:
             self.close()
         except Exception:
             pass
+
+
+class RayHits:
+    """First crossings of ``LevelSetField.raycast`` (DESIGN.md section 15), per ray: ``t`` (M,) float32 (+inf without a crossing),
+    ``positions`` (M, 3) float32 ``origin + t * direction``, ``values`` (M,) float32 the field there, ``status`` (M,) int8 (+1 enters
+    the liquid, -1 leaves it, 0 no crossing, 2 sample limit), and with ``normals=True`` ``gradients`` and ``normals`` (M, 3) float32
+    at the positions (NaN without a crossing); positions and values are NaN without a crossing.  ``rounds``: the rounds the device
+    march took.  Numpy arrays or CUDA tensors, like the rays."""
+    t = positions = values = status = gradients = normals = None
+    rounds = 0
 
 
 class SignedDistanceGrid:

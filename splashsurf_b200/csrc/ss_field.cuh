@@ -6,8 +6,9 @@
 // with their brick folds unchanged (SsAnisoFold, ss_aniso.cuh; SsAvgFold, SsAvgCorrFold, SsAvgRadFold, SsAvgCorrRadFold,
 // ss_averaged.cuh).  Points no candidate reaches are 0.
 //
-//   k_field_keys      per point: group key (compressed subdomain, brick of its cell), or value 0 at once (outside the grid, subdomain
-//                     without members); the first non-finite coordinate
+//   k_field_keys      per point: group key (compressed subdomain, brick of its cell; ss_field_key, which the ray march of
+//                     ss_raycast.cuh shares), or value 0 at once (outside the grid, subdomain without members); the first non-finite
+//                     coordinate
 //   k_field_starts    after the key sort: first point of every group
 //   k_field_fold      warp per (subdomain, brick) group: the candidates of the group's bins staged and sorted as for a brick
 //                     (ss_stage_candidates), then per batch of 32 points the candidates within h of the batch's bounding box
@@ -472,6 +473,41 @@ __device__ __forceinline__ void ss_field_store(const SsDev &P, const SsFieldArgs
     }
 }
 
+// The cell of a point in the grid, clamped (a point on the grid's upper face belongs to the last cell); false outside [gmin, gmax]
+// along an axis (gc then 0 from that axis on).  finite: whether every coordinate is finite.
+__device__ __forceinline__ bool ss_field_cell(const SsDev &P, const float (&p)[3], float3 gmax, int (&gc)[3], bool &finite) {
+    const float hi[3] = { gmax.x, gmax.y, gmax.z };
+    bool inside = true;
+    finite = true;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        finite = finite && isfinite(p[d]);
+        inside = inside && p[d] >= P.gmin[d] && p[d] <= hi[d];
+        gc[d] = inside ? min(max(ss_cell_of(p[d], P.gmin[d], P.c), 0), P.nsd[d] * P.S - 1) : 0;
+    }
+    return inside;
+}
+
+// The group key of a point (k_field_keys, ss_raycast.cuh): compressed subdomain * nb^3 + (bx * nb + by) * nb + bz of its cell, or
+// 0xffffffff outside [gmin, gmax] along an axis, in a subdomain without members (sub_flat: the nsub subdomains with members,
+// ascending) or at a non-finite coordinate.
+__device__ __forceinline__ uint32_t ss_field_key(const SsDev &P, const float (&p)[3], float3 gmax, const uint32_t *__restrict__ sub_flat, uint32_t nsub,
+                                                 bool &finite) {
+    int gc[3];
+    const bool inside = ss_field_cell(P, p, gmax, gc, finite);
+    uint32_t k = 0xffffffffu;
+    if (finite && inside) {
+        int sd[3], lb[3];
+#pragma unroll
+        for (int d = 0; d < 3; ++d) { sd[d] = gc[d] / P.S; lb[d] = (gc[d] - sd[d] * P.S) >> 3; }
+        const uint32_t flat = (uint32_t)(((int64_t)sd[0] * P.nsd[1] + sd[1]) * P.nsd[2] + sd[2]);
+        uint32_t lo = 0, up = nsub;                             // sub_flat is ascending
+        while (lo < up) { const uint32_t mid = (lo + up) >> 1; if (sub_flat[mid] < flat) lo = mid + 1; else up = mid; }
+        if (lo < nsub && sub_flat[lo] == flat) k = lo * (uint32_t)(P.nb * P.nb * P.nb) + (uint32_t)((lb[0] * P.nb + lb[1]) * P.nb + lb[2]);
+    }
+    return k;
+}
+
 // Points outside [gmin, gmax] along an axis, or in a subdomain without members, get 0 and key 0xffffffff (sorted last); chk[0]:
 // lowest index with a non-finite coordinate (preset 0xffffffff), chk[1]: points with a group (preset 0).
 __global__ void k_field_keys(SsDev P, const float *__restrict__ pts, uint32_t m, float3 gmax, const uint32_t *__restrict__ sub_flat, uint32_t nsub,
@@ -480,30 +516,10 @@ __global__ void k_field_keys(SsDev P, const float *__restrict__ pts, uint32_t m,
     bool grouped = false;
     if (i < m) {
         const float p[3] = { pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2] };
-        const float hi[3] = { gmax.x, gmax.y, gmax.z };
-        bool finite = true, inside = true;
-        int gc[3];
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-            finite = finite && isfinite(p[d]);
-            inside = inside && p[d] >= P.gmin[d] && p[d] <= hi[d];
-            // the cell of the point, clamped: a point on the grid's upper face belongs to the last cell
-            gc[d] = inside ? min(max(ss_cell_of(p[d], P.gmin[d], P.c), 0), P.nsd[d] * P.S - 1) : 0;
-        }
+        bool finite;
+        const uint32_t k = ss_field_key(P, p, gmax, sub_flat, nsub, finite);
         if (!finite) atomicMin(&chk[0], i);
-        uint32_t k = 0xffffffffu;
-        if (finite && inside) {
-            int sd[3], lb[3];
-#pragma unroll
-            for (int d = 0; d < 3; ++d) { sd[d] = gc[d] / P.S; lb[d] = (gc[d] - sd[d] * P.S) >> 3; }
-            const uint32_t flat = (uint32_t)(((int64_t)sd[0] * P.nsd[1] + sd[1]) * P.nsd[2] + sd[2]);
-            uint32_t lo = 0, up = nsub;                             // sub_flat is ascending
-            while (lo < up) { const uint32_t mid = (lo + up) >> 1; if (sub_flat[mid] < flat) lo = mid + 1; else up = mid; }
-            if (lo < nsub && sub_flat[lo] == flat) {
-                k = lo * (uint32_t)(P.nb * P.nb * P.nb) + (uint32_t)((lb[0] * P.nb + lb[1]) * P.nb + lb[2]);
-                grouped = true;
-            }
-        }
+        grouped = k != 0xffffffffu;
         key[i] = k; idx[i] = i; out[i] = 0.0f;
     }
     const unsigned w = __ballot_sync(0xffffffffu, grouped);

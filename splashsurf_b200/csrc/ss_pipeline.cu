@@ -11,6 +11,7 @@
 #include "ss_aniso.cuh"
 #include "ss_averaged.cuh"
 #include "ss_field.cuh"
+#include "ss_raycast.cuh"
 #include "ss_sdf.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
@@ -152,6 +153,8 @@ struct ss_context {
     // level-set field queries (ss_field.cuh): points, group keys and caller indices (sorted and not), group starts, values, checks,
     // and the candidate bin ranges of a group
     DevBuf fld_pts, fld_key_a, fld_key_b, fld_idx_a, fld_idx_b, fld_flag, fld_off, fld_starts, fld_out, fld_chk, fld_rng, fld_grad, fld_hess, fld_curv;
+    // ray casts (ss_raycast.cuh): the caller's origins, directions and t_max, per-ray state, results, checks and the keyed-ray count
+    DevBuf ray_o, ray_d, ray_tmax, ray_state, ray_t, ray_pos, ray_val, ray_status, ray_grad, ray_chk, ray_hits;
     uint64_t launches = 0;
     uint64_t pack_n = 0; uint32_t pack_world = 0;   // ss_partition_pack_f32: count phase the scatter phase must match
     // result buffers handed to surfaces and returned by ss_surface_free (avoids cudaMalloc/cudaFree per frame,
@@ -2283,6 +2286,137 @@ extern "C" int ss_levelset_field_paths(const ss_surface *f, uint64_t out[3]) {
     if (!f || !f->fld || !out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or not a level-set field");
     for (int t = 0; t < 3; ++t) out[t] = f->fld_paths[t];
     return SS_OK;
+}
+
+// ------------------------------------------------------------------ first crossings along rays ----
+// DESIGN.md §15.  Rounds of k_ray_keys, the key sort and group starts of a field query, and the cascade of k_ray_fold / k_ray_select
+// with the mode's value fold, until every ray is done; then the gradient fold at the hits through field_run.
+template <class F>
+static void ray_fold(ss_context *c, const SsDev &D, const SsRayArgs &Q0, uint32_t n_groups, uint64_t *received) {
+    uint64_t launches = 0;
+    const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+        SsRayArgs Q = Q0;
+        Q.F.groups = list; Q.F.n_groups = n; Q.F.fallback = left;
+        return Q;
+    };
+    run_cascade(c, nullptr, n_groups, {
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) {
+            LAUNCH(c, (k_ray_fold<F, SS_AN_CAP, SS_FLD_WARPS>), (n + SS_FLD_WARPS - 1) / SS_FLD_WARPS, SS_FLD_WARPS * 32, D, args(list, n, left));
+        },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, (k_ray_fold<F, SS_AN_BIG_CAP, 1>), n, 32, D, args(list, n, left)); },
+        [&](const uint32_t *list, uint32_t n, uint32_t *left) { LAUNCH(c, k_ray_select<F>, n, 32, D, args(list, n, left)); },
+    }, launches, received);
+}
+
+extern "C" int ss_levelset_field_raycast_f32(ss_surface *f, const float *origins, const float *directions, const float *t_max, uint64_t m,
+                                             float step, uint32_t refine, float *t, float *positions, float *values, int8_t *status,
+                                             float *gradients, uint64_t *rounds) {
+    int rc; ss_context *c = field_context(f, &rc);
+    if (!c) return rc;
+    if (rounds) *rounds = 0;
+    if (m && (!origins || !directions || !t || !positions || !values || !status)) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    if (!(std::isfinite(step) && step > 0.0f)) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set raycast: step has to be finite and > 0");
+    if (refine > 64) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set raycast: refine has to lie in [0, 64]");
+    if (m >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "too many rays for one call");
+    if (gradients && (f->fld_mode == SS_FLD_AVG_CORR || f->fld_mode == SS_FLD_AVG_CORR_RAD))
+        return ss_fail(SS_ERR_UNSUPPORTED, "level-set field: the Jacobian-corrected averaged surface has no gradient (DESIGN.md 13.1)");
+    for (uint64_t &q : f->fld_paths) q = 0;
+    if (!m) return SS_OK;
+    return ss_guard([&]() -> int {
+        CK(cudaSetDevice(c->device));
+        cudaStream_t st = c->stream;
+        const SsDev &D = f->fld_D;
+        const uint32_t m32 = (uint32_t)m;
+        c->ray_o.ensure((size_t)m32 * 12); c->ray_d.ensure((size_t)m32 * 12); c->ray_state.ensure((size_t)m32 * sizeof(SsRay));
+        c->ray_t.ensure((size_t)m32 * 4); c->ray_pos.ensure((size_t)m32 * 12); c->ray_val.ensure((size_t)m32 * 4); c->ray_status.ensure(m32);
+        c->ray_chk.ensure(16);
+        CK(cudaMemcpyAsync(c->ray_o.p, origins, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(c->ray_d.p, directions, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        if (t_max) {
+            c->ray_tmax.ensure((size_t)m32 * 4);
+            CK(cudaMemcpyAsync(c->ray_tmax.p, t_max, (size_t)m32 * 4, cudaMemcpyDefault, st));
+        }
+        SsRayOut O{ c->ray_t.as<float>(), c->ray_pos.as<float>(), c->ray_val.as<float>(), c->ray_status.as<int8_t>() };
+        uint32_t chk[4] = { 0xffffffffu, 0xffffffffu, 0xffffffffu, 0u };
+        CK(cudaMemcpyAsync(c->ray_chk.p, chk, 16, cudaMemcpyHostToDevice, st));
+        LAUNCH(c, k_ray_init, nblk(m32, 256), 256, c->ray_o.as<float>(), c->ray_d.as<float>(), t_max ? c->ray_tmax.as<float>() : nullptr, m32, step,
+               c->ray_state.as<SsRay>(), O, c->ray_chk.as<uint32_t>());
+        CK(cudaMemcpyAsync(chk, c->ray_chk.p, 16, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        static const char *const what[3] = { "has a non-finite origin or direction", "has a zero direction, or a step / |direction| of 0 or not finite",
+                                             "has a NaN or negative t_max" };
+        for (int q = 0; q < 3; ++q) {
+            if (chk[q] == 0xffffffffu) continue;
+            char msg[200];
+            snprintf(msg, sizeof msg, "level-set raycast: ray %u %s", chk[q], what[q]);
+            return ss_fail(SS_ERR_INVALID_PARAMETER, msg);
+        }
+        SsRayArgs Q{};
+        Q.F.A.bins = context_bins(c); Q.F.A.bins.brick_rng = c->fld_rng.as<int2>();
+        Q.F.A.grec = c->an_grec.as<float4>(); Q.F.A.rrec = c->av_rrec.as<float>();
+        Q.rays = c->ray_state.as<SsRay>(); Q.O = O;
+        Q.gmax = make_float3(f->grid.mx[0], f->grid.mx[1], f->grid.mx[2]);
+        Q.sub_flat = c->sub_flat.as<uint32_t>(); Q.nsub = f->fld_ready ? f->fld_nsub : 0u;   // no records: every point is 0
+        Q.refine = refine;
+        c->fld_key_a.ensure((size_t)m32 * 4); c->fld_key_b.ensure((size_t)m32 * 4); c->fld_idx_a.ensure((size_t)m32 * 4); c->fld_idx_b.ensure((size_t)m32 * 4);
+        c->fld_chk.ensure(8);
+        uint64_t nround = 0;
+        for (;;) {
+            // one round: the keyed rays' count (the round's synchronisation), their groups, the cascade
+            CK(cudaMemsetAsync(c->fld_chk.p, 0, 4, st));
+            LAUNCH(c, k_ray_keys, nblk(m32, 256), 256, D, Q, m32, c->fld_key_a.as<uint32_t>(), c->fld_idx_a.as<uint32_t>(), c->fld_chk.as<uint32_t>());
+            uint32_t nact = 0;
+            CK(cudaMemcpyAsync(&nact, c->fld_chk.p, 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            if (!nact) break;
+            ++nround;
+            cub_sort(c, c->fld_key_a.as<uint32_t>(), c->fld_key_b.as<uint32_t>(), nact, 32, c->fld_idx_a.as<uint32_t>(), c->fld_idx_b.as<uint32_t>());
+            c->fld_flag.ensure((size_t)nact * 4); c->fld_off.ensure((size_t)nact * 4 + 4); c->fld_starts.ensure((size_t)nact * 4 + 4);
+            LAUNCH(c, k_field_starts, nblk(nact, 256), 256, c->fld_key_b.as<uint32_t>(), nact, c->fld_flag.as<uint32_t>());
+            uint32_t lc[2] = { 0, 0 };
+            scan_compact(c, c->fld_flag.as<uint32_t>(), c->fld_off.as<uint32_t>(), nact, c->fld_starts.as<uint32_t>(), lc);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t n_groups = lc[0] + lc[1];
+            CK(cudaMemcpyAsync(c->fld_starts.as<uint32_t>() + n_groups, &nact, 4, cudaMemcpyHostToDevice, st));
+            Q.F.key = c->fld_key_b.as<uint32_t>(); Q.F.idx = c->fld_idx_b.as<uint32_t>(); Q.F.starts = c->fld_starts.as<uint32_t>();
+            switch (f->fld_mode) {
+            case SS_FLD_ANISO: ray_fold<SsAnisoFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG: ray_fold<SsAvgFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_CORR: ray_fold<SsAvgCorrFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_RAD: ray_fold<SsAvgRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+            case SS_FLD_AVG_CORR_RAD: ray_fold<SsAvgCorrRadFold>(c, D, Q, n_groups, f->fld_paths); break;
+            default: ray_fold<SsSphFold>(c, D, Q, n_groups, f->fld_paths); break;
+            }
+        }
+        if (rounds) *rounds = nround;
+        CK(cudaMemcpyAsync(t, c->ray_t.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(positions, c->ray_pos.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(values, c->ray_val.p, (size_t)m32 * 4, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(status, c->ray_status.p, m32, cudaMemcpyDefault, st));
+        if (gradients) {
+            // the gradient fold at the hits, packed, then scattered: gradient(position) bit for bit, NaN where there is no hit
+            c->ray_grad.ensure((size_t)m32 * 12);
+            LAUNCH(c, k_ray_fill_nan, nblk((uint64_t)m32 * 3, 256), 256, c->ray_grad.as<float>(), (uint64_t)m32 * 3);
+            c->fld_flag.ensure((size_t)m32 * 4); c->fld_off.ensure((size_t)m32 * 4 + 4);
+            c->ray_hits.ensure((size_t)m32 * 4);
+            LAUNCH(c, k_ray_hit_flags, nblk(m32, 256), 256, c->ray_status.as<int8_t>(), m32, c->fld_flag.as<uint32_t>());
+            uint32_t lc[2] = { 0, 0 };
+            scan_compact(c, c->fld_flag.as<uint32_t>(), c->fld_off.as<uint32_t>(), m32, c->ray_hits.as<uint32_t>(), lc);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t nh = lc[0] + lc[1];
+            if (nh) {
+                c->fld_pts.ensure((size_t)nh * 12); c->fld_out.ensure((size_t)nh * 4); c->fld_grad.ensure((size_t)nh * 12);
+                CK(cudaMemsetAsync(c->fld_grad.p, 0, (size_t)nh * 12, st));           // points without candidates: gradient 0
+                LAUNCH(c, k_ray_gather, nblk(nh, 256), 256, c->ray_hits.as<uint32_t>(), nh, c->ray_pos.as<float>(), c->fld_pts.as<float>());
+                const int rc = field_run(f, c, c->fld_pts.as<float>(), nh, c->fld_out.as<float>(), c->fld_grad.as<float>());
+                if (rc) return rc;
+                LAUNCH(c, k_ray_scatter_hits, nblk(nh, 256), 256, c->ray_hits.as<uint32_t>(), nh, c->fld_grad.as<float>(), c->ray_grad.as<float>());
+            }
+            CK(cudaMemcpyAsync(gradients, c->ray_grad.p, (size_t)m32 * 12, cudaMemcpyDefault, st));
+        }
+        CK(cudaStreamSynchronize(st));
+        return SS_OK;
+    });
 }
 
 // ------------------------------------------------------------------ narrow-band signed distance grid ----
