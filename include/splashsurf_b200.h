@@ -381,8 +381,8 @@ int ss_context_set_averaged_radii_f32(ss_context *ctx, const float *radii /* NUL
  * the same context (SS_ERR_INVALID_PARAMETER afterwards).
  * ss_levelset_field_at_f32: m points (m x 3 floats) -> m values; both arrays in host or device memory.  A non-finite coordinate is
  * SS_ERR_INVALID_PARAMETER naming the first such point.
- * ss_levelset_field_paths: the point groups of the last query per tier of the cascade: out[0] 512-slot slice, out[1] 4096-slot
- * slice, out[2] selection walk. */
+ * ss_levelset_field_paths: the work of the last query per tier of the cascade: out[0] 512-slot slice, out[1] 4096-slot slice,
+ * out[2] selection walk -- point groups, or listed lattice bricks after ss_levelset_field_mesh_f32. */
 int ss_levelset_field_create_f32(ss_context *ctx, const float *xyz, uint64_t n, const ss_params_f32 *params, ss_surface **out);
 int ss_levelset_field_at_f32(ss_surface *field, const float *points, uint64_t m, float *out);
 int ss_levelset_field_threshold_f32(const ss_surface *field, float *threshold);
@@ -457,6 +457,23 @@ int ss_sdf_paths(const ss_sdf *sdf, uint64_t out[2]);
 void ss_sdf_set_pass_pairs(uint64_t pairs);
 int ss_sdf_passes(const ss_sdf *sdf, uint64_t out[2]);
 void ss_sdf_free(ss_sdf *sdf);
+
+/* ss_levelset_field_mesh_f32 (DESIGN.md section 16): the field's surface meshed over a box at any cube size.  Lattice point I (global
+ * index per axis) lies at (float)I * cube_size rounded, then + the grid's min rounded, and gets the value ss_levelset_field_at_f32
+ * returns there; cube_size <= 0 selects the field's cell.  The index range per axis is [0, n] at the field's cell and
+ * [0, ceil(n cell / cube_size)] otherwise; a box (aabb_min and aabb_max, both or neither) narrows it to [floor((min - gmin) / cube_size),
+ * ceil((max - gmin) / cube_size)].  Marching cubes as the reconstruction's subdomain path runs it, vertices welded by global edge key;
+ * the mesh is open where the surface leaves the box.  With cube_size <= 0 and no box the result is the raw mesh of the field's
+ * reconstruction (simd off for the standard level set) bit for bit, up to vertex and triangle order.  The result is a surface with a
+ * mesh (ss_surface_copy_vertices / _triangles_u32 / _vertex_edge_keys with global lattice indices; ss_surface_free); it owns its
+ * arrays.  ss_levelset_field_paths counts the listed bricks per tier.  SS_ERR_INVALID_PARAMETER: a non-finite box or cube size,
+ * aabb_min > aabb_max, one of the two NULL, a stale field; SS_ERR_INDEX_TOO_SMALL: a lattice index above 2^20 - 1;
+ * SS_ERR_UNSUPPORTED: a negative threshold.
+ * ss_levelset_mesh_info: the cube size, the index range and the number of batches of such a mesh.
+ * ss_levelset_mesh_set_batch_tiles: at most this many 64^3-cell tiles per batch (0: a third of the free device memory decides). */
+int ss_levelset_field_mesh_f32(ss_surface *field, const float *aabb_min, const float *aabb_max, float cube_size, ss_surface **out);
+int ss_levelset_mesh_info(const ss_surface *mesh, float *cube_size, int64_t index_min[3], int64_t index_max[3], uint64_t *batches);
+void ss_levelset_mesh_set_batch_tiles(uint32_t tiles);
 
 /* ---- Mesh post-processing on the device (SURVEY.md 8f; the steps of splashsurf/src/reconstruct.rs:1094-1391 that follow the
  * reconstruction).  They operate in place on the surface's device mesh; copy results out with the accessors above.

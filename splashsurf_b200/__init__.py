@@ -226,6 +226,10 @@ def _bind(L):
     L.ss_sdf_set_pass_pairs.restype = None
     L.ss_sdf_free.argtypes = [vp]
     L.ss_sdf_free.restype = None
+    L.ss_levelset_field_mesh_f32.argtypes = [vp, vp, vp, C.c_float, C.POINTER(vp)]
+    L.ss_levelset_mesh_info.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]
+    L.ss_levelset_mesh_set_batch_tiles.argtypes = [C.c_uint32]
+    L.ss_levelset_mesh_set_batch_tiles.restype = None
     L.ss_surface_anisotropy_ms.restype = C.c_float
     if L.ss_abi_version() != 3:
         raise ImportError("libsplashsurf_b200.so ABI version mismatch")
@@ -1346,9 +1350,34 @@ class LevelSetField:
         finally:
             L.ss_sdf_free(h)
 
+    def mesh(self, cube_size: Optional[float] = None, *, aabb_min: Optional[Sequence[float]] = None,
+             aabb_max: Optional[Sequence[float]] = None) -> "LevelSetMesh":
+        """The field's surface as a triangle mesh over a box at any cube size, on the GPU (DESIGN.md section 16).  Lattice point
+        ``I`` lies at ``gmin + I * cube_size`` (f32, ``(float)I * cube_size`` rounded, then ``+ gmin`` rounded) and gets the value
+        ``evaluate`` returns there; ``cube_size=None`` is the field's cell.  The box (``aabb_min`` and ``aabb_max``, both or neither)
+        selects the lattice indices ``floor((min - gmin) / cube_size) .. ceil((max - gmin) / cube_size)`` within the field's grid;
+        the mesh is open where the surface leaves the box.  With the defaults the mesh is the raw mesh of ``reconstruct_surface``
+        with this field's keywords (``simd=False`` for the standard level set), bit for bit up to vertex and triangle order, so a
+        close-up at a finer cube size or a coarse preview needs no second reconstruction."""
+        L = self._ctx._L
+        if (aabb_min is None) != (aabb_max is None):
+            raise ValueError("give both aabb_min and aabb_max, or neither")
+        box = [None, None]
+        if aabb_min is not None:
+            box = [(C.c_float * 3)(*[float(x) for x in aabb_min]), (C.c_float * 3)(*[float(x) for x in aabb_max])]
+        cs = 0.0 if cube_size is None else float(cube_size)
+        h = C.c_void_p()
+        _check(L, L.ss_levelset_field_mesh_f32(self._s, box[0], box[1], C.c_float(cs), C.byref(h)))
+        try:
+            return LevelSetMesh._from(L, h, self.paths)
+        finally:
+            L.ss_surface_free(h)
+
     @property
     def paths(self) -> dict:
-        """The point groups of the last ``evaluate`` per tier of the cascade: 512-slot slice, 4096-slot slice, selection walk."""
+        """The work of the last query per tier of the cascade (512-slot slice, 4096-slot slice, selection walk): point groups after
+        ``evaluate``, ``gradient``, ``hessian``, ``curvature``, ``raycast`` and ``signed_distance``; listed lattice bricks after
+        ``mesh``."""
         out = (C.c_uint64 * 3)()
         _check(self._ctx._L, self._ctx._L.ss_levelset_field_paths(self._s, out))
         return {"512": int(out[0]), "4096": int(out[1]), "select": int(out[2])}
@@ -1365,6 +1394,33 @@ class LevelSetField:
             self.close()
         except Exception:
             pass
+
+
+class LevelSetMesh:
+    """The result of ``LevelSetField.mesh`` (DESIGN.md section 16): ``mesh`` a ``TriMesh3d`` (float32 vertices, uint64 triangles, as
+    ``reconstruct_surface`` returns them), ``vertex_edge_keys`` (V, 4) int64 -- the global lattice point and axis of each vertex's
+    edge --, ``cube_size``, the lattice index range ``index_min`` / ``index_max`` (3,) int64, ``paths`` (listed bricks per tier of
+    the fold: 512-slot slice, 4096-slot slice, selection walk) and ``batches`` (tile batches the call ran)."""
+    mesh = vertex_edge_keys = index_min = index_max = paths = None
+    cube_size = 0.0
+    batches = 0
+
+    @classmethod
+    def _from(cls, L, h, paths) -> "LevelSetMesh":
+        r = cls()
+        nv, nt = L.ss_surface_num_vertices(h), L.ss_surface_num_triangles(h)
+        verts, tris, keys = np.empty((nv, 3), np.float32), np.empty((nt, 3), np.uint64), np.empty((nv, 4), np.int64)
+        if nv:
+            _check(L, L.ss_surface_copy_vertices(h, verts.ctypes.data))
+            _check(L, L.ss_surface_copy_vertex_edge_keys(h, keys.ctypes.data))
+        if nt:
+            _check(L, L.ss_surface_copy_triangles_u64(h, tris.ctypes.data))
+        cs, lo, hi, nb = C.c_float(), (C.c_int64 * 3)(), (C.c_int64 * 3)(), C.c_uint64()
+        _check(L, L.ss_levelset_mesh_info(h, C.byref(cs), lo, hi, C.byref(nb)))
+        r.mesh, r.vertex_edge_keys = TriMesh3d(verts, tris), keys
+        r.cube_size, r.index_min, r.index_max = float(cs.value), np.array(lo[:], np.int64), np.array(hi[:], np.int64)
+        r.paths, r.batches = paths, int(nb.value)
+        return r
 
 
 class RayHits:

@@ -15,6 +15,7 @@
 #include "ss_sdf.cuh"
 #include "ss_density.cuh"
 #include "ss_mc.cuh"
+#include "ss_levelset_mesh.cuh"
 
 #ifndef SS_HOST_EMUL               // (tests/emul/cuda_emul.h compiles this file with g++ to step the kernels on the CPU)
 #include <cub/cub.cuh>
@@ -198,6 +199,11 @@ struct ss_surface {
     SsDev fld_D{};
     uint32_t fld_nsub = 0;
     uint64_t fld_paths[3] = {};                              // groups of the last query per tier: 512, 4096, select
+    // mesh of a level-set field (ss_levelset_field_mesh_f32): lattice spacing, index range, batches
+    int lm = 0;
+    float lm_cube = 0.0f;
+    int64_t lm_imin[3] = {}, lm_imax[3] = {};
+    uint64_t lm_batches = 0;
 };
 
 // ------------------------------------------------------------------ host grid math (exact f32) ----
@@ -2609,6 +2615,188 @@ extern "C" void ss_sdf_free(ss_sdf *s) {
     if (!s) return;
     cudaSetDevice(s->device);
     delete s;
+}
+
+// ------------------------------------------------------------------ the field's surface as a mesh ----
+// DESIGN.md §16.  Tiles of 64^3 lattice cells in batches; per batch: listing, the cascade of k_lm_fold / k_lm_select into zero-filled
+// tiles, marching cubes; the weld by global edge key at the end.  The result owns its mesh; the field's records are only read.
+static uint32_t g_lm_batch_tiles = 0;          // 0: as many tiles per batch as fit a third of the free device memory
+extern "C" void ss_levelset_mesh_set_batch_tiles(uint32_t tiles) { g_lm_batch_tiles = tiles; }
+
+// The listed bricks of a batch through the tiers of run_cascade: 512-slot slice, 4096-slot slice, selection walk.  A brick goes on with
+// all its groups; each tier folds only the groups with more candidates than the previous tier's slice (paths: bricks per tier).
+template <class F>
+static void lm_fold(ss_context *c, const SsDev &D, const SsLmFoldArgs &L0, const uint32_t *list, uint32_t n, uint64_t *paths) {
+    uint64_t launches = 0;
+    const auto args = [&](const uint32_t *l, uint32_t m, uint32_t *left, uint32_t done) {
+        SsLmFoldArgs L = L0;
+        L.bricks = l; L.n_bricks = m; L.fallback = left; L.done = done;
+        return L;
+    };
+    run_cascade(c, list, n, {
+        [&](const uint32_t *l, uint32_t m, uint32_t *left) {
+            LAUNCH(c, (k_lm_fold<F, SS_AN_CAP, SS_LM_WARPS>), (m + SS_LM_WARPS - 1) / SS_LM_WARPS, SS_LM_WARPS * 32, D, args(l, m, left, 0));
+        },
+        [&](const uint32_t *l, uint32_t m, uint32_t *left) { LAUNCH(c, (k_lm_fold<F, SS_AN_BIG_CAP, 1>), m, 32, D, args(l, m, left, SS_AN_CAP)); },
+        [&](const uint32_t *l, uint32_t m, uint32_t *left) { LAUNCH(c, k_lm_select<F>, m, 32, D, args(l, m, left, SS_AN_BIG_CAP)); },
+    }, launches, paths);
+}
+
+extern "C" int ss_levelset_field_mesh_f32(ss_surface *f, const float *aabb_min, const float *aabb_max, float cube_size, ss_surface **out) {
+    if (!out) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument");
+    *out = nullptr;
+    int rc; ss_context *c = field_context(f, &rc);
+    if (!c) return rc;
+    if ((aabb_min == nullptr) != (aabb_max == nullptr)) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set mesh: give both aabb_min and aabb_max, or neither");
+    if (!std::isfinite(cube_size)) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set mesh: the cube size has to be finite");
+    if (aabb_min) {
+        for (int d = 0; d < 3; ++d) {
+            if (!std::isfinite(aabb_min[d]) || !std::isfinite(aabb_max[d])) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set mesh: the box has to be finite");
+            if (!(aabb_min[d] <= aabb_max[d])) return ss_fail(SS_ERR_INVALID_PARAMETER, "level-set mesh: aabb_min has to be <= aabb_max");
+        }
+    }
+    const SsDev &D = f->fld_D;
+    if (!(D.thr >= 0.0f))
+        return ss_fail(SS_ERR_UNSUPPORTED, "level-set mesh: a negative threshold would put the points no particle reaches inside (DESIGN.md 16)");
+    const float cell = f->grid.cell, cs = cube_size > 0.0f ? cube_size : cell;
+    // the index range per axis, float64 arithmetic on the f32 values
+    int64_t lo[3], hi[3];
+    bool empty = false;
+    for (int d = 0; d < 3; ++d) {
+        const double top = cs == cell ? (double)f->grid.nc[d] : std::ceil((double)f->grid.nc[d] * (double)cell / (double)cs);
+        double l = 0.0, h = top;
+        if (aabb_min) {
+            l = std::max(l, std::floor(((double)aabb_min[d] - (double)f->grid.mn[d]) / (double)cs));
+            h = std::min(h, std::ceil(((double)aabb_max[d] - (double)f->grid.mn[d]) / (double)cs));
+        }
+        if (l > h) { empty = true; lo[d] = hi[d] = 0; continue; }
+        if (h > (double)((1 << 20) - 1)) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "level-set mesh: lattice index above 2^20 - 1 (the marching-cubes edge key)");
+        lo[d] = (int64_t)l; hi[d] = (int64_t)h;
+    }
+    for (uint64_t &q : f->fld_paths) q = 0;
+    return with_new_surface(c, out, [&](ss_surface *s) -> int {
+        cudaStream_t st = c->stream;
+        s->owner = c; s->frame = f->frame; s->S = 64; s->lm = 1; s->lm_cube = cs;
+        s->grid = f->grid; s->grid.cell = cs;
+        for (int d = 0; d < 3; ++d) { s->lm_imin[d] = lo[d]; s->lm_imax[d] = hi[d]; }
+        const uint32_t nsub = f->fld_ready ? f->fld_nsub : 0u;
+        SsLmGrid G{};
+        uint64_t ntt = 1;
+        for (int d = 0; d < 3; ++d) {
+            G.gmin[d] = f->grid.mn[d]; G.imin[d] = (int)lo[d]; G.npts[d] = (int)(hi[d] - lo[d] + 1);
+            G.ntile[d] = (int)((hi[d] - lo[d] + 63) / 64);
+            ntt *= (uint64_t)G.ntile[d];
+        }
+        if (empty || !nsub || !ntt) return SS_OK;                       // no cell, or no record: the empty mesh
+        if (ntt >= 0x7fffffffull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "level-set mesh: 2^31 or more tiles in the range");
+        G.c = cs; G.Sb = cs == cell ? D.S : 0; G.sub_size = G.Sb ? fmulr(cs, (float)G.Sb) : 0.0f;
+        G.gmax = make_float3(f->grid.mx[0], f->grid.mx[1], f->grid.mx[2]);
+        G.sub_flat = c->sub_flat.as<uint32_t>(); G.nsub = nsub;
+        // groups with records, tiles that can hold a nonzero point
+        const uint32_t nb3 = (uint32_t)(D.nb * D.nb * D.nb), ngroups = nsub * nb3, ntt32 = (uint32_t)ntt;
+        SsBins bins = context_bins(c); bins.brick_rng = c->fld_rng.as<int2>();
+        DevBuf grp, tflag, toff, tchunk, tlist, fflag, foff, flist, mflag, moff, mlist, tiles, voff, vmask, vcnt, tcnt, vblk_off, tblk_off;
+        grp.ensure(ngroups);
+        LAUNCH(c, k_lm_groups, nblk(ngroups, 256), 256, D, bins, ngroups, grp.as<uint8_t>());
+        G.grp = grp.as<uint8_t>();
+        // in chunks of SS_LM_TILE_CHUNK tiles: 12 bytes per tile of the chunk, then 4 per tile that can hold a nonzero point
+        const uint32_t chunk = std::min<uint32_t>(ntt32, SS_LM_TILE_CHUNK);
+        tflag.ensure((size_t)chunk * 4); toff.ensure((size_t)chunk * 4 + 4); tchunk.ensure((size_t)chunk * 4);
+        uint32_t ntl = 0;
+        for (uint32_t t0 = 0; t0 < ntt32; t0 += chunk) {
+            const uint32_t nc = std::min<uint32_t>(chunk, ntt32 - t0);
+            LAUNCH(c, k_lm_tiles, nblk(nc, 128), 128, D, G, t0, nc, tflag.as<uint32_t>());
+            uint32_t lt[2] = { 0, 0 };
+            scan_compact(c, tflag.as<uint32_t>(), toff.as<uint32_t>(), nc, tchunk.as<uint32_t>(), lt);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t k = lt[0] + lt[1];
+            if (!k) continue;
+            tlist.grow_keep(((size_t)ntl + k) * 4, (size_t)ntl * 4, st);
+            LAUNCH(c, k_lm_offset, nblk(k, 256), 256, tchunk.as<uint32_t>(), k, t0, tlist.as<uint32_t>() + ntl);
+            ntl += k;
+        }
+        if (!ntl) return SS_OK;
+        // batch size: a third of the free memory (values, vertex offsets and masks per point, six lists per brick)
+        const size_t np3 = 65ull * 65 * 65, per_tile = np3 * 9 + 729ull * 40 + 256;
+        size_t free_b = 0, total_b = 0;
+        CK(cudaMemGetInfo(&free_b, &total_b));
+        size_t max_tiles = std::max<size_t>(1, free_b / 3 / per_tile);
+        if (g_lm_batch_tiles) max_tiles = std::min<size_t>(max_tiles, g_lm_batch_tiles);
+        max_tiles = std::min<size_t>(max_tiles, ntl);
+        const size_t nbr_max = max_tiles * 729;
+        tiles.ensure(max_tiles * np3 * 4); voff.ensure(max_tiles * np3 * 4); vmask.ensure(max_tiles * np3);
+        for (DevBuf *b : { &fflag, &foff, &flist, &mflag, &moff, &mlist, &vcnt, &tcnt, &vblk_off, &tblk_off }) b->ensure(nbr_max * 4 + 4);
+        SsDev Pm = D;                                                   // the tile layout of marching cubes
+        Pm.S = 64; Pm.np = 65; Pm.nb = SS_LM_NB; Pm.np_magic = (uint32_t)(4294967296ull / 65ull) + 1u;
+        SsLmFoldArgs L{};
+        L.A.bins = bins; L.A.grec = c->an_grec.as<float4>(); L.A.rrec = c->av_rrec.as<float>();
+        L.tiles = tiles.as<float>();
+        s->verts.ensure(1 << 16); s->vkeys.ensure(1 << 16); s->tris.ensure(1 << 16);
+        c->bkeys_a.ensure(1 << 16); c->bids_a.ensure(1 << 16); c->bcount.ensure(4);
+        CK(cudaMemsetAsync(c->bcount.p, 0, 4, st));
+        uint64_t vtotal = 0, ttotal = 0;
+        for (uint32_t t0 = 0; t0 < ntl; t0 += (uint32_t)max_tiles) {
+            const uint32_t nbatch = std::min<uint32_t>((uint32_t)max_tiles, ntl - t0), nbr = nbatch * 729u;
+            G.tiles = tlist.as<uint32_t>() + t0; L.G = G;
+            CK(cudaMemsetAsync(tiles.p, 0, (size_t)nbatch * np3 * 4, st));
+            LAUNCH(c, k_lm_list, nblk(nbr, 128), 128, D, G, nbr, fflag.as<uint32_t>());
+            LAUNCH(c, k_lm_mc_flags, nblk(nbr, 256), 256, fflag.as<uint32_t>(), nbr, mflag.as<uint32_t>());
+            uint32_t lf[2] = { 0, 0 }, lm[2] = { 0, 0 };
+            scan_compact(c, fflag.as<uint32_t>(), foff.as<uint32_t>(), nbr, flist.as<uint32_t>(), lf);
+            scan_compact(c, mflag.as<uint32_t>(), moff.as<uint32_t>(), nbr, mlist.as<uint32_t>(), lm);
+            CK(cudaStreamSynchronize(st));
+            const uint32_t nf = lf[0] + lf[1], n_mc = lm[0] + lm[1];
+            ++s->lm_batches;
+            switch (f->fld_mode) {
+            case SS_FLD_ANISO: lm_fold<SsAnisoFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            case SS_FLD_AVG: lm_fold<SsAvgFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            case SS_FLD_AVG_CORR: lm_fold<SsAvgCorrFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            case SS_FLD_AVG_RAD: lm_fold<SsAvgRadFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            case SS_FLD_AVG_CORR_RAD: lm_fold<SsAvgCorrRadFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            default: lm_fold<SsSphFold>(c, D, L, flist.as<uint32_t>(), nf, f->fld_paths); break;
+            }
+            if (!n_mc) continue;
+            // marching cubes of the batch, appended to the result (as marching_cubes_batch)
+            LAUNCH(c, k_lm_mc_count, (n_mc + SS_MW_WARPS - 1) / SS_MW_WARPS, SS_MW_WARPS * 32, Pm, G, tiles.as<float>(), mlist.as<uint32_t>(), n_mc,
+                   vmask.as<uint8_t>(), voff.as<uint32_t>(), vcnt.as<uint32_t>(), tcnt.as<uint32_t>());
+            uint32_t lv[2] = { 0, 0 }, ltr[2] = { 0, 0 }, bc = 0;
+            scan_with_total(c, vcnt.as<uint32_t>(), vblk_off.as<uint32_t>(), n_mc, lv);
+            scan_with_total(c, tcnt.as<uint32_t>(), tblk_off.as<uint32_t>(), n_mc, ltr);
+            CK(cudaMemcpyAsync(&bc, c->bcount.p, 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            const uint64_t bv = (uint64_t)lv[0] + lv[1], bt = (uint64_t)ltr[0] + ltr[1];
+            if (vtotal + bv >= 0xfffffff0ull || ttotal + bt >= 0xfffffff0ull) return ss_fail(SS_ERR_INDEX_TOO_SMALL, "mesh too large for 32-bit vertex / triangle ids");
+            if (!bv && !bt) continue;
+            s->verts.grow_keep((vtotal + bv) * 12, vtotal * 12, st);
+            s->vkeys.grow_keep((vtotal + bv) * 8, vtotal * 8, st);
+            s->tris.grow_keep((ttotal + bt) * 12, ttotal * 12, st);
+            c->bkeys_a.grow_keep(((size_t)bc + bv) * 8, (size_t)bc * 8, st);
+            c->bids_a.grow_keep(((size_t)bc + bv) * 4, (size_t)bc * 4, st);
+            SsMcOut O{};
+            O.verts = s->verts.as<float>(); O.tris = s->tris.as<uint32_t>(); O.vkeys = s->vkeys.as<unsigned long long>();
+            O.bkeys = c->bkeys_a.as<unsigned long long>(); O.bids = c->bids_a.as<uint32_t>(); O.bcount = c->bcount.as<uint32_t>();
+            O.vbase = (uint32_t)vtotal; O.tbase = (uint32_t)ttotal; O.bcap = (uint32_t)std::min<size_t>((size_t)bc + bv, 0xffffffffu);
+            LAUNCH(c, k_lm_mc_emit, (n_mc + SS_MW_WARPS - 1) / SS_MW_WARPS, SS_MW_WARPS * 32, Pm, G, tiles.as<float>(), mlist.as<uint32_t>(), n_mc,
+                   vmask.as<uint8_t>(), voff.as<uint32_t>(), vcnt.as<uint32_t>(), tcnt.as<uint32_t>(), vblk_off.as<uint32_t>(), tblk_off.as<uint32_t>(),
+                   mflag.as<uint32_t>(), moff.as<uint32_t>(), O);
+            vtotal += bv; ttotal += bt;
+        }
+        uint64_t nv_final = vtotal;
+        uint32_t bc = 0;
+        rc = weld_boundary_vertices(c, s, vtotal, ttotal, nv_final, bc);
+        if (rc) return rc;
+        s->nv = nv_final; s->nt = ttotal;
+        CK(cudaStreamSynchronize(st));
+        return SS_OK;
+    });
+}
+
+extern "C" int ss_levelset_mesh_info(const ss_surface *m, float *cube_size, int64_t index_min[3], int64_t index_max[3], uint64_t *batches) {
+    if (!m || !m->lm) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL argument or not a level-set mesh (ss_levelset_field_mesh_f32)");
+    if (cube_size) *cube_size = m->lm_cube;
+    for (int d = 0; d < 3; ++d) { if (index_min) index_min[d] = m->lm_imin[d]; if (index_max) index_max[d] = m->lm_imax[d]; }
+    if (batches) *batches = m->lm_batches;
+    return SS_OK;
 }
 
 #include "ss_post.cuh"
