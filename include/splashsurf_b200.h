@@ -287,6 +287,13 @@ int ss_context_set_density_variant(ss_context *ctx, int variant);
  * 0 = one CTA per brick, three marching-cubes launches.  Replaces dense_subdomains.rs:1470-1568. */
 int ss_context_set_mc_variant(ss_context *ctx, int variant);
 int ss_context_set_count_pairs(ss_context *ctx, int on);
+/* Phase timing of the exact level-set pass (profiling; same results, slower): with `on` the subdomain path without count_pairs
+ * runs an instrumented k_exact_warp that sums clock64() cycles per phase over its warps, from zero at this call.
+ * ss_context_exact_phases copies SS_EXACT_PHASES + 1 counters: the cycles of lookup, copy wait, key staging, sort, list
+ * compaction, fold and stores, then the number of bricks timed. */
+#define SS_EXACT_PHASES 7
+int ss_context_set_exact_phases(ss_context *ctx, int on);
+int ss_context_exact_phases(ss_context *ctx, uint64_t *out);
 
 /* ---- SPH normals at the mesh vertices: SphInterpolator::interpolate_normals (sph_interpolation.rs:82-133) as used by the
  * pipeline's `--sph-normals` (splashsurf/src/reconstruct.rs:1126-1129, :1287-1294): particle volume = (4/3 pi r^3 rho0) /

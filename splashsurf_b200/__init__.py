@@ -160,6 +160,8 @@ def _bind(L):
     L.ss_context_set_mc_variant.argtypes = [vp, C.c_int]
     L.ss_context_set_copy_chunk_bytes.argtypes = [vp, u64]
     L.ss_context_set_count_pairs.argtypes = [vp, C.c_int]
+    L.ss_context_set_exact_phases.argtypes = [vp, C.c_int]
+    L.ss_context_exact_phases.argtypes = [vp, vp]
     L.ss_context_set_compute_sph_normals.argtypes = [vp, C.c_int]
     L.ss_surface_copy_normals.argtypes = [vp, vp]
     L.ss_surface_device_normals.argtypes = [vp]
@@ -824,6 +826,20 @@ class Context:
 
     def set_count_pairs(self, on: bool):
         _check(self._L, self._L.ss_context_set_count_pairs(self._h, int(bool(on))))
+
+    EXACT_PHASES = ("lookup", "copy_wait", "key_staging", "sort", "list", "fold", "stores")
+
+    def set_exact_phases(self, on: bool):
+        """Time the phases of the exact level-set pass (subdomain path, profiling only; slower): counters start from zero."""
+        _check(self._L, self._L.ss_context_set_exact_phases(self._h, int(bool(on))))
+
+    def exact_phases(self) -> dict:
+        """clock64() cycles per phase of the exact pass summed over its warps since set_exact_phases(True), and the bricks timed."""
+        out = (C.c_uint64 * (len(self.EXACT_PHASES) + 1))()
+        _check(self._L, self._L.ss_context_exact_phases(self._h, out))
+        d = {k: int(out[i]) for i, k in enumerate(self.EXACT_PHASES)}
+        d["bricks"] = int(out[len(self.EXACT_PHASES)])
+        return d
 
     def reconstruct_raw(self, xyz_ptr: int, n: int, params: _Params):
         """Low-level call: pointer (host or device) to n x 3 f32 -> opaque surface handle."""

@@ -130,6 +130,7 @@ struct ss_context {
     int ls_exact_all = 0;           // 1: evaluate every grid point exactly (no certification)
     int ls_variant = 2;              // 2 (default): warp-per-brick certification + exact kernels (ss_certify.cuh, ss_exact.cuh); 1: CTA-per-brick certification kernel; 0: fused k_levelset
     int count_pairs = 0;             // 1: count in-support evaluations (work model; slower)
+    int exact_phases = 0;            // 1: time the phases of k_exact_warp into xphase (ss_context_set_exact_phases; slower)
     int density_variant = 0;         // 0 (default): thread-per-particle k_density; 1 / 2: cell-cooperative kernel (ss_density.cuh), candidates staged by bulk copies / 16-byte loads
     int mc_variant = 1;              // 1 (default): warp-per-brick marching cubes (count + emit) and fix-up sweep (ss_mc.cuh); 0: CTA-per-brick passes
     void *h_stage[2] = { nullptr, nullptr };   // page-locked staging buffers of the result copies (copy_out), allocated on first use
@@ -149,7 +150,7 @@ struct ss_context {
     // reusable scratch
     DevBuf xyz, xyz_f, filt_flag, filt_flag32, filt_off, aabb, cnt, off, key_a, key_b, val_a, val_b, cid, cub_tmp,
         sub_flat, sub_off, sub_owned, gkey_a, gkey_b, gval_a, gval_b, flags, scan, spos, rho, tab_a, tab_b, rec, ksplit, tiles, vcnt,
-        tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, an_det, an_grec;
+        tcnt, vmask, voff, vblk_off, tblk_off, tile_tab, brick_rng, bstate, flag_ls, off_ls, list_ls, flag_mc, flag_fix, off_mc, off_fix, list_mc, list_fix, wflag, wstate, desc_ls, dflag, doff, dlist, fallback, fallback2, fallback3, pack_cnt, pack_off, brick_seen, fix_list, nflag, bkeys_a, bkeys_b, bids_a, bids_b, bcount, remap, keep, newid, err, pairs, xphase, xw_taken, an_det, an_grec;
     DevBuf av_radii, av_delta, av_rrec, av_chk;      // per-particle radii: the caller's copy, delta_j (filtered), per membership, check
     // level-set field queries (ss_field.cuh): points, group keys and caller indices (sorted and not), group starts, values, checks,
     // and the candidate bin ranges of a group
@@ -391,6 +392,25 @@ extern "C" int ss_surface_copy_normals(const ss_surface *s, float *dst) {
 }
 extern "C" const float *ss_surface_device_normals(const ss_surface *s) { return (s && s->has_normals) ? s->normals.as<float>() : nullptr; }
 extern "C" int ss_context_set_count_pairs(ss_context *c, int on) { if (!c) return SS_ERR_INVALID_PARAMETER; c->count_pairs = on ? 1 : 0; return SS_OK; }
+static_assert(SS_XP_N == SS_EXACT_PHASES, "phases of the exact pass: kernel and header disagree");
+extern "C" int ss_context_set_exact_phases(ss_context *c, int on) {
+    if (!c) return SS_ERR_INVALID_PARAMETER;
+    c->exact_phases = on ? 1 : 0;
+    if (!on) return SS_OK;
+    return ss_guard([&] {
+        CK(cudaSetDevice(c->device));
+        c->xphase.ensure((SS_XP_N + 1) * 8);
+        CK(cudaMemset(c->xphase.p, 0, (SS_XP_N + 1) * 8));
+        return SS_OK;
+    });
+}
+extern "C" int ss_context_exact_phases(ss_context *c, uint64_t *out) {
+    if (!c || !out) return SS_ERR_INVALID_PARAMETER;
+    if (!c->xphase.p) return ss_fail(SS_ERR_INVALID_PARAMETER, "phase timing is off (ss_context_set_exact_phases)");
+    cudaSetDevice(c->device);
+    const cudaError_t e = cudaMemcpy(out, c->xphase.p, (SS_XP_N + 1) * 8, cudaMemcpyDeviceToHost);
+    return e == cudaSuccess ? SS_OK : ss_fail(SS_ERR_CUDA, cudaGetErrorString(e));
+}
 extern "C" int ss_context_set_anisotropy_f32(ss_context *c, const ss_anisotropy_f32 *a) {
     if (!c) return ss_fail(SS_ERR_INVALID_PARAMETER, "NULL context");
     if (!a) { c->an_on = 0; return SS_OK; }
@@ -858,15 +878,20 @@ static void launch_exact(ss_context *c, const SsDev &D, const SsLsArgs &F, uint3
     const auto args = [&](const uint32_t *list, uint32_t n, uint32_t *left) {
         SsXwArgs X{};
         X.bins = F.bins; X.bricks = list; X.n_bricks = n; X.wflag = F.wflag; X.tiles = F.tiles; X.fallback = left; X.pairs = F.pairs;
+        X.taken = c->xw_taken.as<uint32_t>();
+        X.phases = c->exact_phases ? c->xphase.as<unsigned long long>() : nullptr;
         return X;
     };
     // dense clusters: the same kernel with one warp per CTA and a larger slice -- up to 1024 candidates per brick (27 KB, static),
     // then up to 4096 (108 KB of dynamic shared memory); beyond that k_levelset's O(C^2) selection path (extreme clustering only)
     run_cascade(c, F.fix_bricks, n_bricks, {
         [&](const uint32_t *list, uint32_t n, uint32_t *left) {
-            with_global_count(global_mode, count, [&](auto G, auto C) {
-                LAUNCH(c, (k_exact_warp<G, C>), (n + SS_XW_WARPS - 1) / SS_XW_WARPS, SS_XW_THREADS, D, args(list, n, left));
-            });
+            // persistent warps: one wave of CTAs (15 warps per SM), fewer when the list is short; the counter hands out the rest
+            const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)c->sm_count * 5, (n + SS_XW_WARPS - 1) / SS_XW_WARPS);
+            c->xw_taken.ensure(4);
+            CK(cudaMemsetAsync(c->xw_taken.p, 0, 4, c->stream));
+            if (c->exact_phases && !global_mode && !count) LAUNCH(c, (k_exact_warp<false, false, true>), grid, SS_XW_THREADS, D, args(list, n, left));
+            else with_global_count(global_mode, count, [&](auto G, auto C) { LAUNCH(c, (k_exact_warp<G, C>), grid, SS_XW_THREADS, D, args(list, n, left)); });
         },
         [&](const uint32_t *list, uint32_t n, uint32_t *left) {
             with_global_count(global_mode, count, [&](auto G, auto C) { LAUNCH(c, (k_exact_warp_mid<G, C>), n, 32, D, args(list, n, left)); });

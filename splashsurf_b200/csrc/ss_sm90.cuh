@@ -63,4 +63,6 @@ static inline void ss_bulk_g2s(void *dst, const void *src, uint32_t bytes, unsig
 static inline void ss_mbar_wait(unsigned long long *bar, uint32_t) {
     if (*bar != 0) { fprintf(stderr, "emul: mbarrier wait with %lld bytes outstanding (expect_tx does not match the copies issued)\n", (long long)*bar); abort(); }
 }
+// the phase clocks of instrumented kernels count nanoseconds here
+static inline long long clock64() { return (long long)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 #endif
